@@ -12,15 +12,14 @@
 #include <string.h>
 #include <utility>
 
-namespace b200 {
-int launch_itx_grouped(bool hbd, const void *const *blocks, const int32_t *n, void *coefs, void *pic, const int32_t *st,
+namespace b200 {   // itx.cu
+int launch_itx_grouped(const void *const *blocks, const int32_t *n, void *coefs, void *pic, const int32_t *st,
                        int bdmax, int zero, cudaStream_t stream);
-int launch_itx(int tx, bool hbd, const B200ItxBlock *blocks, int n, void *coefs, void *pic,
-               const int32_t *st, int bdmax, int zero, cudaStream_t stream);
+int launch_itx(int tx, const B200ItxBlock *blocks, int n, void *coefs, void *pic, const int32_t *st, int bdmax, int zero,
+               cudaStream_t stream);
 }
 
 static thread_local char g_err[512];
-namespace b200 { std::mutex &host_lock() { static std::mutex m; return m; } }
 static std::atomic<uint64_t> g_launches{0};
 
 void b200_set_error(const char *fmt, ...) {
@@ -77,18 +76,20 @@ int b200_dev_memset(void *p, int value, size_t bytes, void *stream) {
 
 // ---------------------------------------------------------------------------------------
 namespace {
-using b200::Scratch;
-Scratch g_s_blocks, g_s_coef, g_s_pic;
-#define g_mu (b200::host_lock())
-
-const uint8_t k_tx_w[19] = { 4, 8, 16, 32, 64, 4, 8, 8, 16, 16, 32, 32, 64, 4, 16, 8, 32, 16, 64 };
-const uint8_t k_tx_h[19] = { 4, 8, 16, 32, 64, 8, 4, 16, 8, 32, 16, 64, 32, 16, 4, 32, 8, 64, 16 };
+// width and height of transform size tx (0 <= tx < 19)
+void tx_size(int tx, int *w, int *h) {
+#define X(TX, W, H, SH) if (tx == TX) { *w = W; *h = H; }
+    B200_ITX_SIZES(X)
+#undef X
+}
 
 // is (tx, txtp) a slot dav1d defines? (reference src/itx_tmpl.c:220-288)
 bool itx_defined(int tx, int txtp) {
     if (tx < 0 || tx >= 19 || txtp < 0 || txtp > 16) return false;
     if (txtp == 16) return tx == 0;
-    const int w = k_tx_w[tx], h = k_tx_h[tx], mx = w > h ? w : h, mn = w < h ? w : h;
+    int w, h;
+    tx_size(tx, &w, &h);
+    const int mx = w > h ? w : h, mn = w < h ? w : h;
     if (mx == 64) return txtp == 0;
     if (mx == 32) return txtp == 0 || txtp == 9;
     if (mx == 16 && mn == 16) return txtp <= 11;
@@ -96,6 +97,8 @@ bool itx_defined(int tx, int txtp) {
 }
 
 using b200::die;
+using b200::Level1;
+enum { BLOCKS, COEF, PIC };   // Level1 scratch slots
 }  // namespace
 
 extern "C" {
@@ -105,52 +108,32 @@ int b200_itx_add_batch(int bitdepth_max, int tx, const B200ItxBlock *d_blocks, i
                        void *stream)
 {
     if (tx < 0 || tx >= 19) { b200_set_error("b200_itx_add_batch: bad tx %d", tx); return -2; }
-    if (bitdepth_max != 255 && bitdepth_max != 1023 && bitdepth_max != 4095) {
-        b200_set_error("b200_itx_add_batch: bad bitdepth_max %d", bitdepth_max);
-        return -2;
-    }
+    if (int r = b200::check_bdmax(bitdepth_max, "b200_itx_add_batch")) return r;
     if (n_blocks <= 0) return 0;
-    if (b200::launch_itx(tx, bitdepth_max > 255, d_blocks, n_blocks, d_coef, d_pic, stride_px,
-                         bitdepth_max, zero_coefs, (cudaStream_t)stream))
-        { b200_set_error("b200_itx_add_batch: launch failed"); return -1; }
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return b200::launch_itx(tx, d_blocks, n_blocks, d_coef, d_pic, stride_px, bitdepth_max, zero_coefs, (cudaStream_t)stream);
 }
 
 int b200_itx_add_frame(int bitdepth_max, const void *const d_blocks[19], const int32_t n_blocks[19], void *d_coef,
                        void *d_pic, const int32_t stride_px[3], int zero_coefs, void *stream)
 {
-    if (bitdepth_max != 255 && bitdepth_max != 1023 && bitdepth_max != 4095) {
-        b200_set_error("b200_itx_add_frame: bad bitdepth_max %d", bitdepth_max);
-        return -2;
-    }
-    if (b200::launch_itx_grouped(bitdepth_max > 255, d_blocks, n_blocks, d_coef, d_pic, stride_px, bitdepth_max,
-                                 zero_coefs, (cudaStream_t)stream))
-        { b200_set_error("b200_itx_add_frame: launch failed"); return -1; }
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    if (int r = b200::check_bdmax(bitdepth_max, "b200_itx_add_frame")) return r;
+    return b200::launch_itx_grouped(d_blocks, n_blocks, d_coef, d_pic, stride_px, bitdepth_max, zero_coefs, (cudaStream_t)stream);
 }
 
 int b200_itx_add_batch_host(int bitdepth_max, int tx, const B200ItxBlock *blocks, int n_blocks,
                             void *coef, size_t coef_bytes, void *pic, size_t pic_bytes,
                             const int32_t stride_px[3], int zero_coefs)
 {
-    std::lock_guard<std::mutex> lk(g_mu);
+    Level1 L;
     if (n_blocks <= 0) return 0;
-    const size_t bb = (size_t)n_blocks * sizeof(B200ItxBlock);
-    if (g_s_blocks.reserve(bb) || g_s_coef.reserve(coef_bytes) || g_s_pic.reserve(pic_bytes)) return -1;
-    cudaStream_t st = 0;
-    B200_CUDA_OK(cudaMemcpyAsync(g_s_blocks.p, blocks, bb, cudaMemcpyHostToDevice, st));
-    B200_CUDA_OK(cudaMemcpyAsync(g_s_coef.p, coef, coef_bytes, cudaMemcpyHostToDevice, st));
-    B200_CUDA_OK(cudaMemcpyAsync(g_s_pic.p, pic, pic_bytes, cudaMemcpyHostToDevice, st));
-    int r = b200_itx_add_batch(bitdepth_max, tx, (const B200ItxBlock *)g_s_blocks.p, n_blocks,
-                               g_s_coef.p, g_s_pic.p, stride_px, zero_coefs, st);
-    if (r) return r;
-    B200_CUDA_OK(cudaMemcpyAsync(pic, g_s_pic.p, pic_bytes, cudaMemcpyDeviceToHost, st));
-    if (zero_coefs)
-        B200_CUDA_OK(cudaMemcpyAsync(coef, g_s_coef.p, coef_bytes, cudaMemcpyDeviceToHost, st));
-    B200_CUDA_OK(cudaStreamSynchronize(st));
-    return 0;
+    void *d_blocks, *d_coef, *d_pic;
+    if (!(d_blocks = L.upload(BLOCKS, blocks, (size_t)n_blocks * sizeof(B200ItxBlock))) || !(d_coef = L.upload(COEF, coef, coef_bytes)) ||
+        !(d_pic = L.upload(PIC, pic, pic_bytes)))
+        return -1;
+    if (int r = b200_itx_add_batch(bitdepth_max, tx, (const B200ItxBlock *)d_blocks, n_blocks, d_coef, d_pic, stride_px, zero_coefs, 0))
+        return r;
+    if (L.download(PIC, pic, pic_bytes) || (zero_coefs && L.download(COEF, coef, coef_bytes))) return -1;
+    return L.sync();
 }
 
 // Level-1 single call, host pointers, arbitrary (possibly negative) byte stride.
@@ -159,23 +142,22 @@ int b200_inv_txfm_add(void *dst, ptrdiff_t dst_stride, void *coeff, int eob, int
 {
     if (!itx_defined(tx, txtp)) { b200_set_error("b200_inv_txfm_add: undefined (tx=%d, txtp=%d)", tx, txtp); return -2; }
     if (eob < 0) { b200_set_error("b200_inv_txfm_add: eob < 0"); return -2; }
+    Level1 L;
     const bool hbd = bitdepth_max > 255;
-    const int w = k_tx_w[tx], h = k_tx_h[tx];
+    int w, h;
+    tx_size(tx, &w, &h);
     const int sw = w < 32 ? w : 32, sh = h < 32 ? h : 32;
-    const size_t px = hbd ? 2 : 1, cs = hbd ? 4 : 2;
-    // pack the w x h destination rectangle densely (handles negative strides)
-    uint8_t rect[64 * 64 * 2];
-    for (int y = 0; y < h; y++)
-        memcpy(rect + (size_t)y * w * px, (const uint8_t *)dst + (ptrdiff_t)y * dst_stride, (size_t)w * px);
+    const size_t px = hbd ? 2 : 1, coef_bytes = (size_t)sw * sh * (hbd ? 4 : 2);
     B200ItxBlock b;
     b.dst_off = 0; b.coef_off = 0; b.eob = (int16_t)eob; b.txtp = (uint8_t)txtp; b.plane = 0;
     const int32_t st[3] = { w, w, w };
-    int r = b200_itx_add_batch_host(bitdepth_max, tx, &b, 1, coeff, (size_t)sw * sh * cs, rect,
-                                    (size_t)w * h * px, st, 1);
-    if (r) return r;
-    for (int y = 0; y < h; y++)
-        memcpy((uint8_t *)dst + (ptrdiff_t)y * dst_stride, rect + (size_t)y * w * px, (size_t)w * px);
-    return 0;
+    void *d_blocks, *d_coef, *d_pic;
+    if (!(d_blocks = L.upload(BLOCKS, &b, sizeof(b))) || !(d_coef = L.upload(COEF, coeff, coef_bytes)) ||
+        !(d_pic = L.upload_rect(PIC, dst, dst_stride, w, h, px)))
+        return -1;
+    if (int r = b200_itx_add_batch(bitdepth_max, tx, (const B200ItxBlock *)d_blocks, 1, d_coef, d_pic, st, 1, 0)) return r;
+    if (L.download(COEF, coeff, coef_bytes)) return -1;
+    return L.download_rect(PIC, dst, dst_stride, w, h, px);
 }
 
 }  // extern "C"

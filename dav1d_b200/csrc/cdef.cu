@@ -411,27 +411,18 @@ __global__ void cdef_dir_kernel(const typename Bd<HBD>::pixel *img, int *out, in
 
 using namespace b200;
 
-static int cdef_check_bd(int bdmax, const char *who) {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("%s: bad bitdepth_max %d", who, bdmax); return -2; }
-    return 0;
-}
-
 namespace b200 {
 // tile rows [t0, t1) of the sweep: a tile row is 32 luma rows (16 subsampled chroma rows) and reads 2 rows beyond each side
 int cdef_frame_rows(int bdmax, const B200CdefFrame *f, int t0, int t1, cudaStream_t stream)
 {
-    if (cdef_check_bd(bdmax, "b200_cdef_frame")) return -2;
+    if (int r = check_bdmax(bdmax, "b200_cdef_frame")) return r;
     const size_t px = bdmax > 255 ? 2 : 1;
     for (int pl = 0; pl < 3; pl++)   // the tile loader reads 4 samples at a time
         if ((f->stride[pl] & 3) || (f->plane_off[pl] & 3) || ((uintptr_t)f->src * 1 % (4 * px))) { b200_set_error("b200_cdef_frame: planes must be 4-sample aligned"); return -2; }
     t0 = imax(t0, 0); t1 = imin(t1, (f->bh + 7) / 8);
     if (t1 <= t0) return 0;
-    dim3 grid((f->bw + 15) / 16, t1 - t0);
-    if (bdmax > 255) { auto k = cdef_frame_kernel<true>; B200_LAUNCH_PDL(k, grid, dim3(kCdefThreads), 0, stream, *f, bdmax, t0); }
-    else { auto k = cdef_frame_kernel<false>; B200_LAUNCH_PDL(k, grid, dim3(kCdefThreads), 0, stream, *f, bdmax, t0); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return launch_hbd(bdmax, Launch::pdl, dim3((f->bw + 15) / 16, t1 - t0), dim3(kCdefThreads), 0, stream,
+                      [&](auto hbd) { return std::make_tuple(cdef_frame_kernel<hbd>, *f, bdmax, t0); });
 }
 }  // namespace b200
 
@@ -444,19 +435,17 @@ int b200_cdef_frame(int bdmax, const B200CdefFrame *f, void *stream)
 
 int b200_cdef_dir(const void *img, ptrdiff_t stride, unsigned *var, int bdmax)
 {
-    if (cdef_check_bd(bdmax, "b200_cdef_dir")) return -2;
-    std::lock_guard<std::mutex> lk(host_lock());
-    static Scratch s_in, s_out;
+    if (int r = check_bdmax(bdmax, "b200_cdef_dir")) return r;
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
-    uint8_t blk[64 * 2];
-    pack_rect(blk, img, stride, 8, 8, px);
-    if (s_in.upload(blk, 64 * px) || s_out.reserve(8)) return -1;
-    if (bdmax > 255) { auto k = cdef_dir_kernel<true>; B200_LAUNCH(k, dim3(1), dim3(32), 0, (cudaStream_t)0, (const uint16_t *)s_in.p, (int *)s_out.p, bdmax); }
-    else { auto k = cdef_dir_kernel<false>; B200_LAUNCH(k, dim3(1), dim3(32), 0, (cudaStream_t)0, (const uint8_t *)s_in.p, (int *)s_out.p, bdmax); }
-    b200_count_launch();
+    void *in, *out;
+    if (!(in = L.upload_rect(0, img, stride, 8, 8, px)) || !(out = L.dev(1, 8))) return -1;
+    if (int r = launch_hbd(bdmax, Launch::plain, dim3(1), dim3(32), 0, 0, [&](auto hbd) {
+            return std::make_tuple(cdef_dir_kernel<hbd>, (const typename Bd<hbd>::pixel *)in, (int *)out, bdmax);
+        }))
+        return r;
     int res[2];
-    if (s_out.download(res, 8)) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
+    if (L.download_rect(1, res, 0, 1, 1, sizeof(res))) return -1;
     *var = (unsigned)res[1];
     return res[0];   // 0..7
 }
@@ -464,10 +453,9 @@ int b200_cdef_dir(const void *img, ptrdiff_t stride, unsigned *var, int bdmax)
 int b200_cdef_fb(void *dst, ptrdiff_t stride, const void *left, const void *top, const void *bottom, int pri,
                  int sec, int dir, int damping, int w, int h, int edges, int bdmax)
 {
-    if (cdef_check_bd(bdmax, "b200_cdef_fb")) return -2;
+    if (int r = check_bdmax(bdmax, "b200_cdef_fb")) return r;
     if (!((w == 4 || w == 8) && (h == 4 || h == 8)) || dir < 0 || dir > 7 || (!pri && !sec)) { b200_set_error("b200_cdef_fb: bad arguments"); return -2; }
-    std::lock_guard<std::mutex> lk(host_lock());
-    static Scratch s_in, s_out;
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
     const int ww = w + 4;
     uint8_t win[12 * 12 * 2];
@@ -484,15 +472,14 @@ int b200_cdef_fb(void *dst, ptrdiff_t stride, const void *left, const void *top,
     if (edges & B200_CDEF_HAVE_BOTTOM)
         for (int y = 0; y < 2; y++) for (int x = xs; x < xe; x++)
             put(2 + x, 2 + h + y, (const uint8_t *)bottom + (ptrdiff_t)y * stride + (ptrdiff_t)x * (ptrdiff_t)px);
-    if (s_in.upload(win, (size_t)ww * (h + 4) * px) || s_out.reserve(64 * 2)) return -1;
-    if (bdmax > 255) { auto k = cdef_fb_kernel<true>; B200_LAUNCH(k, dim3(1), dim3(64), 0, (cudaStream_t)0, (const uint16_t *)s_in.p, (uint16_t *)s_out.p, w, h, pri, sec, dir, damping, edges, bdmax); }
-    else { auto k = cdef_fb_kernel<false>; B200_LAUNCH(k, dim3(1), dim3(64), 0, (cudaStream_t)0, (const uint8_t *)s_in.p, (uint8_t *)s_out.p, w, h, pri, sec, dir, damping, edges, bdmax); }
-    b200_count_launch();
-    uint8_t out[64 * 2];
-    if (s_out.download(out, (size_t)w * h * px)) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
-    unpack_rect(dst, stride, out, w, h, px);
-    return 0;
+    void *in, *out;
+    if (!(in = L.upload(0, win, (size_t)ww * (h + 4) * px)) || !(out = L.dev(1, 64 * 2))) return -1;
+    if (int r = launch_hbd(bdmax, Launch::plain, dim3(1), dim3(64), 0, 0, [&](auto hbd) {
+            typedef typename Bd<hbd>::pixel pixel;
+            return std::make_tuple(cdef_fb_kernel<hbd>, (const pixel *)in, (pixel *)out, w, h, pri, sec, dir, damping, edges, bdmax);
+        }))
+        return r;
+    return L.download_rect(1, dst, stride, w, h, px);
 }
 
 }  // extern "C"

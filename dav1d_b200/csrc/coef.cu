@@ -31,15 +31,12 @@ extern "C" {
 int b200_coef_expand(int bitdepth_max, const B200CoefBlock *d_blocks, int n_blocks, const void *d_compact, void *d_dense,
                      void *stream)
 {
-    if (bitdepth_max != 255 && bitdepth_max != 1023 && bitdepth_max != 4095) { b200_set_error("b200_coef_expand: bad bitdepth_max"); return -2; }
+    if (int r = b200::check_bdmax(bitdepth_max, "b200_coef_expand")) return r;
     if (n_blocks <= 0) return 0;
-    using namespace b200;
-    const dim3 grid((n_blocks + 3) / 4);
-    if (bitdepth_max > 255) { auto k = coef_expand_kernel<int32_t>; B200_LAUNCH_PDL(k, grid, dim3(128), 0, (cudaStream_t)stream, d_blocks, n_blocks, (const int32_t *)d_compact, (int32_t *)d_dense); }
-    else { auto k = coef_expand_kernel<int16_t>; B200_LAUNCH_PDL(k, grid, dim3(128), 0, (cudaStream_t)stream, d_blocks, n_blocks, (const int16_t *)d_compact, (int16_t *)d_dense); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return b200::launch_hbd(bitdepth_max, b200::Launch::pdl, dim3((n_blocks + 3) / 4), dim3(128), 0, (cudaStream_t)stream, [&](auto hbd) {
+        typedef typename b200::Bd<hbd>::coef coef;
+        return std::make_tuple(b200::coef_expand_kernel<coef>, d_blocks, n_blocks, (const coef *)d_compact, (coef *)d_dense);
+    });
 }
 
 }

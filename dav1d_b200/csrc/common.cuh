@@ -66,6 +66,12 @@ static const uint32_t c_recip16[64] = { 0, 65536, 32768, 21846, 16384, 13108, 10
 #endif
 B200_DEV unsigned recip16(int d) { return d < 64 ? (unsigned)c_recip16[d] : (d & (d - 1)) ? (65536u + d - 1) / d : 65536u >> (31 - __clz(d)); }
 
+// transform size tx -> (w, h, inter-pass shift), largest first: reference src/itx_tmpl.c:160-178
+#define B200_ITX_SIZES(X) \
+    X(4, 64, 64, 2) X(11, 32, 64, 1) X(12, 64, 32, 1) X(17, 16, 64, 2) X(18, 64, 16, 2) X(3, 32, 32, 2) X(9, 16, 32, 1) \
+    X(10, 32, 16, 1) X(15, 8, 32, 2) X(16, 32, 8, 2) X(2, 16, 16, 2) X(7, 8, 16, 1) X(8, 16, 8, 1) X(13, 4, 16, 1) \
+    X(14, 16, 4, 1) X(1, 8, 8, 1) X(5, 4, 8, 0) X(6, 8, 4, 0) X(0, 4, 4, 0)
+
 // pixel / coefficient types per bit-depth class (reference include/common/bitdepth.h:42-86)
 template <bool HBD> struct Bd;
 template <> struct Bd<false> { typedef uint8_t pixel; typedef int16_t coef; };

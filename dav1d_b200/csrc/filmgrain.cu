@@ -372,7 +372,7 @@ extern "C" {
 
 static int fg_check(int bdmax, const B200FgFrame *f, const char *who)
 {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("%s: bad bitdepth_max", who); return -2; }
+    if (int r = check_bdmax(bdmax, who)) return r;
     const int rows = (f->h + 31) / 32, nbx = (f->w + 31) / 32;
     if (nbx > kMaxBlocksX || (size_t)rows * kMaxBlocksX > sizeof(((FgScratch *)0)->offsets)) { b200_set_error("%s: picture too large", who); return -2; }
     return 0;
@@ -380,7 +380,7 @@ static int fg_check(int bdmax, const B200FgFrame *f, const char *who)
 
 int b200_fg_prep(int bdmax, const B200FgFrame *f, void *stream)
 {
-    if (fg_check(bdmax, f, "b200_fg_prep")) return -2;
+    if (int r = fg_check(bdmax, f, "b200_fg_prep")) return r;
     B200_LAUNCH(fg_prep_kernel, dim3(1), dim3(kFgPrepThreads), 0, (cudaStream_t)stream, *f, bdmax);
     b200_count_launch();
     B200_CUDA_OK(cudaGetLastError());
@@ -389,13 +389,9 @@ int b200_fg_prep(int bdmax, const B200FgFrame *f, void *stream)
 
 int b200_fg_apply(int bdmax, const B200FgFrame *f, void *stream)
 {
-    if (fg_check(bdmax, f, "b200_fg_apply")) return -2;
-    dim3 grid((f->w + 127) / 128, (f->h + 7) / 8, 3);
-    if (bdmax > 255) { auto k = fg_apply_kernel<true>; B200_LAUNCH_PDL(k, grid, dim3(32, 8), 0, (cudaStream_t)stream, *f, bdmax); }
-    else { auto k = fg_apply_kernel<false>; B200_LAUNCH_PDL(k, grid, dim3(32, 8), 0, (cudaStream_t)stream, *f, bdmax); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    if (int r = fg_check(bdmax, f, "b200_fg_apply")) return r;
+    return launch_hbd(bdmax, Launch::pdl, dim3((f->w + 127) / 128, (f->h + 7) / 8, 3), dim3(32, 8), 0, (cudaStream_t)stream,
+                      [&](auto hbd) { return std::make_tuple(fg_apply_kernel<hbd>, *f, bdmax); });
 }
 
 int b200_fg_apply_frame(int bdmax, const B200FgFrame *f, void *stream)
@@ -404,28 +400,34 @@ int b200_fg_apply_frame(int bdmax, const B200FgFrame *f, void *stream)
     return r ? r : b200_fg_apply(bdmax, f, stream);
 }
 
+// a grain LUT of 8-bit (int8) or high bit-depth (int16) entries, widened to the (GH + 1) x GW int16 the kernels read
+static void widen_lut(int16_t *dst, const void *lut, bool hbd)
+{
+    for (int i = 0; i < GH * GW; i++) dst[i] = hbd ? ((const int16_t *)lut)[i] : ((const int8_t *)lut)[i];
+    memset(dst + GH * GW, 0, GW * sizeof(int16_t));
+}
+
 int b200_fg_generate_grain(void *buf, const void *buf_y, const B200FilmGrainData *data, int uv, int ss_hor, int ss_ver, int bdmax)
 {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("b200_fg_generate_grain: bad bitdepth_max"); return -2; }
-    std::lock_guard<std::mutex> lk(host_lock());
-    static Scratch s_buf, s_y;
+    if (int r = check_bdmax(bdmax, "b200_fg_generate_grain")) return r;
+    Level1 L;
     const bool hbd = bdmax > 255;
-    const int n = (GH + 1) * GW;
-    static int16_t h16[2][(GH + 1) * GW];
-    if (s_buf.reserve(n * 2) || s_y.reserve(n * 2)) return -1;
-    if (uv >= 0) {
-        for (int i = 0; i < GH * GW; i++) h16[1][i] = hbd ? ((const int16_t *)buf_y)[i] : ((const int8_t *)buf_y)[i];
-        if (s_y.upload(h16[1], n * 2)) return -1;
-    }
+    const size_t n = (GH + 1) * GW;
+    int16_t *lut = (int16_t *)L.host(n * 2);
+    void *d_buf, *d_y;
+    if (!lut || !(d_buf = L.dev(0, n * 2))) return -1;
+    if (uv >= 0) widen_lut(lut, buf_y, hbd);
+    if (!(d_y = uv >= 0 ? L.upload(1, lut, n * 2) : L.dev(1, n * 2))) return -1;
     const int cw = uv >= 0 && ss_hor ? 44 : GW, ch = uv >= 0 && ss_ver ? 38 : GH;
-    B200_LAUNCH(fg_gen_l1_kernel, dim3(1), dim3(128), 0, (cudaStream_t)0, (int16_t *)s_buf.p, (const int16_t *)s_y.p, *data, uv, ss_hor, ss_ver, bdmax);
+    B200_LAUNCH(fg_gen_l1_kernel, dim3(1), dim3(128), 0, (cudaStream_t)0, (int16_t *)d_buf, (const int16_t *)d_y, *data, uv, ss_hor, ss_ver, bdmax);
     b200_count_launch();
-    if (s_buf.download(h16[0], n * 2)) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
+    B200_CUDA_OK(cudaGetLastError());
+    int16_t grain[(GH + 1) * GW];
+    if (L.download_rect(0, grain, 0, 1, 1, sizeof(grain))) return -1;
     for (int y = 0; y < ch; y++)
         for (int x = 0; x < cw; x++) {
-            if (hbd) ((int16_t *)buf)[y * GW + x] = h16[0][y * GW + x];
-            else ((int8_t *)buf)[y * GW + x] = (int8_t)h16[0][y * GW + x];
+            if (hbd) ((int16_t *)buf)[y * GW + x] = grain[y * GW + x];
+            else ((int8_t *)buf)[y * GW + x] = (int8_t)grain[y * GW + x];
         }
     return 0;
 }
@@ -434,40 +436,31 @@ static int fg_strip_l1(void *dst_row, const void *src_row, ptrdiff_t stride, con
                        const uint8_t *scaling, const void *grain_lut, int bh, int row_num, const void *luma_row,
                        ptrdiff_t luma_stride, int uv, int is_id, int sx, int sy, int bdmax)
 {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("fg strip: bad bitdepth_max"); return -2; }
+    if (int r = check_bdmax(bdmax, "fg strip")) return r;
     const int pw = (int)pw_;
     if (pw < 1 || pw > 16384 || bh < 1 || bh > 32) { b200_set_error("fg strip: bad geometry"); return -2; }
-    std::lock_guard<std::mutex> lk(host_lock());
-    static Scratch s_src, s_dst, s_luma, s_scal, s_lut;
-    const bool hbd = bdmax > 255;
-    const size_t px = hbd ? 2 : 1;
-    uint8_t *stage = (uint8_t *)malloc((size_t)pw * 32 * px * 2 + (size_t)(pw * 2 + 2) * 64 * px);
-    if (!stage) { b200_set_error("oom"); return -1; }
-    int rc = -1;
-    do {
-        pack_rect(stage, src_row, stride, pw, bh, px);
-        if (s_src.upload(stage, (size_t)pw * bh * px) || s_dst.reserve((size_t)pw * bh * px)) break;
-        int lw = 0;
-        if (uv >= 0) {
-            lw = (pw << sx) + (sx ? 0 : 0);
-            const int lh = ((bh - 1) << sy) + 1;
-            uint8_t *ls = stage + (size_t)pw * 32 * px * 2;
-            pack_rect(ls, luma_row, luma_stride, lw, lh, px);
-            if (s_luma.upload(ls, (size_t)lw * lh * px)) break;
-        }
-        static int16_t lut16[(GH + 1) * GW];
-        for (int i = 0; i < GH * GW; i++) lut16[i] = hbd ? ((const int16_t *)grain_lut)[i] : ((const int8_t *)grain_lut)[i];
-        if (s_lut.upload(lut16, sizeof(lut16)) || s_scal.upload(scaling, hbd ? 4096 : 256)) break;
-        if (hbd) { auto k = fg_strip_l1_kernel<true>; B200_LAUNCH(k, dim3(1), dim3(256), 0, (cudaStream_t)0, (uint16_t *)s_dst.p, (const uint16_t *)s_src.p, (const uint16_t *)s_luma.p, *data, pw, lw, (const uint8_t *)s_scal.p, (const int16_t *)s_lut.p, bh, row_num, uv, is_id, sx, sy, bdmax); }
-        else { auto k = fg_strip_l1_kernel<false>; B200_LAUNCH(k, dim3(1), dim3(256), 0, (cudaStream_t)0, (uint8_t *)s_dst.p, (const uint8_t *)s_src.p, (const uint8_t *)s_luma.p, *data, pw, lw, (const uint8_t *)s_scal.p, (const int16_t *)s_lut.p, bh, row_num, uv, is_id, sx, sy, bdmax); }
-        b200_count_launch();
-        if (s_dst.download(stage, (size_t)pw * bh * px)) break;
-        if (cudaStreamSynchronize(0) != cudaSuccess) { b200_set_error("sync failed"); break; }
-        unpack_rect(dst_row, stride, stage, pw, bh, px);
-        rc = 0;
-    } while (0);
-    free(stage);
-    return rc;
+    Level1 L;
+    const size_t px = bdmax > 255 ? 2 : 1;
+    enum { SRC, DST, LUMA, SCAL, LUT };
+    void *src, *dst, *luma = nullptr, *scal, *lut;
+    if (!(src = L.upload_rect(SRC, src_row, stride, pw, bh, px)) || !(dst = L.dev(DST, (size_t)pw * bh * px))) return -1;
+    int lw = 0;
+    if (uv >= 0) {
+        lw = pw << sx;
+        if (!(luma = L.upload_rect(LUMA, luma_row, luma_stride, lw, ((bh - 1) << sy) + 1, px))) return -1;
+    }
+    const size_t lut_bytes = (GH + 1) * GW * 2;
+    int16_t *lut16 = (int16_t *)L.host(lut_bytes);
+    if (!lut16) return -1;
+    widen_lut(lut16, grain_lut, bdmax > 255);
+    if (!(lut = L.upload(LUT, lut16, lut_bytes)) || !(scal = L.upload(SCAL, scaling, bdmax > 255 ? 4096 : 256))) return -1;
+    if (int r = launch_hbd(bdmax, Launch::plain, dim3(1), dim3(256), 0, 0, [&](auto hbd) {
+            typedef typename Bd<hbd>::pixel pixel;
+            return std::make_tuple(fg_strip_l1_kernel<hbd>, (pixel *)dst, (const pixel *)src, (const pixel *)luma, *data, pw, lw,
+                                   (const uint8_t *)scal, (const int16_t *)lut, bh, row_num, uv, is_id, sx, sy, bdmax);
+        }))
+        return r;
+    return L.download_rect(DST, dst_row, stride, pw, bh, px);
 }
 
 int b200_fgy_32x32xn(void *dst_row, const void *src_row, ptrdiff_t stride, const B200FilmGrainData *data, size_t pw,

@@ -4,142 +4,28 @@
 // reference src/thread_task.c:699-854) with whole-frame stages instead of superblock rows.
 #include "host_util.h"
 
-extern "C" {
-
-// the stages before intra reconstruction; *fg_side is set when the film grain preparation was forked to a side stream
-static int frame_phase_recon(const B200FrameJob *j, void *stream, void **fg_side)
-{
-    int r;
-    const int bd = j->bitdepth_max;
-    *fg_side = nullptr;
-#ifndef B200_EMU
-    // film grain LUT preparation: one CTA, latency bound, depends only on the frame header -> side stream. The
-    // scratch is reused frame after frame on this stream, hence the fork (after everything enqueued so far).
-    SideStream *fs = nullptr;
-    if (j->run_fg && (fs = side_stream_for((cudaStream_t)stream, 0)) && fs->fork((cudaStream_t)stream)) {
-        if ((r = b200_fg_prep(bd, &j->fg, fs->side))) return r;
-        *fg_side = fs;
-    }
-#endif
-    if (j->n_expand > 0) {
-        B200_CUDA_OK(cudaMemsetAsync(j->d_coef, 0, j->coef_bytes, (cudaStream_t)stream));
-        if ((r = b200_coef_expand(bd, j->d_expand, j->n_expand, j->d_ccoef, j->d_coef, stream))) return r;
-    }
-    if ((r = b200_mc_batch(bd, &j->mc, j->d_pred, j->n_pred, stream))) return r;
-    if ((r = b200_mc_scaled_batch(bd, &j->mc, j->d_scaled, j->n_scaled, stream))) return r;
-    if ((r = b200_mc_warp_batch(bd, &j->mc, j->d_warp, j->n_warp, stream))) return r;
-    if ((r = b200_mc_comp_fused_batch(bd, &j->mc, j->d_cfused, j->n_cfused, stream))) return r;
-    if ((r = b200_mc_comp_fused_batch(bd, &j->mc, j->d_cfused2, j->n_cfused2, stream))) return r;
-    if ((r = b200_mc_comp_batch(bd, &j->mc, j->d_comp, j->n_comp, stream))) return r;
-    if ((r = b200_mc_comp_batch(bd, &j->mc, j->d_comp2, j->n_comp2, stream))) return r;
-    if ((r = b200_mc_blend_batch(bd, &j->mc, j->d_blend, j->n_blend, stream))) return r;
-    if ((r = b200_mc_blend_batch(bd, &j->mc, j->d_blend2, j->n_blend2, stream))) return r;
-    if ((r = b200_itx_add_frame(bd, (const void *const *)j->d_itx, j->n_itx, j->d_coef, j->mc.dst, j->itx_stride,
-                                j->zero_coefs, stream)))
-        return r;
-    return 0;
-}
-
-static int frame_phase_post(const B200FrameJob *j, void *stream, void *fg_side)
-{
-    int r;
-    const int bd = j->bitdepth_max;
-    if (j->run_lf && (r = b200_lf_frame(bd, &j->lf, stream))) return r;
-    if (j->run_cdef && (r = b200_cdef_frame(bd, &j->cdef, stream))) return r;
-    if (j->run_resize) {                     // super-resolution: CDEF output (and the deblocked picture LR reads) upscaled
-        if ((r = b200_resize_frame(bd, &j->resize[0], stream))) return r;
-        if ((r = b200_resize_frame(bd, &j->resize[1], stream))) return r;
-    }
-    if (j->run_lr && (r = b200_lr_frame(bd, &j->lr, stream))) return r;
-    if (j->run_fg) {
-#ifndef B200_EMU
-        if (fg_side && !((SideStream *)fg_side)->join((cudaStream_t)stream)) { b200_set_error("b200_frame_run: stream join failed"); return -1; }
-#endif
-        if (!fg_side && (r = b200_fg_prep(bd, &j->fg, stream))) return r;
-        if ((r = b200_fg_apply(bd, &j->fg, stream))) return r;
-    }
-    return 0;
-}
-
-int b200_frame_run(const B200FrameJob *j, void *stream)
-{
-    int r;
-    void *fg_side;
-    if ((r = frame_phase_recon(j, stream, &fg_side))) return r;
-    if (j->n_intra > 0 && (r = b200_intra_frame(j->bitdepth_max, &j->intra, j->d_intra, j->n_intra, stream))) return r;
-    return frame_phase_post(j, stream, fg_side);
-}
-
-int b200_frame_run_batch(const B200FrameJob *const *jobs, int n, void *stream)
-{
-    if (n <= 0) return 0;
-    if (n > 256) { b200_set_error("b200_frame_run_batch: too many jobs"); return -2; }
-    int r;
-    void *fg_side[256];
-    B200IntraFrame frames[256];
-    const B200IntraTx *tx[256];
-    int32_t ntx[256];
-    for (int i = 0; i < n; i++) {
-        if (jobs[i]->bitdepth_max != jobs[0]->bitdepth_max) { b200_set_error("b200_frame_run_batch: mixed bit depths"); return -2; }
-        if (jobs[i]->run_fg) { b200_set_error("b200_frame_run_batch: film grain jobs must be run one by one"); return -2; }
-        if ((r = frame_phase_recon(jobs[i], stream, &fg_side[i]))) return r;
-        frames[i] = jobs[i]->intra; tx[i] = jobs[i]->d_intra; ntx[i] = jobs[i]->n_intra;
-    }
-    if ((r = b200_intra_frames(jobs[0]->bitdepth_max, frames, tx, ntx, n, stream))) return r;
-    for (int i = 0; i < n; i++)
-        if ((r = frame_phase_post(jobs[i], stream, fg_side[i]))) return r;
-    return 0;
-}
-
-// ---- band-sliced job (include/b200av1.h, B200FrameBand) --------------------------------------------------------
 static int job_luma_h(const B200FrameJob *j) { return j->lr.h > 0 ? j->lr.h : j->lf.h4 * 4; }
 
-int b200_band_progress(const B200FrameJob *j, int y1, int last, int plane)
+// the whole frame as one band: every record, every row
+static B200FrameBand whole_band(const B200FrameJob *j)
 {
-    const int ssv = plane ? j->lf.ss_ver : 0;
-    const int ph = (job_luma_h(j) + ssv) >> ssv;
-    if (last) return ph;
-    int p;
-    if (j->run_lr)        p = ssv ? (y1 >> 1) - 36 : (y1 <= 64 ? 0 : y1 - 40);   // the last tile row that could run (see b200_frame_run_band)
-    else if (j->run_cdef) p = (y1 - 32) >> ssv;
-    else if (j->run_lf)   p = ssv ? (y1 >> 1) - 4 : y1 - 8;        // a row edge at y1 still changes up to 6 (chroma: 2) rows above it
-    else                  p = y1 >> ssv;
-    return p < 0 ? 0 : (p > ph ? ph : p);
+    B200FrameBand b;
+    memset(&b, 0, sizeof(b));
+    b.y1 = job_luma_h(j); b.last = 1;
+    b.pred[1] = j->n_pred; b.warp[1] = j->n_warp; b.comp[1] = j->n_comp; b.comp2[1] = j->n_comp2; b.blend[1] = j->n_blend;
+    b.blend2[1] = j->n_blend2; b.scaled[1] = j->n_scaled; b.cfused[1] = j->n_cfused; b.cfused2[1] = j->n_cfused2;
+    b.expand[1] = j->n_expand;
+    for (int t = 0; t < B200_N_RECT_TX_SIZES; t++) b.itx[t][1] = j->n_itx[t];
+    return b;
 }
 
-int b200_frame_run_band(const B200FrameJob *j, const B200FrameBand *b, void *stream)
-{
-    return b200_frame_run_band_phase(j, b, B200_BAND_RECON | B200_BAND_POST, stream);
-}
-
-int b200_frame_run_band_phase(const B200FrameJob *j, const B200FrameBand *b, int phases, void *stream)
+// The stages before intra reconstruction, over the band's records. The first band zeroes the dense coefficients that
+// the coefficient expansion of every band fills.
+static int band_recon(const B200FrameJob *j, const B200FrameBand *b, void *stream)
 {
     int r;
-    const bool do_recon = phases & B200_BAND_RECON, do_post = phases & B200_BAND_POST;
     const int bd = j->bitdepth_max;
-    const int H = job_luma_h(j);
-    if ((b->y0 & 63) || b->y0 < 0 || b->y1 <= b->y0 || (!b->last && (b->y1 & 63)) || (b->last && b->y1 < H)) {
-        b200_set_error("b200_frame_run_band: band [%d, %d) must be 64-row aligned (last band: down to the picture height %d)", b->y0, b->y1, H);
-        return -2;
-    }
-    const bool first = b->y0 == 0;
-    // intra records form a dependency graph over the whole frame: they run with a band only when that band IS the frame
-    if (j->n_intra > 0 && !(first && b->last)) { b200_set_error("b200_frame_run_band: intra records are not band-sliced (one band, or b200_frame_run)"); return -2; }
-    if (j->run_resize) { b200_set_error("b200_frame_run_band: the super-resolution stage is not band-sliced (b200_frame_run)"); return -2; }
-    // (the grain LUTs belong to the post phase: its stream forks the preparation beside the first band and joins it before
-    // the last band's application)
-#ifndef B200_EMU
-    bool fg_forked = false;
-    if (do_post && first && j->run_fg) {       // grain LUTs depend on the frame header only
-        SideStream *fs = side_stream_for((cudaStream_t)stream, 0);
-        if (fs && fs->fork((cudaStream_t)stream)) { if ((r = b200_fg_prep(bd, &j->fg, fs->side))) return r; fg_forked = true; }
-    }
-    if (do_post && first && j->run_fg && !fg_forked && (r = b200_fg_prep(bd, &j->fg, stream))) return r;
-#else
-    if (do_post && first && j->run_fg && (r = b200_fg_prep(bd, &j->fg, stream))) return r;
-#endif
-    if (do_recon) {
-    if (first && j->n_expand > 0) B200_CUDA_OK(cudaMemsetAsync(j->d_coef, 0, j->coef_bytes, (cudaStream_t)stream));
+    if (b->y0 == 0 && j->n_expand > 0) B200_CUDA_OK(cudaMemsetAsync(j->d_coef, 0, j->coef_bytes, (cudaStream_t)stream));
 #define SUB(ptr, rng) ((ptr) ? (ptr) + (rng)[0] : (ptr)), ((ptr) ? (rng)[1] : 0)
     if (j->n_expand > 0 && (r = b200_coef_expand(bd, SUB(j->d_expand, b->expand), j->d_ccoef, j->d_coef, stream))) return r;
     if ((r = b200_mc_batch(bd, &j->mc, SUB(j->d_pred, b->pred), stream))) return r;
@@ -158,30 +44,133 @@ int b200_frame_run_band_phase(const B200FrameJob *j, const B200FrameBand *b, int
         itx_p[t] = j->d_itx[t] ? j->d_itx[t] + b->itx[t][0] : nullptr;
         itx_n[t] = j->d_itx[t] ? b->itx[t][1] : 0;
     }
-    if ((r = b200_itx_add_frame(bd, itx_p, itx_n, j->d_coef, j->mc.dst, j->itx_stride, j->zero_coefs, stream))) return r;
-    if (j->n_intra > 0 && (r = b200_intra_frame(bd, &j->intra, j->d_intra, j->n_intra, stream))) return r;
-    }
-    if (!do_post) return 0;
-    // sweeps: what this band's reconstruction makes final. Deblock: the band's own rows (a row-edge filter at y1 will still
-    // change rows >= y1 - 6). CDEF tile rows (32 luma rows, reading 2 more on each side): those ending at or above y1 - 32.
-    // Loop restoration tile rows (32 rows inside the 64-row stripes that end at 64 k - 8, reading CDEF output up to 3 rows
-    // further inside the stripe and 2 deblocked rows beyond it): luma tile rows ending at or above y1 - 40, a subsampled
-    // chroma stripe (one tile) once it ends at or above (y1 - 32) / 2 - 12.
+    return b200_itx_add_frame(bd, itx_p, itx_n, j->d_coef, j->mc.dst, j->itx_stride, j->zero_coefs, stream);
+}
+
+// film grain LUT preparation: one CTA, latency bound, depends only on the frame header -> a side stream, forked with the
+// first band (after everything enqueued so far: the scratch is reused frame after frame on this stream) and joined
+// before the last band applies the grain. Without a side stream it runs on the job's stream.
+static int fg_fork(const B200FrameJob *j, void *stream)
+{
+#ifndef B200_EMU
+    SideStream *fs = side_stream_for((cudaStream_t)stream, 0);
+    if (fs && fs->fork((cudaStream_t)stream)) return b200_fg_prep(j->bitdepth_max, &j->fg, fs->side);
+#endif
+    return b200_fg_prep(j->bitdepth_max, &j->fg, stream);
+}
+
+static int fg_join(void *stream)
+{
+#ifndef B200_EMU
+    SideStream *fs = side_stream_for((cudaStream_t)stream, 0);
+    if (fs && !fs->join((cudaStream_t)stream)) { b200_set_error("b200_frame_run: stream join failed"); return -1; }
+#else
+    (void)stream;
+#endif
+    return 0;
+}
+
+// The sweeps: what the band's reconstruction makes final. Deblock: the band's own rows (a row-edge filter at y1 will
+// still change rows >= y1 - 6). CDEF tile rows (32 luma rows, reading 2 more on each side): those ending at or above
+// y1 - 32. Loop restoration tile rows (32 rows inside the 64-row stripes that end at 64 k - 8, reading CDEF output up to
+// 3 rows further inside the stripe and 2 deblocked rows beyond it): luma tile rows ending at or above y1 - 40, a
+// subsampled chroma stripe (one tile) once it ends at or above (y1 - 32) / 2 - 12. Super-resolution (rejected for a band
+// that is not the whole frame) upscales between CDEF and loop restoration. The last band applies the film grain.
+static int band_post(const B200FrameJob *j, const B200FrameBand *b, void *stream)
+{
+    int r;
+    const int bd = j->bitdepth_max;
     const cudaStream_t st = (cudaStream_t)stream;
     if (j->run_lf && (r = b200::lf_frame_rows(bd, &j->lf, b->y0 >> 2, b->last ? j->lf.h4 : b->y1 >> 2, st))) return r;
     const int big = 1 << 28;
     if (j->run_cdef && (r = b200::cdef_frame_rows(bd, &j->cdef, b->y0 ? (b->y0 >> 5) - 1 : 0, b->last ? big : (b->y1 >> 5) - 1, st))) return r;
+    if (j->run_resize) {                     // CDEF output (and the deblocked picture LR reads) upscaled
+        if ((r = b200_resize_frame(bd, &j->resize[0], stream))) return r;
+        if ((r = b200_resize_frame(bd, &j->resize[1], stream))) return r;
+    }
     // (the top stripe is 8 rows shorter and its first tile row spans rows 0 .. 31: it needs CDEF rows up to 34, i.e. the band below)
     const int lr0 = b->y0 > 64 ? 2 * (b->y0 >> 6) - 1 : 0, lr1 = b->last ? big : (b->y1 > 64 ? 2 * (b->y1 >> 6) - 1 : 0);
     if (j->run_lr && (r = b200::lr_frame_rows(bd, &j->lr, lr0, lr1, st))) return r;
     if (b->last && j->run_fg) {
-#ifndef B200_EMU
-        SideStream *fs = side_stream_for(st, 0);
-        if (fs && !fs->join(st)) { b200_set_error("b200_frame_run_band: stream join failed"); return -1; }
-#endif
+        if ((r = fg_join(stream))) return r;
         if ((r = b200_fg_apply(bd, &j->fg, stream))) return r;
     }
     return 0;
+}
+
+static int run_band(const B200FrameJob *j, const B200FrameBand *b, int phases, void *stream)
+{
+    int r;
+    // the grain LUTs belong to the post phase: its stream forks the preparation beside the first band
+    if ((phases & B200_BAND_POST) && b->y0 == 0 && j->run_fg && (r = fg_fork(j, stream))) return r;
+    if (phases & B200_BAND_RECON) {
+        if ((r = band_recon(j, b, stream))) return r;
+        if (j->n_intra > 0 && (r = b200_intra_frame(j->bitdepth_max, &j->intra, j->d_intra, j->n_intra, stream))) return r;
+    }
+    return (phases & B200_BAND_POST) ? band_post(j, b, stream) : 0;
+}
+
+extern "C" {
+
+int b200_frame_run(const B200FrameJob *j, void *stream)
+{
+    const B200FrameBand b = whole_band(j);
+    return run_band(j, &b, B200_BAND_RECON | B200_BAND_POST, stream);
+}
+
+int b200_frame_run_batch(const B200FrameJob *const *jobs, int n, void *stream)
+{
+    if (n <= 0) return 0;
+    if (n > 256) { b200_set_error("b200_frame_run_batch: too many jobs"); return -2; }
+    int r;
+    B200IntraFrame frames[256];
+    const B200IntraTx *tx[256];
+    int32_t ntx[256];
+    for (int i = 0; i < n; i++) {
+        if (jobs[i]->bitdepth_max != jobs[0]->bitdepth_max) { b200_set_error("b200_frame_run_batch: mixed bit depths"); return -2; }
+        if (jobs[i]->run_fg) { b200_set_error("b200_frame_run_batch: film grain jobs must be run one by one"); return -2; }
+        const B200FrameBand b = whole_band(jobs[i]);
+        if ((r = band_recon(jobs[i], &b, stream))) return r;
+        frames[i] = jobs[i]->intra; tx[i] = jobs[i]->d_intra; ntx[i] = jobs[i]->n_intra;
+    }
+    if ((r = b200_intra_frames(jobs[0]->bitdepth_max, frames, tx, ntx, n, stream))) return r;
+    for (int i = 0; i < n; i++) {
+        const B200FrameBand b = whole_band(jobs[i]);
+        if ((r = band_post(jobs[i], &b, stream))) return r;
+    }
+    return 0;
+}
+
+// ---- band-sliced job (include/b200av1.h, B200FrameBand) --------------------------------------------------------
+int b200_band_progress(const B200FrameJob *j, int y1, int last, int plane)
+{
+    const int ssv = plane ? j->lf.ss_ver : 0;
+    const int ph = (job_luma_h(j) + ssv) >> ssv;
+    if (last) return ph;
+    int p;
+    if (j->run_lr)        p = ssv ? (y1 >> 1) - 36 : (y1 <= 64 ? 0 : y1 - 40);   // the last tile row that could run (see band_post)
+    else if (j->run_cdef) p = (y1 - 32) >> ssv;
+    else if (j->run_lf)   p = ssv ? (y1 >> 1) - 4 : y1 - 8;        // a row edge at y1 still changes up to 6 (chroma: 2) rows above it
+    else                  p = y1 >> ssv;
+    return p < 0 ? 0 : (p > ph ? ph : p);
+}
+
+int b200_frame_run_band(const B200FrameJob *j, const B200FrameBand *b, void *stream)
+{
+    return b200_frame_run_band_phase(j, b, B200_BAND_RECON | B200_BAND_POST, stream);
+}
+
+int b200_frame_run_band_phase(const B200FrameJob *j, const B200FrameBand *b, int phases, void *stream)
+{
+    const int H = job_luma_h(j);
+    if ((b->y0 & 63) || b->y0 < 0 || b->y1 <= b->y0 || (!b->last && (b->y1 & 63)) || (b->last && b->y1 < H)) {
+        b200_set_error("b200_frame_run_band: band [%d, %d) must be 64-row aligned (last band: down to the picture height %d)", b->y0, b->y1, H);
+        return -2;
+    }
+    // intra records form a dependency graph over the whole frame: they run with a band only when that band IS the frame
+    if (j->n_intra > 0 && !(b->y0 == 0 && b->last)) { b200_set_error("b200_frame_run_band: intra records are not band-sliced (one band, or b200_frame_run)"); return -2; }
+    if (j->run_resize) { b200_set_error("b200_frame_run_band: the super-resolution stage is not band-sliced (b200_frame_run)"); return -2; }
+    return run_band(j, b, phases, stream);
 }
 
 // ---- cross-GPU exchange primitives -------------------------------------------------------------------------------

@@ -875,7 +875,7 @@ static size_t intra_canvas_bytes(const B200IntraFrame *f, size_t px)
 int b200_intra_frames(int bdmax, const B200IntraFrame *frames, const B200IntraTx *const *d_tx, const int32_t *n_tx,
                       int n_frames, void *stream)
 {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("b200_intra_frames: bad bitdepth_max"); return -2; }
+    if (int r = check_bdmax(bdmax, "b200_intra_frames")) return r;
     const size_t px = bdmax > 255 ? 2 : 1;
     static const bool use_cta_kernel = getenv("B200_INTRA_CTA") != nullptr;      // round-1 CTA-per-block kernel (A/B measurements)
     for (int mode = 0; mode < 2; mode++)          // 0: per-transform-block dataflow, 1: superblock-granular
@@ -911,6 +911,8 @@ int b200_intra_frames(int bdmax, const B200IntraFrame *frames, const B200IntraTx
         }
         base = i;
         if (!nb) continue;
+        const dim3 cta_grid(grid, nb);
+        int r;
         if (mode == 0 && !use_cta_kernel) {
             // warp-per-block: a CTA carries kIwWarps blocks, so the same number of blocks in flight needs a quarter of the CTAs
             const size_t iw = kIwWarps * (bdmax > 255 ? sizeof(IwShared<true>) : sizeof(IwShared<false>));
@@ -922,11 +924,11 @@ int b200_intra_frames(int bdmax, const B200IntraFrame *frames, const B200IntraTx
                 iw_attr[bdmax > 255] = true;
             }
 #endif
-            if (bdmax > 255) { auto k = intra_warp_kernel<true>; B200_LAUNCH(k, dim3(grid, nb), dim3(kIwWarps * 32), iw, (cudaStream_t)stream, B, bdmax); }
-            else { auto k = intra_warp_kernel<false>; B200_LAUNCH(k, dim3(grid, nb), dim3(kIwWarps * 32), iw, (cudaStream_t)stream, B, bdmax); }
+            r = launch_hbd(bdmax, Launch::plain, cta_grid, dim3(kIwWarps * 32), iw, (cudaStream_t)stream,
+                           [&](auto hbd) { return std::make_tuple(intra_warp_kernel<hbd>, B, bdmax); });
         } else if (mode == 0) {
-            if (bdmax > 255) { auto k = intra_frame_kernel<true>; B200_LAUNCH(k, dim3(grid, nb), dim3(kIpT), 0, (cudaStream_t)stream, B, bdmax); }
-            else { auto k = intra_frame_kernel<false>; B200_LAUNCH(k, dim3(grid, nb), dim3(kIpT), 0, (cudaStream_t)stream, B, bdmax); }
+            r = launch_hbd(bdmax, Launch::plain, cta_grid, dim3(kIpT), 0, (cudaStream_t)stream,
+                           [&](auto hbd) { return std::make_tuple(intra_frame_kernel<hbd>, B, bdmax); });
         } else {
 #ifndef B200_EMU
             static bool attr_set[2] = { false, false };
@@ -936,11 +938,10 @@ int b200_intra_frames(int bdmax, const B200IntraFrame *frames, const B200IntraTx
                 attr_set[bdmax > 255] = true;
             }
 #endif
-            if (bdmax > 255) { auto k = intra_sb_kernel<true>; B200_LAUNCH(k, dim3(grid, nb), dim3(kIpT), dyn, (cudaStream_t)stream, B, bdmax); }
-            else { auto k = intra_sb_kernel<false>; B200_LAUNCH(k, dim3(grid, nb), dim3(kIpT), dyn, (cudaStream_t)stream, B, bdmax); }
+            r = launch_hbd(bdmax, Launch::plain, cta_grid, dim3(kIpT), dyn, (cudaStream_t)stream,
+                           [&](auto hbd) { return std::make_tuple(intra_sb_kernel<hbd>, B, bdmax); });
         }
-        b200_count_launch();
-        B200_CUDA_OK(cudaGetLastError());
+        if (r) return r;
     }
     return 0;
 }

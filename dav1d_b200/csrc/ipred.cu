@@ -56,46 +56,44 @@ extern "C" {
 
 int b200_ipred_batch(int bdmax, const B200IpredFrame *f, const B200IpredBlock *d_blocks, int n, void *stream)
 {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("b200_ipred_batch: bad bitdepth_max"); return -2; }
+    if (int r = check_bdmax(bdmax, "b200_ipred_batch")) return r;
     if (n <= 0) return 0;
-    if (bdmax > 255) { auto k = ipred_kernel<true>; B200_LAUNCH(k, dim3(n), dim3(kIpT), 0, (cudaStream_t)stream, d_blocks, n, *f, bdmax); }
-    else { auto k = ipred_kernel<false>; B200_LAUNCH(k, dim3(n), dim3(kIpT), 0, (cudaStream_t)stream, d_blocks, n, *f, bdmax); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return launch_hbd(bdmax, Launch::plain, dim3(n), dim3(kIpT), 0, (cudaStream_t)stream,
+                      [&](auto hbd) { return std::make_tuple(ipred_kernel<hbd>, d_blocks, n, *f, bdmax); });
 }
 
 }
 
 // ---- Level 1 -------------------------------------------------------------------------------
 namespace {
-Scratch s_dst, s_edge, s_ac, s_idx, s_desc;
-uint8_t h_px[64 * 64 * 2];
+enum { DST, EDGE, AC, IDX, DESC };   // Level1 scratch slots
 
-int ipred_l1(int op, int mode, void *dst, ptrdiff_t stride, const void *topleft, int w, int h, int angle, int max_w,
-             int max_h, const int16_t *ac, int alpha, int bdmax)
+// the one-record batch of f / b, then the w x h pixels it wrote into the rectangle at dst
+int ipred_l1(Level1 &L, B200IpredFrame &f, const B200IpredBlock &b, void *dst, ptrdiff_t stride, int bdmax)
 {
-    std::lock_guard<std::mutex> lk(host_lock());
+    const void *desc = L.upload(DESC, &b, sizeof(b));
+    if (!desc) return -1;
+    if (int r = b200_ipred_batch(bdmax, &f, (const B200IpredBlock *)desc, 1, 0)) return r;
+    return L.download_rect(DST, dst, stride, b.w, b.h, bdmax > 255 ? 2 : 1);
+}
+
+int ipred_pred_l1(int op, int mode, void *dst, ptrdiff_t stride, const void *topleft, int w, int h, int angle, int max_w,
+                  int max_h, const int16_t *ac, int alpha, int bdmax)
+{
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
-    const int n_edge = 2 * (w + h) + 1;
-    // the edge window [-(w+h), w+h] around topleft
-    if (s_edge.upload((const uint8_t *)topleft - (ptrdiff_t)(w + h) * (ptrdiff_t)px, (size_t)n_edge * px)) return -1;
-    if (s_dst.reserve((size_t)w * h * px) || s_desc.reserve(sizeof(B200IpredBlock))) return -1;
-    if (op == B200_IPRED_OP_CFL_PRED && s_ac.upload(ac, (size_t)w * h * 2)) return -1;
     B200IpredFrame f;
     memset(&f, 0, sizeof(f));
-    f.dst = s_dst.p; f.dst_stride[0] = w; f.edge = s_edge.p; f.ac = (int16_t *)s_ac.p;
+    f.dst_stride[0] = w;
+    // the edge window [-(w+h), w+h] around topleft
+    if (!(f.edge = L.upload(EDGE, (const uint8_t *)topleft - (ptrdiff_t)(w + h) * (ptrdiff_t)px, (size_t)(2 * (w + h) + 1) * px)) ||
+        !(f.dst = L.dev(DST, (size_t)w * h * px)) || (op == B200_IPRED_OP_CFL_PRED && !(f.ac = (int16_t *)L.upload(AC, ac, (size_t)w * h * 2))))
+        return -1;
     B200IpredBlock b;
     memset(&b, 0, sizeof(b));
     b.edge_off = (uint32_t)(w + h); b.w = (uint8_t)w; b.h = (uint8_t)h; b.mode = (uint8_t)mode; b.op = (uint8_t)op;
     b.angle = (int16_t)angle; b.max_w = max_w; b.max_h = max_h; b.alpha = (int8_t)alpha;
-    if (s_desc.upload(&b, sizeof(b))) return -1;
-    int r = b200_ipred_batch(bdmax, &f, (const B200IpredBlock *)s_desc.p, 1, 0);
-    if (r) return r;
-    if (s_dst.download(h_px, (size_t)w * h * px)) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
-    unpack_rect(dst, stride, h_px, w, h, px);
-    return 0;
+    return ipred_l1(L, f, b, dst, stride, bdmax);
 }
 }  // namespace
 
@@ -104,53 +102,47 @@ extern "C" {
 int b200_ipred(int mode, void *dst, ptrdiff_t stride, const void *topleft, int w, int h, int angle, int max_w, int max_h, int bdmax)
 {
     if (mode < 0 || mode > 13 || w < 4 || w > 64 || h < 4 || h > 64 || (mode == 13 && (w > 32 || h > 32))) { b200_set_error("b200_ipred: bad arguments"); return -2; }
-    return ipred_l1(B200_IPRED_OP_PRED, mode, dst, stride, topleft, w, h, angle, max_w, max_h, nullptr, 0, bdmax);
+    return ipred_pred_l1(B200_IPRED_OP_PRED, mode, dst, stride, topleft, w, h, angle, max_w, max_h, nullptr, 0, bdmax);
 }
 int b200_cfl_pred(int mode, void *dst, ptrdiff_t stride, const void *topleft, int w, int h, const int16_t *ac, int alpha, int bdmax)
 {
     if (!(mode == 0 || mode == 3 || mode == 4 || mode == 5) || w < 4 || w > 32 || h < 4 || h > 32) { b200_set_error("b200_cfl_pred: bad arguments"); return -2; }
-    return ipred_l1(B200_IPRED_OP_CFL_PRED, mode, dst, stride, topleft, w, h, 0, 0, 0, ac, alpha, bdmax);
+    return ipred_pred_l1(B200_IPRED_OP_CFL_PRED, mode, dst, stride, topleft, w, h, 0, 0, 0, ac, alpha, bdmax);
 }
 int b200_cfl_ac(int16_t *ac, const void *ypx, ptrdiff_t stride, int w_pad, int h_pad, int cw, int ch, int ss_hor, int ss_ver, int bdmax)
 {
     if (cw < 4 || cw > 32 || ch < 4 || ch > 32) { b200_set_error("b200_cfl_ac: bad arguments"); return -2; }
-    std::lock_guard<std::mutex> lk(host_lock());
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
     const int lw = (cw - 4 * w_pad) << ss_hor, lh = (ch - 4 * h_pad) << ss_ver;   // luma samples actually read
-    pack_rect(h_px, ypx, stride, lw, lh, px);
-    if (s_dst.upload(h_px, (size_t)lw * lh * px) || s_ac.reserve((size_t)cw * ch * 2) || s_desc.reserve(sizeof(B200IpredBlock))) return -1;
     B200IpredFrame f;
     memset(&f, 0, sizeof(f));
-    f.dst = s_dst.p; f.dst_stride[0] = lw; f.ss_hor = ss_hor; f.ss_ver = ss_ver; f.ac = (int16_t *)s_ac.p;
+    f.dst_stride[0] = lw; f.ss_hor = ss_hor; f.ss_ver = ss_ver;
     B200IpredBlock b;
     memset(&b, 0, sizeof(b));
     b.w = (uint8_t)cw; b.h = (uint8_t)ch; b.op = B200_IPRED_OP_CFL_AC; b.angle = (int16_t)(w_pad | (h_pad << 8));
-    if (s_desc.upload(&b, sizeof(b))) return -1;
-    int r = b200_ipred_batch(bdmax, &f, (const B200IpredBlock *)s_desc.p, 1, 0);
-    if (r) return r;
-    if (s_ac.download(ac, (size_t)cw * ch * 2)) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
-    return 0;
+    const void *desc;
+    if (!(f.dst = L.upload_rect(DST, ypx, stride, lw, lh, px)) || !(f.ac = (int16_t *)L.dev(AC, (size_t)cw * ch * 2)) ||
+        !(desc = L.upload(DESC, &b, sizeof(b))))
+        return -1;
+    if (int r = b200_ipred_batch(bdmax, &f, (const B200IpredBlock *)desc, 1, 0)) return r;
+    return L.download_rect(AC, ac, (ptrdiff_t)cw * 2, cw, ch, 2);
 }
 int b200_pal_pred(void *dst, ptrdiff_t stride, const void *pal, const uint8_t *idx, int w, int h, int bdmax)
 {
     if (w < 4 || w > 64 || h < 4 || h > 64) { b200_set_error("b200_pal_pred: bad arguments"); return -2; }
-    std::lock_guard<std::mutex> lk(host_lock());
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
-    if (s_edge.upload(pal, 8 * px) || s_idx.upload(idx, (size_t)w * h / 2) || s_dst.reserve((size_t)w * h * px) || s_desc.reserve(sizeof(B200IpredBlock))) return -1;
     B200IpredFrame f;
     memset(&f, 0, sizeof(f));
-    f.dst = s_dst.p; f.dst_stride[0] = w; f.edge = s_edge.p; f.pal_idx = (const uint8_t *)s_idx.p;
+    f.dst_stride[0] = w;
+    if (!(f.edge = L.upload(EDGE, pal, 8 * px)) || !(f.pal_idx = (const uint8_t *)L.upload(IDX, idx, (size_t)w * h / 2)) ||
+        !(f.dst = L.dev(DST, (size_t)w * h * px)))
+        return -1;
     B200IpredBlock b;
     memset(&b, 0, sizeof(b));
     b.w = (uint8_t)w; b.h = (uint8_t)h; b.op = B200_IPRED_OP_PAL_PRED;
-    if (s_desc.upload(&b, sizeof(b))) return -1;
-    int r = b200_ipred_batch(bdmax, &f, (const B200IpredBlock *)s_desc.p, 1, 0);
-    if (r) return r;
-    if (s_dst.download(h_px, (size_t)w * h * px)) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
-    unpack_rect(dst, stride, h_px, w, h, px);
-    return 0;
+    return ipred_l1(L, f, b, dst, stride, bdmax);
 }
 
 }  // extern "C"

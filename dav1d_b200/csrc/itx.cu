@@ -68,7 +68,7 @@ itx_add_grouped_kernel(const __grid_constant__ ItxGroups g, typename Bd<HBD>::co
 #undef X
 }
 
-int launch_itx_grouped(bool hbd, const void *const *blocks, const int32_t *n, void *coefs, void *pic, const int32_t *st,
+int launch_itx_grouped(const void *const *blocks, const int32_t *n, void *coefs, void *pic, const int32_t *st,
                        int bdmax, int zero, cudaStream_t stream)
 {
     for (int big = 1; big >= 0; big--) {
@@ -83,67 +83,34 @@ int launch_itx_grouped(bool hbd, const void *const *blocks, const int32_t *n, vo
         B200_ITX_SIZES(X)
 #undef X
         if (!total) continue;
-        if (hbd) {
-            if (big) { auto k = itx_add_grouped_kernel<true, true>; B200_LAUNCH_PDL(k, dim3(total), dim3(kItxWarps * 32), 0, stream, g, (int32_t *)coefs, (uint16_t *)pic, st[0], st[1], st[2], bdmax, zero); }
-            else { auto k = itx_add_grouped_kernel<true, false>; B200_LAUNCH_PDL(k, dim3(total), dim3(kItxWarps * 32), 0, stream, g, (int32_t *)coefs, (uint16_t *)pic, st[0], st[1], st[2], bdmax, zero); }
-        } else {
-            if (big) { auto k = itx_add_grouped_kernel<false, true>; B200_LAUNCH_PDL(k, dim3(total), dim3(kItxWarps * 32), 0, stream, g, (int16_t *)coefs, (uint8_t *)pic, st[0], st[1], st[2], bdmax, zero); }
-            else { auto k = itx_add_grouped_kernel<false, false>; B200_LAUNCH_PDL(k, dim3(total), dim3(kItxWarps * 32), 0, stream, g, (int16_t *)coefs, (uint8_t *)pic, st[0], st[1], st[2], bdmax, zero); }
-        }
-        b200_count_launch();
+        if (int r = launch_hbd(bdmax, Launch::pdl, dim3(total), dim3(kItxWarps * 32), 0, stream, [&](auto hbd) {
+                typedef Bd<hbd> B;
+                return std::make_tuple(big ? itx_add_grouped_kernel<hbd, true> : itx_add_grouped_kernel<hbd, false>, g,
+                                       (typename B::coef *)coefs, (typename B::pixel *)pic, st[0], st[1], st[2], bdmax, zero);
+            }))
+            return r;
     }
     return 0;
 }
 
-template <int W, int H, int TX, int SHIFT>
-static int launch_itx_wh(bool hbd, const B200ItxBlock *blocks, int n, void *coefs, void *pic,
-                         const int32_t *st, int bdmax, int zero, cudaStream_t stream)
+// one transform size: n blocks of the batch, BPC of them per CTA
+int launch_itx(int tx, const B200ItxBlock *blocks, int n, void *coefs, void *pic, const int32_t *st, int bdmax, int zero,
+               cudaStream_t stream)
 {
-    typedef ItxGeom<W, H> G;
-    const int per_cta = ItxGeom<W, H>::BPC;
-    const int grid = (n + per_cta - 1) / per_cta;
-    if (grid <= 0) return 0;
-    if (hbd) {
-        auto k = itx_add_kernel<W, H, TX, SHIFT, true>;
-        B200_LAUNCH(k, dim3(grid), dim3(kItxWarps * 32), 0, stream, blocks, n, (int32_t *)coefs,
-                    (uint16_t *)pic, st[0], st[1], st[2], bdmax, zero);
-    } else {
-        auto k = itx_add_kernel<W, H, TX, SHIFT, false>;
-        B200_LAUNCH(k, dim3(grid), dim3(kItxWarps * 32), 0, stream, blocks, n, (int16_t *)coefs,
-                    (uint8_t *)pic, st[0], st[1], st[2], bdmax, zero);
-    }
-    b200_count_launch();
-    return 0;
-}
-
-// tx -> (w, h, inter-pass shift): reference src/itx_tmpl.c:160-178
-int launch_itx(int tx, bool hbd, const B200ItxBlock *blocks, int n, void *coefs, void *pic,
-               const int32_t *st, int bdmax, int zero, cudaStream_t stream)
-{
-#define CASE(TX, W, H, SH) case TX: return launch_itx_wh<W, H, TX, SH>(hbd, blocks, n, coefs, pic, st, bdmax, zero, stream)
     switch (tx) {
-    CASE(0, 4, 4, 0);
-    CASE(1, 8, 8, 1);
-    CASE(2, 16, 16, 2);
-    CASE(3, 32, 32, 2);
-    CASE(4, 64, 64, 2);
-    CASE(5, 4, 8, 0);
-    CASE(6, 8, 4, 0);
-    CASE(7, 8, 16, 1);
-    CASE(8, 16, 8, 1);
-    CASE(9, 16, 32, 1);
-    CASE(10, 32, 16, 1);
-    CASE(11, 32, 64, 1);
-    CASE(12, 64, 32, 1);
-    CASE(13, 4, 16, 1);
-    CASE(14, 16, 4, 1);
-    CASE(15, 8, 32, 2);
-    CASE(16, 32, 8, 2);
-    CASE(17, 16, 64, 2);
-    CASE(18, 64, 16, 2);
+#define X(TX, W, H, SH) \
+    case TX: \
+        return launch_hbd(bdmax, Launch::plain, dim3((n + ItxGeom<W, H>::BPC - 1) / ItxGeom<W, H>::BPC), dim3(kItxWarps * 32), 0, stream, \
+                          [&](auto hbd) { \
+                              typedef Bd<hbd> B; \
+                              return std::make_tuple(itx_add_kernel<W, H, TX, SH, hbd>, blocks, n, (typename B::coef *)coefs, \
+                                                     (typename B::pixel *)pic, st[0], st[1], st[2], bdmax, zero); \
+                          });
+    B200_ITX_SIZES(X)
+#undef X
     }
-#undef CASE
-    return -1;
+    b200_set_error("bad transform size %d", tx);
+    return -2;
 }
 
 }  // namespace b200

@@ -329,13 +329,6 @@ B200_DEV void itx_add_warp(int *const t, typename Bd<HBD>::coef *const cf, typen
     __syncwarp();
 }
 
-// tx -> (w, h, inter-pass shift): reference src/itx_tmpl.c:160-178
-#define B200_ITX_SIZES(X) \
-    X(4, 64, 64, 2) X(11, 32, 64, 1) X(12, 64, 32, 1) X(17, 16, 64, 2) X(18, 64, 16, 2) X(3, 32, 32, 2) X(9, 16, 32, 1) \
-    X(10, 32, 16, 1) X(15, 8, 32, 2) X(16, 32, 8, 2) X(2, 16, 16, 2) X(7, 8, 16, 1) X(8, 16, 8, 1) X(13, 4, 16, 1) \
-    X(14, 16, 4, 1) X(1, 8, 8, 1) X(5, 4, 8, 0) X(6, 8, 4, 0) X(0, 4, 4, 0)
-
-
 // transform size -> width / height in 4-sample units
 static __constant__ uint8_t c_tx_w4[B200_N_RECT_TX_SIZES] = { 1, 2, 4, 8, 16, 1, 2, 2, 4, 4, 8, 8, 16, 1, 4, 2, 8, 4, 16 };
 static __constant__ uint8_t c_tx_h4[B200_N_RECT_TX_SIZES] = { 1, 2, 4, 8, 16, 2, 1, 4, 2, 8, 4, 16, 8, 4, 1, 8, 2, 16, 4 };

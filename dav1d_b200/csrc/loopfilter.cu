@@ -201,24 +201,17 @@ __global__ void lf_sb_kernel(typename Bd<HBD>::pixel *dst, LfSbArgs a, int bdmax
 // whole-frame order: a row-edge filter at y touches rows y - 7 .. y + 6 only, all of them column-filtered already.
 int lf_frame_rows(int bdmax, const B200LfFrame *f, int ya4, int yb4, cudaStream_t stream)
 {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("b200_lf_frame: bad bitdepth_max %d", bdmax); return -2; }
+    if (int r = check_bdmax(bdmax, "b200_lf_frame")) return r;
     if (!f->filter_y) return 0;   // dav1d skips deblocking entirely when both luma levels are 0 (src/recon_tmpl.c:1988)
     ya4 = imax(ya4, 0); yb4 = imin(yb4, f->h4);
     if (yb4 <= ya4) return 0;
     if ((ya4 & 1) || ((yb4 & 1) && yb4 != f->h4)) { b200_set_error("b200_lf_frame: odd band boundary"); return -2; }
     const int w4 = f->w4, n4 = yb4 - ya4;
-    dim3 g1((w4 + 31) / 32, (n4 + 7) / 8, 3), b1(32, 8);
-    dim3 g2((w4 * 4 + 127) / 128, (n4 + 1) / 2, 3), b2(128, 2);
-    if (bdmax > 255) {
-        auto k1 = lf_cols_kernel<true>; B200_LAUNCH_PDL(k1, g1, b1, 0, stream, *f, bdmax, ya4, yb4);
-        auto k2 = lf_rows_kernel<true>; B200_LAUNCH_PDL(k2, g2, b2, 0, stream, *f, bdmax, ya4, yb4);
-    } else {
-        auto k1 = lf_cols_kernel<false>; B200_LAUNCH_PDL(k1, g1, b1, 0, stream, *f, bdmax, ya4, yb4);
-        auto k2 = lf_rows_kernel<false>; B200_LAUNCH_PDL(k2, g2, b2, 0, stream, *f, bdmax, ya4, yb4);
-    }
-    b200_count_launch(); b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    if (int r = launch_hbd(bdmax, Launch::pdl, dim3((w4 + 31) / 32, (n4 + 7) / 8, 3), dim3(32, 8), 0, stream,
+                           [&](auto hbd) { return std::make_tuple(lf_cols_kernel<hbd>, *f, bdmax, ya4, yb4); }))
+        return r;
+    return launch_hbd(bdmax, Launch::pdl, dim3((w4 * 4 + 127) / 128, (n4 + 1) / 2, 3), dim3(128, 2), 0, stream,
+                      [&](auto hbd) { return std::make_tuple(lf_rows_kernel<hbd>, *f, bdmax, ya4, yb4); });
 }
 
 }  // namespace b200
@@ -236,13 +229,11 @@ int b200_loop_filter_sb(int plane_class, int dir, void *dst, ptrdiff_t stride, c
                         const uint8_t (*lvl)[4], ptrdiff_t lvl_stride, const B200FilterLUT *lut, int w, int bdmax)
 {
     (void)w;   // like the C reference, the extent comes from the highest set mask bit
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("b200_loop_filter_sb: bad bitdepth_max"); return -2; }
+    if (int r = check_bdmax(bdmax, "b200_loop_filter_sb")) return r;
     const uint32_t vm = mask[0] | mask[1] | (plane_class ? 0 : mask[2]);
     if (!vm) return 0;
     int n_units = 32 - __builtin_clz(vm);
-    std::lock_guard<std::mutex> lk(host_lock());
-    static Scratch s_win;
-    static uint8_t h_win[16 * 128 * 2];
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
     LfSbArgs a;
     memset(&a, 0, sizeof(a));
@@ -254,20 +245,16 @@ int b200_loop_filter_sb(int plane_class, int dir, void *dst, ptrdiff_t stride, c
         a.prev[u] = dir ? l[-lvl_stride][0] : l[-1][0];
     }
     const int lines = n_units * 4;
-    int ww, wh; const uint8_t *org;
-    if (dir) { ww = lines; wh = 16; org = (const uint8_t *)dst - 8 * stride; }
-    else { ww = 16; wh = lines; org = (const uint8_t *)dst - 8 * (ptrdiff_t)px; }
+    int ww, wh; uint8_t *org;
+    if (dir) { ww = lines; wh = 16; org = (uint8_t *)dst - 8 * stride; }
+    else { ww = 16; wh = lines; org = (uint8_t *)dst - 8 * (ptrdiff_t)px; }
     a.stride = ww;
-    pack_rect(h_win, org, stride, ww, wh, px);
-    if (s_win.upload(h_win, (size_t)ww * wh * px)) return -1;
-    const int grid = (lines + 127) / 128;
-    if (bdmax > 255) { auto k = lf_sb_kernel<true>; B200_LAUNCH(k, dim3(grid), dim3(128), 0, (cudaStream_t)0, (uint16_t *)s_win.p, a, bdmax); }
-    else { auto k = lf_sb_kernel<false>; B200_LAUNCH(k, dim3(grid), dim3(128), 0, (cudaStream_t)0, (uint8_t *)s_win.p, a, bdmax); }
-    b200_count_launch();
-    if (s_win.download(h_win, (size_t)ww * wh * px)) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
-    unpack_rect((uint8_t *)org, stride, h_win, ww, wh, px);
-    return 0;
+    void *win = L.upload_rect(0, org, stride, ww, wh, px);
+    if (!win) return -1;
+    if (int r = launch_hbd(bdmax, Launch::plain, dim3((lines + 127) / 128), dim3(128), 0, 0,
+                           [&](auto hbd) { return std::make_tuple(lf_sb_kernel<hbd>, (typename Bd<hbd>::pixel *)win, a, bdmax); }))
+        return r;
+    return L.download_rect(0, org, stride, ww, wh, px);
 }
 
 }  // extern "C"

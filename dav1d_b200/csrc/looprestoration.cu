@@ -339,7 +339,7 @@ __global__ void __launch_bounds__(256) lr_window_kernel(const typename Bd<HBD>::
 // [r0 / 2, r1 / 2) — callers that cut a frame into bands pass r0, r1 odd: a chroma stripe runs with the band that completes it.
 int lr_frame_rows(int bdmax, const B200LrFrame *f, int r0, int r1, cudaStream_t stream)
 {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("b200_lr_frame: bad bitdepth_max %d", bdmax); return -2; }
+    if (int r = check_bdmax(bdmax, "b200_lr_frame")) return r;
     for (int i = 0; i < 2; i++)
         if (f->unit_size_log2[i] < 5 || f->unit_size_log2[i] > 8) { b200_set_error("b200_lr_frame: bad unit size"); return -2; }
     const int n_stripes = (f->h + 8 + 63) / 64;
@@ -360,12 +360,8 @@ int lr_frame_rows(int bdmax, const B200LrFrame *f, int r0, int r1, cudaStream_t 
         total += lg.nx[p] * imax(b - a, 0);
     }
     if (!total) return 0;
-    dim3 grid(total);
-    if (bdmax > 255) { auto k = lr_frame_kernel<true>; B200_LAUNCH_PDL(k, grid, dim3(256), 0, stream, *f, lg, bdmax); }
-    else { auto k = lr_frame_kernel<false>; B200_LAUNCH_PDL(k, grid, dim3(256), 0, stream, *f, lg, bdmax); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return launch_hbd(bdmax, Launch::pdl, dim3(total), dim3(256), 0, stream,
+                      [&](auto hbd) { return std::make_tuple(lr_frame_kernel<hbd>, *f, lg, bdmax); });
 }
 
 }  // namespace b200
@@ -382,19 +378,18 @@ int b200_lr_frame(int bdmax, const B200LrFrame *f, void *stream)
 int b200_lr_filter(int kind, void *dst, ptrdiff_t stride, const void *left, const void *lpf, int w, int h,
                    const void *params, int edges, int bdmax)
 {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("b200_lr_filter: bad bitdepth_max"); return -2; }
+    if (int r = check_bdmax(bdmax, "b200_lr_filter")) return r;
     if (kind < 0 || kind > 3 || w < 1 || w > 384 || h < 1 || h > 64) { b200_set_error("b200_lr_filter: bad arguments"); return -2; }
-    std::lock_guard<std::mutex> lk(host_lock());
-    static Scratch s_win, s_out;
-    static uint8_t h_win[(384 + 6) * (64 + 6) * 2], h_out[384 * 64 * 2];
-    const bool hbd = bdmax > 255;
-    const size_t px = hbd ? 2 : 1;
+    Level1 L;
+    const size_t px = bdmax > 255 ? 2 : 1;
     // which short-stripe exits of the C reference skip the bottom rows (see oracle/looprestoration.c header)
     int use_bottom;
     if (kind == 0) use_bottom = (edges & 8) && h > ((edges & 4) ? 3 : 5);
     else if (kind == 2) use_bottom = (edges & 8) && h > 2;
     else use_bottom = (edges & 8) && !(h & 1) && h > ((edges & 4) ? 2 : 4);
     // assemble the virtual source window (pure data movement; all arithmetic happens on the device)
+    uint8_t *win = (uint8_t *)L.host((size_t)(w + 6) * (h + 6) * px);
+    if (!win) return -1;
     for (int y = -3; y < h + 3; y++) {
         const uint8_t *row; int from_unit = 0, yy = y;
         if (y < 0 && (edges & 4)) row = (const uint8_t *)lpf + (ptrdiff_t)((y < -2 ? -2 : y) + 2) * stride;
@@ -408,7 +403,7 @@ int b200_lr_filter(int kind, void *dst, ptrdiff_t stride, const void *left, cons
                 else sp = row + (ptrdiff_t)x * (ptrdiff_t)px;
             } else if (x >= w && !(edges & 2)) sp = row + (size_t)(w - 1) * px;
             else sp = row + (size_t)x * px;
-            memcpy(h_win + ((size_t)(y + 3) * (w + 6) + (x + 3)) * px, sp, px);
+            memcpy(win + ((size_t)(y + 3) * (w + 6) + (x + 3)) * px, sp, px);
         }
     }
     LrTileParams P;
@@ -425,15 +420,14 @@ int b200_lr_filter(int kind, void *dst, ptrdiff_t stride, const void *left, cons
         P.w0 = kind == 2 ? 0 : wp[0]; P.w1 = kind == 1 ? 0 : wp[1];
         if (kind == 1) P.w0 = wp[0];   // sgr_5x5 weights its single term with w0
     }
-    if (s_win.upload(h_win, (size_t)(w + 6) * (h + 6) * px) || s_out.reserve((size_t)w * h * px)) return -1;
-    dim3 grid((w + kTW - 1) / kTW, (h + kTH - 1) / kTH);
-    if (hbd) { auto k = lr_window_kernel<true>; B200_LAUNCH(k, grid, dim3(256), 0, (cudaStream_t)0, (const uint16_t *)s_win.p, (uint16_t *)s_out.p, w, h, P, bdmax); }
-    else { auto k = lr_window_kernel<false>; B200_LAUNCH(k, grid, dim3(256), 0, (cudaStream_t)0, (const uint8_t *)s_win.p, (uint8_t *)s_out.p, w, h, P, bdmax); }
-    b200_count_launch();
-    if (s_out.download(h_out, (size_t)w * h * px)) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
-    unpack_rect(dst, stride, h_out, w, h, px);
-    return 0;
+    void *in, *out;
+    if (!(in = L.upload(0, win, (size_t)(w + 6) * (h + 6) * px)) || !(out = L.dev(1, (size_t)w * h * px))) return -1;
+    if (int r = launch_hbd(bdmax, Launch::plain, dim3((w + kTW - 1) / kTW, (h + kTH - 1) / kTH), dim3(256), 0, 0, [&](auto hbd) {
+            typedef typename Bd<hbd>::pixel pixel;
+            return std::make_tuple(lr_window_kernel<hbd>, (const pixel *)in, (pixel *)out, w, h, P, bdmax);
+        }))
+        return r;
+    return L.download_rect(1, dst, stride, w, h, px);
 }
 
 }  // extern "C"

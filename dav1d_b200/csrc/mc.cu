@@ -676,158 +676,101 @@ __global__ void __launch_bounds__(256) resize_frame_kernel(const __grid_constant
 // =======================================================================================
 using namespace b200;
 
-static int check_bd(int bdmax, const char *who) {
-    if (bdmax != 255 && bdmax != 1023 && bdmax != 4095) { b200_set_error("%s: bad bitdepth_max %d", who, bdmax); return -2; }
-    return 0;
+// one prediction stage of a frame: records [0, n), `per_cta` of them per CTA of `threads` threads
+template <class Rec, class Kern>
+static int mc_stage(const char *who, int bdmax, const B200McFrame *frame, const Rec *d_blocks, int n, int per_cta, int threads,
+                    void *stream, Kern kern)
+{
+    if (int r = check_bdmax(bdmax, who)) return r;
+    if (n <= 0) return 0;
+    return launch_hbd(bdmax, Launch::pdl, dim3((n + per_cta - 1) / per_cta), dim3(threads), 0, (cudaStream_t)stream,
+                      [&](auto hbd) { return std::make_tuple(kern(hbd), d_blocks, n, *frame, bdmax); });
 }
 
 extern "C" {
 
 int b200_mc_batch(int bitdepth_max, const B200McFrame *frame, const B200McBlock *d_blocks, int n, void *stream) {
-    if (check_bd(bitdepth_max, "b200_mc_batch")) return -2;
-    if (n <= 0) return 0;
-    if (bitdepth_max > 255) { auto k = mc_pred_kernel<true>; B200_LAUNCH_PDL(k, dim3((n + kMcWarps - 1) / kMcWarps), dim3(kMcWarps * 32), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    else { auto k = mc_pred_kernel<false>; B200_LAUNCH_PDL(k, dim3((n + kMcWarps - 1) / kMcWarps), dim3(kMcWarps * 32), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return mc_stage("b200_mc_batch", bitdepth_max, frame, d_blocks, n, kMcWarps, kMcWarps * 32, stream, [](auto hbd) { return mc_pred_kernel<hbd>; });
 }
 int b200_mc_scaled_batch(int bitdepth_max, const B200McFrame *frame, const B200McScaledBlock *d_blocks, int n, void *stream) {
-    if (check_bd(bitdepth_max, "b200_mc_scaled_batch")) return -2;
-    if (n <= 0) return 0;
-    if (bitdepth_max > 255) { auto k = mc_scaled_kernel<true>; B200_LAUNCH_PDL(k, dim3(n), dim3(256), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    else { auto k = mc_scaled_kernel<false>; B200_LAUNCH_PDL(k, dim3(n), dim3(256), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return mc_stage("b200_mc_scaled_batch", bitdepth_max, frame, d_blocks, n, 1, 256, stream, [](auto hbd) { return mc_scaled_kernel<hbd>; });
 }
 int b200_mc_comp_fused_batch(int bitdepth_max, const B200McFrame *frame, const B200CompFusedBlock *d_blocks, int n, void *stream) {
-    if (check_bd(bitdepth_max, "b200_mc_comp_fused_batch")) return -2;
-    if (n <= 0) return 0;
-    if (bitdepth_max > 255) { auto k = mc_comp_fused_kernel<true>; B200_LAUNCH_PDL(k, dim3((n + kMcWarps - 1) / kMcWarps), dim3(kMcWarps * 32), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    else { auto k = mc_comp_fused_kernel<false>; B200_LAUNCH_PDL(k, dim3((n + kMcWarps - 1) / kMcWarps), dim3(kMcWarps * 32), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return mc_stage("b200_mc_comp_fused_batch", bitdepth_max, frame, d_blocks, n, kMcWarps, kMcWarps * 32, stream, [](auto hbd) { return mc_comp_fused_kernel<hbd>; });
 }
 int b200_mc_comp_batch(int bitdepth_max, const B200McFrame *frame, const B200CompBlock *d_blocks, int n, void *stream) {
-    if (check_bd(bitdepth_max, "b200_mc_comp_batch")) return -2;
-    if (n <= 0) return 0;
-    if (bitdepth_max > 255) { auto k = mc_comp_kernel<true>; B200_LAUNCH_PDL(k, dim3(n), dim3(128), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    else { auto k = mc_comp_kernel<false>; B200_LAUNCH_PDL(k, dim3(n), dim3(128), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return mc_stage("b200_mc_comp_batch", bitdepth_max, frame, d_blocks, n, 1, 128, stream, [](auto hbd) { return mc_comp_kernel<hbd>; });
 }
 int b200_mc_blend_batch(int bitdepth_max, const B200McFrame *frame, const B200BlendBlock *d_blocks, int n, void *stream) {
-    if (check_bd(bitdepth_max, "b200_mc_blend_batch")) return -2;
-    if (n <= 0) return 0;
-    if (bitdepth_max > 255) { auto k = mc_blend_kernel<true>; B200_LAUNCH_PDL(k, dim3(n), dim3(128), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    else { auto k = mc_blend_kernel<false>; B200_LAUNCH_PDL(k, dim3(n), dim3(128), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return mc_stage("b200_mc_blend_batch", bitdepth_max, frame, d_blocks, n, 1, 128, stream, [](auto hbd) { return mc_blend_kernel<hbd>; });
 }
 int b200_mc_warp_batch(int bitdepth_max, const B200McFrame *frame, const B200WarpBlock *d_blocks, int n, void *stream) {
-    if (check_bd(bitdepth_max, "b200_mc_warp_batch")) return -2;
-    if (n <= 0) return 0;
-    const int grid = (n + kWarpWarps - 1) / kWarpWarps;
-    if (bitdepth_max > 255) { auto k = mc_warp_kernel<true>; B200_LAUNCH_PDL(k, dim3(grid), dim3(kWarpWarps * 32), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    else { auto k = mc_warp_kernel<false>; B200_LAUNCH_PDL(k, dim3(grid), dim3(kWarpWarps * 32), 0, (cudaStream_t)stream, d_blocks, n, *frame, bitdepth_max); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return mc_stage("b200_mc_warp_batch", bitdepth_max, frame, d_blocks, n, kWarpWarps, kWarpWarps * 32, stream, [](auto hbd) { return mc_warp_kernel<hbd>; });
 }
 
 }  // extern "C"
 
 // ---- Level 1: host pointers -------------------------------------------------------------
-namespace {
-Scratch s_ref, s_dst, s_tmp, s_mask, s_desc, s_px;
-uint8_t h_stage[2 * (128 + 8) * (128 + 8) * 2 + 64];
-}
+enum { REF, DST, TMP, MASK, DESC };   // Level1 scratch slots
 
 static int mc_l1(int op, void *out, ptrdiff_t out_stride, const void *src, ptrdiff_t src_stride, int w, int h,
                  int mx, int my, int f2d, int bdmax)
 {
-    if (check_bd(bdmax, "b200_mc")) return -2;
+    if (int r = check_bdmax(bdmax, "b200_mc")) return r;
     if (f2d < 0 || f2d > 9 || w < 2 || w > 128 || (w & (w - 1)) || h < 2 || h > 128 || mx < 0 || mx > 15 || my < 0 || my > 15) {
         b200_set_error("b200_mc: bad arguments (w=%d h=%d mx=%d my=%d filter=%d)", w, h, mx, my, f2d);
         return -2;
     }
-    std::lock_guard<std::mutex> lk(host_lock());
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
     // the window the reference reads: 3 before / 4 after for 8-tap, 0 / 1 for bilinear, only on filtered axes
     const int bl = f2d == 9 ? 0 : 3, al = f2d == 9 ? 1 : 4;
     const int x0 = mx ? bl : 0, x1 = mx ? al : 0, y0 = my ? bl : 0, y1 = my ? al : 0;
     const int ww = w + x0 + x1, wh = h + y0 + y1;
-    pack_rect(h_stage, (const uint8_t *)src - (ptrdiff_t)y0 * src_stride - (ptrdiff_t)x0 * (ptrdiff_t)px, src_stride, ww, wh, px);
-    if (s_ref.upload(h_stage, (size_t)ww * wh * px)) return -1;
-    if (s_dst.reserve((size_t)w * h * 2) || s_desc.reserve(sizeof(B200McBlock))) return -1;
-    B200McFrame fr;
-    memset(&fr, 0, sizeof(fr));
-    fr.ref[0] = s_ref.p; fr.ref_stride[0] = ww; fr.ref_w[0] = ww; fr.ref_h[0] = wh;
-    fr.dst = s_dst.p; fr.dst_stride[0] = w; fr.tmp = (int16_t *)s_dst.p;
     B200McBlock b;
     memset(&b, 0, sizeof(b));
     b.dst_off = 0; b.src_x = x0; b.src_y = y0; b.w = (uint8_t)w; b.h = (uint8_t)h; b.mx = (uint8_t)mx; b.my = (uint8_t)my;
     b.filter2d = (uint8_t)f2d; b.op = (uint8_t)op;
-    if (s_desc.upload(&b, sizeof(b))) return -1;
-    int r = b200_mc_batch(bdmax, &fr, (const B200McBlock *)s_desc.p, 1, 0);
-    if (r) return r;
-    if (op) {
-        if (s_dst.download(out, (size_t)w * h * 2)) return -1;
-        B200_CUDA_OK(cudaStreamSynchronize(0));
-    } else {
-        static uint8_t h_out[128 * 128 * 2];
-        if (s_dst.download(h_out, (size_t)w * h * px)) return -1;
-        B200_CUDA_OK(cudaStreamSynchronize(0));
-        unpack_rect(out, out_stride, h_out, w, h, px);
-    }
-    return 0;
+    void *ref, *dst, *desc;
+    if (!(ref = L.upload_rect(REF, (const uint8_t *)src - (ptrdiff_t)y0 * src_stride - (ptrdiff_t)x0 * (ptrdiff_t)px, src_stride, ww, wh, px)) ||
+        !(dst = L.dev(DST, (size_t)w * h * 2)) || !(desc = L.upload(DESC, &b, sizeof(b))))
+        return -1;
+    B200McFrame fr;
+    memset(&fr, 0, sizeof(fr));
+    fr.ref[0] = ref; fr.ref_stride[0] = ww; fr.ref_w[0] = ww; fr.ref_h[0] = wh;
+    fr.dst = dst; fr.dst_stride[0] = w; fr.tmp = (int16_t *)dst;
+    if (int r = b200_mc_batch(bdmax, &fr, (const B200McBlock *)desc, 1, 0)) return r;
+    return op ? L.download_rect(DST, out, (ptrdiff_t)w * 2, w, h, 2) : L.download_rect(DST, out, out_stride, w, h, px);
 }
 
 static int mc_scaled_l1(int op, void *out, ptrdiff_t out_stride, const void *src, ptrdiff_t src_stride, int w, int h,
                         int mx, int my, int dx, int dy, int f2d, int bdmax)
 {
-    if (check_bd(bdmax, "b200_mc_scaled")) return -2;
+    if (int r = check_bdmax(bdmax, "b200_mc_scaled")) return r;
     if (f2d < 0 || f2d > 9 || w < 2 || w > 128 || h < 2 || h > 128 || mx < 0 || mx > 1023 || my < 0 || my > 1023 ||
         dx < 1 || dx > 2048 || dy < 1 || dy > 2048) {
         b200_set_error("b200_mc_scaled: bad arguments (w=%d h=%d mx=%d my=%d dx=%d dy=%d filter=%d)", w, h, mx, my, dx, dy, f2d);
         return -2;
     }
-    std::lock_guard<std::mutex> lk(host_lock());
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
     // the window the reference reads (8-tap: 3 before / 4 after the integer position; bilinear: 0 / 1)
     const int bl = f2d == 9 ? 0 : 3, al = f2d == 9 ? 1 : 4;
     const int ww = ((mx + (w - 1) * dx) >> 10) + 1 + bl + al, wh = ((my + (h - 1) * dy) >> 10) + 1 + bl + al;
-    static uint8_t *stage = nullptr; static size_t stage_sz = 0;
-    const size_t need = (size_t)ww * wh * px;
-    if (need > stage_sz) { free(stage); stage = (uint8_t *)malloc(need); stage_sz = stage ? need : 0; if (!stage) { b200_set_error("oom"); return -1; } }
-    pack_rect(stage, (const uint8_t *)src - (ptrdiff_t)bl * src_stride - (ptrdiff_t)bl * (ptrdiff_t)px, src_stride, ww, wh, px);
-    if (s_ref.upload(stage, need)) return -1;
-    if (s_dst.reserve((size_t)w * h * 2)) return -1;
-    B200McFrame fr;
-    memset(&fr, 0, sizeof(fr));
-    fr.ref[0] = s_ref.p; fr.ref_stride[0] = ww; fr.ref_w[0] = ww; fr.ref_h[0] = wh;
-    fr.dst = s_dst.p; fr.dst_stride[0] = w; fr.tmp = (int16_t *)s_dst.p;
     B200McScaledBlock b;
     memset(&b, 0, sizeof(b));
     b.src_x = bl; b.src_y = bl; b.w = (uint8_t)w; b.h = (uint8_t)h; b.mx = (uint16_t)mx; b.my = (uint16_t)my;
     b.dx = (uint16_t)dx; b.dy = (uint16_t)dy; b.filter2d = (uint8_t)f2d; b.op = (uint8_t)op;
-    if (s_desc.upload(&b, sizeof(b))) return -1;
-    int r = b200_mc_scaled_batch(bdmax, &fr, (const B200McScaledBlock *)s_desc.p, 1, 0);
-    if (r) return r;
-    if (op) {
-        if (s_dst.download(out, (size_t)w * h * 2)) return -1;
-        B200_CUDA_OK(cudaStreamSynchronize(0));
-    } else {
-        static uint8_t h_out[128 * 128 * 2];
-        if (s_dst.download(h_out, (size_t)w * h * px)) return -1;
-        B200_CUDA_OK(cudaStreamSynchronize(0));
-        unpack_rect(out, out_stride, h_out, w, h, px);
-    }
-    return 0;
+    void *ref, *dst, *desc;
+    if (!(ref = L.upload_rect(REF, (const uint8_t *)src - (ptrdiff_t)bl * src_stride - (ptrdiff_t)bl * (ptrdiff_t)px, src_stride, ww, wh, px)) ||
+        !(dst = L.dev(DST, (size_t)w * h * 2)) || !(desc = L.upload(DESC, &b, sizeof(b))))
+        return -1;
+    B200McFrame fr;
+    memset(&fr, 0, sizeof(fr));
+    fr.ref[0] = ref; fr.ref_stride[0] = ww; fr.ref_w[0] = ww; fr.ref_h[0] = wh;
+    fr.dst = dst; fr.dst_stride[0] = w; fr.tmp = (int16_t *)dst;
+    if (int r = b200_mc_scaled_batch(bdmax, &fr, (const B200McScaledBlock *)desc, 1, 0)) return r;
+    return op ? L.download_rect(DST, out, (ptrdiff_t)w * 2, w, h, 2) : L.download_rect(DST, out, out_stride, w, h, px);
 }
 
 extern "C" {
@@ -853,123 +796,102 @@ int b200_mc_prep(int16_t *tmp, const void *src, ptrdiff_t src_stride, int w, int
 int b200_mc_comp(void *dst, ptrdiff_t dst_stride, const int16_t *tmp1, const int16_t *tmp2, int w, int h,
                  int op, int param, uint8_t *mask, int bdmax)
 {
-    if (check_bd(bdmax, "b200_mc_comp")) return -2;
+    if (int r = check_bdmax(bdmax, "b200_mc_comp")) return r;
     if (op < 0 || op > B200_COMP_W_MASK_420 || w < 4 || w > 128 || h < 4 || h > 128 || (w & 1) || (op == B200_COMP_W_MASK_420 && (h & 1))) {
         b200_set_error("b200_mc_comp: bad arguments (op=%d w=%d h=%d)", op, w, h);
         return -2;
     }
-    std::lock_guard<std::mutex> lk(host_lock());
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1, n = (size_t)w * h;
-    if (s_tmp.reserve(n * 4) || s_dst.reserve(n * 2) || s_mask.reserve(n) || s_desc.reserve(sizeof(B200CompBlock))) return -1;
-    B200_CUDA_OK(cudaMemcpyAsync(s_tmp.p, tmp1, n * 2, cudaMemcpyHostToDevice, 0));
-    B200_CUDA_OK(cudaMemcpyAsync((int16_t *)s_tmp.p + n, tmp2, n * 2, cudaMemcpyHostToDevice, 0));
-    if (op == B200_COMP_MASK) B200_CUDA_OK(cudaMemcpyAsync(s_mask.p, mask, n, cudaMemcpyHostToDevice, 0));
-    B200McFrame fr;
-    memset(&fr, 0, sizeof(fr));
-    fr.dst = s_dst.p; fr.dst_stride[0] = w; fr.tmp = (int16_t *)s_tmp.p; fr.mask = (uint8_t *)s_mask.p;
     B200CompBlock b;
     memset(&b, 0, sizeof(b));
     b.tmp1_off = 0; b.tmp2_off = (uint32_t)n; b.w = (uint8_t)w; b.h = (uint8_t)h; b.op = (uint8_t)op; b.param = (uint8_t)param;
-    if (s_desc.upload(&b, sizeof(b))) return -1;
-    int r = b200_mc_comp_batch(bdmax, &fr, (const B200CompBlock *)s_desc.p, 1, 0);
-    if (r) return r;
-    static uint8_t h_out[128 * 128 * 2];
-    if (s_dst.download(h_out, n * px)) return -1;
-    if (op >= B200_COMP_W_MASK_444) {
-        const size_t mn = (size_t)(w >> (op != B200_COMP_W_MASK_444)) * (h >> (op == B200_COMP_W_MASK_420));
-        if (s_mask.download(mask, mn)) return -1;
-    }
-    B200_CUDA_OK(cudaStreamSynchronize(0));
-    unpack_rect(dst, dst_stride, h_out, w, h, px);
-    return 0;
+    int16_t *both = (int16_t *)L.host(n * 4);     // tmp1 and tmp2 back to back
+    if (!both) return -1;
+    memcpy(both, tmp1, n * 2);
+    memcpy(both + n, tmp2, n * 2);
+    void *tmp, *out, *m, *desc;
+    if (!(tmp = L.upload(TMP, both, n * 4)) || !(out = L.dev(DST, n * 2)) ||
+        !(m = op == B200_COMP_MASK ? L.upload(MASK, mask, n) : L.dev(MASK, n)) || !(desc = L.upload(DESC, &b, sizeof(b))))
+        return -1;
+    B200McFrame fr;
+    memset(&fr, 0, sizeof(fr));
+    fr.dst = out; fr.dst_stride[0] = w; fr.tmp = (int16_t *)tmp; fr.mask = (uint8_t *)m;
+    if (int r = b200_mc_comp_batch(bdmax, &fr, (const B200CompBlock *)desc, 1, 0)) return r;
+    if (op >= B200_COMP_W_MASK_444 && L.download(MASK, mask, (size_t)(w >> (op != B200_COMP_W_MASK_444)) * (h >> (op == B200_COMP_W_MASK_420))))
+        return -1;
+    return L.download_rect(DST, dst, dst_stride, w, h, px);
 }
 
 int b200_mc_blend(void *dst, ptrdiff_t dst_stride, const void *tmp, int w, int h, int op, const uint8_t *mask, int bdmax)
 {
-    if (check_bd(bdmax, "b200_mc_blend")) return -2;
+    if (int r = check_bdmax(bdmax, "b200_mc_blend")) return r;
     if (op < 0 || op > B200_BLEND_H || w < 1 || w > 128 || h < 1 || h > 128) { b200_set_error("b200_mc_blend: bad arguments"); return -2; }
-    std::lock_guard<std::mutex> lk(host_lock());
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1, n = (size_t)w * h;
-    static uint8_t h_io[128 * 128 * 2];
-    pack_rect(h_io, dst, dst_stride, w, h, px);
-    if (s_dst.upload(h_io, n * px) || s_px.upload(tmp, n * px) || s_desc.reserve(sizeof(B200BlendBlock))) return -1;
-    if (op == B200_BLEND && s_mask.upload(mask, n)) return -1;
-    B200McFrame fr;
-    memset(&fr, 0, sizeof(fr));
-    fr.dst = s_dst.p; fr.dst_stride[0] = w; fr.px_tmp = s_px.p; fr.mask = (uint8_t *)s_mask.p;
     B200BlendBlock b;
     memset(&b, 0, sizeof(b));
     b.w = (uint8_t)w; b.h = (uint8_t)h; b.op = (uint8_t)op;
-    if (s_desc.upload(&b, sizeof(b))) return -1;
-    int r = b200_mc_blend_batch(bdmax, &fr, (const B200BlendBlock *)s_desc.p, 1, 0);
-    if (r) return r;
-    if (s_dst.download(h_io, n * px)) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
-    unpack_rect(dst, dst_stride, h_io, w, h, px);
-    return 0;
+    void *out, *t, *m = nullptr, *desc;
+    if (!(out = L.upload_rect(DST, dst, dst_stride, w, h, px)) || !(t = L.upload(TMP, tmp, n * px)) ||
+        (op == B200_BLEND && !(m = L.upload(MASK, mask, n))) || !(desc = L.upload(DESC, &b, sizeof(b))))
+        return -1;
+    B200McFrame fr;
+    memset(&fr, 0, sizeof(fr));
+    fr.dst = out; fr.dst_stride[0] = w; fr.px_tmp = t; fr.mask = (uint8_t *)m;
+    if (int r = b200_mc_blend_batch(bdmax, &fr, (const B200BlendBlock *)desc, 1, 0)) return r;
+    return L.download_rect(DST, dst, dst_stride, w, h, px);
 }
 
 int b200_mc_warp8x8(int op, void *out, ptrdiff_t out_stride, const void *src, ptrdiff_t src_stride,
                     const int16_t *abcd, int mx, int my, int bdmax)
 {
-    if (check_bd(bdmax, "b200_mc_warp8x8")) return -2;
-    std::lock_guard<std::mutex> lk(host_lock());
+    if (int r = check_bdmax(bdmax, "b200_mc_warp8x8")) return r;
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
-    pack_rect(h_stage, (const uint8_t *)src - 3 * src_stride - 3 * (ptrdiff_t)px, src_stride, 15, 15, px);
-    if (s_ref.upload(h_stage, 15 * 15 * px) || s_dst.reserve(64 * 2) || s_desc.reserve(sizeof(B200WarpBlock))) return -1;
-    B200McFrame fr;
-    memset(&fr, 0, sizeof(fr));
-    fr.ref[0] = s_ref.p; fr.ref_stride[0] = 15; fr.ref_w[0] = 15; fr.ref_h[0] = 15;
-    fr.dst = s_dst.p; fr.dst_stride[0] = 8; fr.tmp = (int16_t *)s_dst.p;
     B200WarpBlock b;
     memset(&b, 0, sizeof(b));
     b.src_x = 3; b.src_y = 3; b.mx = mx; b.my = my; b.op = (uint8_t)op; b.tmp_stride = 8;
     memcpy(b.abcd, abcd, 8);
-    if (s_desc.upload(&b, sizeof(b))) return -1;
-    int r = b200_mc_warp_batch(bdmax, &fr, (const B200WarpBlock *)s_desc.p, 1, 0);
-    if (r) return r;
-    uint8_t h_out[64 * 2];
-    if (s_dst.download(h_out, 64 * (op ? 2 : px))) return -1;
-    B200_CUDA_OK(cudaStreamSynchronize(0));
-    if (op) for (int y = 0; y < 8; y++) memcpy((int16_t *)out + (ptrdiff_t)y * out_stride, h_out + y * 16, 16);
-    else unpack_rect(out, out_stride, h_out, 8, 8, px);
-    return 0;
+    void *ref, *dst, *desc;
+    if (!(ref = L.upload_rect(REF, (const uint8_t *)src - 3 * src_stride - 3 * (ptrdiff_t)px, src_stride, 15, 15, px)) ||
+        !(dst = L.dev(DST, 64 * 2)) || !(desc = L.upload(DESC, &b, sizeof(b))))
+        return -1;
+    B200McFrame fr;
+    memset(&fr, 0, sizeof(fr));
+    fr.ref[0] = ref; fr.ref_stride[0] = 15; fr.ref_w[0] = 15; fr.ref_h[0] = 15;
+    fr.dst = dst; fr.dst_stride[0] = 8; fr.tmp = (int16_t *)dst;
+    if (int r = b200_mc_warp_batch(bdmax, &fr, (const B200WarpBlock *)desc, 1, 0)) return r;
+    return op ? L.download_rect(DST, out, out_stride * 2, 8, 8, 2) : L.download_rect(DST, out, out_stride, 8, 8, px);
 }
 
 int b200_mc_emu_edge(intptr_t bw, intptr_t bh, intptr_t iw, intptr_t ih, intptr_t x, intptr_t y, void *dst,
                      ptrdiff_t dst_stride, const void *ref, ptrdiff_t ref_stride, int bdmax)
 {
-    if (check_bd(bdmax, "b200_mc_emu_edge")) return -2;
+    if (int r = check_bdmax(bdmax, "b200_mc_emu_edge")) return r;
     if (bw < 1 || bh < 1 || iw < 1 || ih < 1 || bw * bh > (1 << 22) || iw * ih > (1 << 26)) { b200_set_error("b200_mc_emu_edge: bad geometry"); return -2; }
-    std::lock_guard<std::mutex> lk(host_lock());
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
     // only the part of the plane the window can touch is shipped: rows/cols clamp(x..x+bw-1)
     const int cx0 = iclip((int)x, 0, (int)iw - 1), cx1 = iclip((int)(x + bw - 1), 0, (int)iw - 1);
     const int cy0 = iclip((int)y, 0, (int)ih - 1), cy1 = iclip((int)(y + bh - 1), 0, (int)ih - 1);
     const int sw = cx1 - cx0 + 1, shh = cy1 - cy0 + 1;
-    uint8_t *stage = (uint8_t *)malloc((size_t)sw * shh * px + (size_t)bw * bh * px);
-    if (!stage) { b200_set_error("oom"); return -1; }
-    pack_rect(stage, (const uint8_t *)ref + (ptrdiff_t)cy0 * ref_stride + (ptrdiff_t)cx0 * (ptrdiff_t)px, ref_stride, sw, shh, px);
-    int rc = -1;
-    do {
-        if (s_ref.upload(stage, (size_t)sw * shh * px) || s_dst.reserve((size_t)bw * bh * px)) break;
-        const int n = (int)(bw * bh), grid = imin((n + 255) / 256, 1184);
-        if (bdmax > 255) { auto k = emu_edge_kernel<true>; B200_LAUNCH(k, dim3(grid), dim3(256), 0, (cudaStream_t)0, (int)bw, (int)bh, sw, shh, (int)x - cx0, (int)y - cy0, (uint16_t *)s_dst.p, (const uint16_t *)s_ref.p); }
-        else { auto k = emu_edge_kernel<false>; B200_LAUNCH(k, dim3(grid), dim3(256), 0, (cudaStream_t)0, (int)bw, (int)bh, sw, shh, (int)x - cx0, (int)y - cy0, (uint8_t *)s_dst.p, (const uint8_t *)s_ref.p); }
-        b200_count_launch();
-        uint8_t *outb = stage + (size_t)sw * shh * px;
-        if (s_dst.download(outb, (size_t)bw * bh * px)) break;
-        if (cudaStreamSynchronize(0) != cudaSuccess) { b200_set_error("sync failed"); break; }
-        unpack_rect(dst, dst_stride, outb, (int)bw, (int)bh, px);
-        rc = 0;
-    } while (0);
-    free(stage);
-    return rc;
+    void *s, *d;
+    if (!(s = L.upload_rect(REF, (const uint8_t *)ref + (ptrdiff_t)cy0 * ref_stride + (ptrdiff_t)cx0 * (ptrdiff_t)px, ref_stride, sw, shh, px)) ||
+        !(d = L.dev(DST, (size_t)bw * bh * px)))
+        return -1;
+    const int n = (int)(bw * bh), grid = imin((n + 255) / 256, 1184);
+    if (int r = launch_hbd(bdmax, Launch::plain, dim3(grid), dim3(256), 0, 0, [&](auto hbd) {
+            typedef typename Bd<hbd>::pixel pixel;
+            return std::make_tuple(emu_edge_kernel<hbd>, (int)bw, (int)bh, sw, shh, (int)x - cx0, (int)y - cy0, (pixel *)d, (const pixel *)s);
+        }))
+        return r;
+    return L.download_rect(DST, dst, dst_stride, (int)bw, (int)bh, px);
 }
 
 int b200_resize_frame(int bitdepth_max, const B200ResizeFrame *fr, void *stream)
 {
-    if (check_bd(bitdepth_max, "b200_resize_frame")) return -2;
+    if (int r = check_bdmax(bitdepth_max, "b200_resize_frame")) return r;
     if (fr->n_planes <= 0) return 0;
     if (fr->n_planes > 3 || !fr->src || !fr->dst) { b200_set_error("b200_resize_frame: bad arguments"); return -2; }
     int most = 0;
@@ -978,38 +900,26 @@ int b200_resize_frame(int bitdepth_max, const B200ResizeFrame *fr, void *stream)
         most = imax(most, fr->dst_w[p] * fr->h[p]);
     }
     const dim3 grid(imin((most + 255) / 256, 8 * kSmCount), fr->n_planes);
-    if (bitdepth_max > 255) { auto k = resize_frame_kernel<true>; B200_LAUNCH_PDL(k, grid, dim3(256), 0, (cudaStream_t)stream, *fr, bitdepth_max); }
-    else { auto k = resize_frame_kernel<false>; B200_LAUNCH_PDL(k, grid, dim3(256), 0, (cudaStream_t)stream, *fr, bitdepth_max); }
-    b200_count_launch();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return launch_hbd(bitdepth_max, Launch::pdl, grid, dim3(256), 0, (cudaStream_t)stream,
+                      [&](auto hbd) { return std::make_tuple(resize_frame_kernel<hbd>, *fr, bitdepth_max); });
 }
 
 int b200_mc_resize(void *dst, ptrdiff_t dst_stride, const void *src, ptrdiff_t src_stride, int dst_w, int h,
                    int src_w, int dx, int mx, int bdmax)
 {
-    if (check_bd(bdmax, "b200_mc_resize")) return -2;
+    if (int r = check_bdmax(bdmax, "b200_mc_resize")) return r;
     if (dst_w < 1 || h < 1 || src_w < 1 || (size_t)dst_w * h > (1u << 26)) { b200_set_error("b200_mc_resize: bad geometry"); return -2; }
-    std::lock_guard<std::mutex> lk(host_lock());
+    Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
-    uint8_t *stage = (uint8_t *)malloc(((size_t)src_w + dst_w) * h * px);
-    if (!stage) { b200_set_error("oom"); return -1; }
-    pack_rect(stage, src, src_stride, src_w, h, px);
-    int rc = -1;
-    do {
-        if (s_ref.upload(stage, (size_t)src_w * h * px) || s_dst.reserve((size_t)dst_w * h * px)) break;
-        const int n = dst_w * h, grid = imin((n + 255) / 256, 1184);
-        if (bdmax > 255) { auto k = resize_kernel<true>; B200_LAUNCH(k, dim3(grid), dim3(256), 0, (cudaStream_t)0, (uint16_t *)s_dst.p, (const uint16_t *)s_ref.p, dst_w, h, src_w, dx, mx, bdmax); }
-        else { auto k = resize_kernel<false>; B200_LAUNCH(k, dim3(grid), dim3(256), 0, (cudaStream_t)0, (uint8_t *)s_dst.p, (const uint8_t *)s_ref.p, dst_w, h, src_w, dx, mx, bdmax); }
-        b200_count_launch();
-        uint8_t *outb = stage + (size_t)src_w * h * px;
-        if (s_dst.download(outb, (size_t)dst_w * h * px)) break;
-        if (cudaStreamSynchronize(0) != cudaSuccess) { b200_set_error("sync failed"); break; }
-        unpack_rect(dst, dst_stride, outb, dst_w, h, px);
-        rc = 0;
-    } while (0);
-    free(stage);
-    return rc;
+    void *s, *d;
+    if (!(s = L.upload_rect(REF, src, src_stride, src_w, h, px)) || !(d = L.dev(DST, (size_t)dst_w * h * px))) return -1;
+    const int n = dst_w * h, grid = imin((n + 255) / 256, 1184);
+    if (int r = launch_hbd(bdmax, Launch::plain, dim3(grid), dim3(256), 0, 0, [&](auto hbd) {
+            typedef typename Bd<hbd>::pixel pixel;
+            return std::make_tuple(resize_kernel<hbd>, (pixel *)d, (const pixel *)s, dst_w, h, src_w, dx, mx, bdmax);
+        }))
+        return r;
+    return L.download_rect(DST, dst, dst_stride, dst_w, h, px);
 }
 
 }  // extern "C"
