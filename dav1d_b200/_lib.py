@@ -171,7 +171,7 @@ class FrameBand(C.Structure):
     """struct B200FrameBand"""
     _fields_ = [("y0", C.c_int32), ("y1", C.c_int32), ("last", C.c_int32), ("pad", C.c_int32)] + \
                [(n, C.c_int32 * 2) for n in ("pred", "warp", "comp", "comp2", "blend", "blend2", "scaled", "cfused", "cfused2", "expand")] + \
-               [("itx", (C.c_int32 * 2) * 19)]
+               [("itx", (C.c_int32 * 2) * 19), ("intra", C.c_int32 * 2), ("intra_edge", C.c_void_p)]
 
 
 class PutRange(C.Structure):
@@ -279,6 +279,7 @@ _SIGS = {
     "b200_frame_run_band": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_frame_run_band_phase": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "b200_band_progress": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int]),
+    "b200_band_edge_bytes": (C.c_size_t, [C.c_void_p]),
     "b200_ipc_export": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_ipc_open": (C.c_void_p, [C.c_void_p]),
     "b200_ipc_close": (C.c_int, [C.c_void_p]),

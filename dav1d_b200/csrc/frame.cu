@@ -14,7 +14,7 @@ static B200FrameBand whole_band(const B200FrameJob *j)
     b.y1 = job_luma_h(j); b.last = 1;
     b.pred[1] = j->n_pred; b.warp[1] = j->n_warp; b.comp[1] = j->n_comp; b.comp2[1] = j->n_comp2; b.blend[1] = j->n_blend;
     b.blend2[1] = j->n_blend2; b.scaled[1] = j->n_scaled; b.cfused[1] = j->n_cfused; b.cfused2[1] = j->n_cfused2;
-    b.expand[1] = j->n_expand;
+    b.expand[1] = j->n_expand; b.intra[1] = j->n_intra;
     for (int t = 0; t < B200_N_RECT_TX_SIZES; t++) b.itx[t][1] = j->n_itx[t];
     return b;
 }
@@ -105,7 +105,13 @@ static int run_band(const B200FrameJob *j, const B200FrameBand *b, int phases, v
     if ((phases & B200_BAND_POST) && b->y0 == 0 && j->run_fg && (r = fg_fork(j, stream))) return r;
     if (phases & B200_BAND_RECON) {
         if ((r = band_recon(j, b, stream))) return r;
-        if (j->n_intra > 0 && (r = b200_intra_frame(j->bitdepth_max, &j->intra, j->d_intra, j->n_intra, stream))) return r;
+        if (j->n_intra > 0) {
+            const int bd = j->bitdepth_max;
+            const cudaStream_t st = (cudaStream_t)stream;
+            if ((r = b200::intra_band(bd, &j->intra, j->d_intra + b->intra[0], b->intra[1], b->y0, b->intra_edge, st))) return r;
+            // the next band's intra records read this band's bottom rows as they are now, before the post filters change them
+            if (!b->last && (r = b200::intra_edge_save(bd, &j->intra, b->y1, b->intra_edge, st))) return r;
+        }
     }
     return (phases & B200_BAND_POST) ? band_post(j, b, stream) : 0;
 }
@@ -167,10 +173,23 @@ int b200_frame_run_band_phase(const B200FrameJob *j, const B200FrameBand *b, int
         b200_set_error("b200_frame_run_band: band [%d, %d) must be 64-row aligned (last band: down to the picture height %d)", b->y0, b->y1, H);
         return -2;
     }
-    // intra records form a dependency graph over the whole frame: they run with a band only when that band IS the frame
-    if (j->n_intra > 0 && !(b->y0 == 0 && b->last)) { b200_set_error("b200_frame_run_band: intra records are not band-sliced (one band, or b200_frame_run)"); return -2; }
+    if (b->intra[0] < 0 || b->intra[1] < 0 || b->intra[1] > j->n_intra - b->intra[0]) {
+        b200_set_error("b200_frame_run_band: intra range [%d, +%d) outside the job's %d intra records", b->intra[0], b->intra[1], j->n_intra);
+        return -2;
+    }
+    if (j->n_intra > 0 && !(b->y0 == 0 && b->last)) {
+        if (j->intra.sb) { b200_set_error("b200_frame_run_band: superblock-mode intra is not band-sliced (one band, or b200_frame_run)"); return -2; }
+        if (!b->intra_edge) { b200_set_error("b200_frame_run_band: a band of a job with intra records needs intra_edge (b200_band_edge_bytes)"); return -2; }
+    }
     if (j->run_resize) { b200_set_error("b200_frame_run_band: the super-resolution stage is not band-sliced (b200_frame_run)"); return -2; }
     return run_band(j, b, phases, stream);
+}
+
+size_t b200_band_edge_bytes(const B200FrameJob *j)
+{
+    const size_t boundaries = (size_t)((job_luma_h(j) - 1) / 64);          // luma rows 64, 128, ... inside the picture
+    const B200IntraFrame &f = j->intra;
+    return boundaries * (size_t)(f.stride[0] + f.stride[1] + f.stride[2]) * (j->bitdepth_max > 255 ? 2 : 1);
 }
 
 // ---- cross-GPU exchange primitives -------------------------------------------------------------------------------

@@ -47,6 +47,11 @@ int launch_hbd(int bdmax, Launch mode, dim3 grid, dim3 block, size_t smem, cudaS
 int lf_frame_rows(int bdmax, const B200LfFrame *f, int ya4, int yb4, cudaStream_t stream);
 int cdef_frame_rows(int bdmax, const B200CdefFrame *f, int t0, int t1, cudaStream_t stream);
 int lr_frame_rows(int bdmax, const B200LrFrame *f, int r0, int r1, cudaStream_t stream);
+// band-sliced intra (intra.cu): the n records at d_tx of the band starting at luma row y0 (the band at y0 = 0 initialises the
+// done map, records on a later band's first row read the row above from `edge`); and the copy of the rows above luma row
+// y1 into `edge` at the end of a band's reconstruction
+int intra_band(int bdmax, const B200IntraFrame *f, const B200IntraTx *d_tx, int n, int y0, const void *edge, cudaStream_t stream);
+int intra_edge_save(int bdmax, const B200IntraFrame *f, int y1, void *edge, cudaStream_t stream);
 
 [[noreturn]] inline void die(const char *what) {
     fprintf(stderr, "b200av1: %s failed: %s\n", what, b200_last_error());

@@ -66,8 +66,24 @@ struct IntraParams {
 // several independent frames per launch (blockIdx.y = frame): frames are the parallel axis of intra decoding and
 // one launch is not limited by the number of hardware work queues the way one stream per frame is
 constexpr int kIntraMaxBatch = 24;
-struct IntraBatch { IntraParams p[kIntraMaxBatch]; };
+// A band of a frame job (one frame per launch): the records on the band's first row read the row above from the copy the
+// previous band's reconstruction saved (intra_edge_save), because the previous band's post filters may already have
+// rewritten it in the picture. rows == nullptr: every record reads the picture.
+struct IntraBandEdge {
+    const void *rows;       // saved rows of the band's top boundary: luma, then the two chroma planes, stride[p] pixels each
+    int32_t y0, pad;        // luma row of the band's top
+};
+struct IntraBatch { IntraParams p[kIntraMaxBatch]; IntraBandEdge band; };
 static_assert(sizeof(IntraBatch) <= 4080, "kernel parameter space (4 KB with the trailing int)");
+
+// the row above a block: in the picture, or in the saved edge when the block sits on the band's first row
+template <class pixel>
+B200_DEV const pixel *intra_top_row(const IntraBandEdge &band, const IntraFrameDev &f, const pixel *dst, int pl, int x4, int y4, bool have_top)
+{
+    if (band.rows && have_top && y4 * 4 == (band.y0 >> (pl ? f.ss_ver : 0)))
+        return (const pixel *)band.rows + (pl ? f.stride[0] : 0) + (pl > 1 ? f.stride[1] : 0) + x4 * 4;
+    return dst - f.stride[pl];
+}
 
 B200_DEV int ld_cell(const uint8_t *p) { return *(const volatile uint8_t *)p; }
 // a dependency that never arrives (records not in a topological order) must not hang the GPU: fail the launch
@@ -256,7 +272,7 @@ __global__ void __launch_bounds__(kIpT, B200_INTRA_MINB) intra_frame_kernel(cons
         }
         // ---- edge gather (every part is filled; the predictors read only what the reference fills)
         {
-            const pixel *const top = dst - st;
+            const pixel *const top = intra_top_row(B.band, f, (const pixel *)dst, pl, x, y, have_top);
             const int half = (1 << bitdepth) >> 1;
             const int lpx = imin(h, (ye - y) << 2), lpx2 = imin(h, (ye - y - th) << 2);
             const int tpx = imin(w, (xe - x) << 2), tpx2 = imin(w, (xe - x - tw) << 2);
@@ -527,7 +543,7 @@ __global__ void __launch_bounds__(kIwWarps * 32) intra_warp_kernel(const __grid_
         }
         // ---- edge gather (every part is filled; the predictors read only what the reference fills)
         if (!is_resid && !is_pal && !is_ibc) {
-            const pixel *const top = dst - st;
+            const pixel *const top = intra_top_row(B.band, f, (const pixel *)dst, pl, x, y, have_top);
             const int half = (1 << bitdepth) >> 1;
             const int lpx = imin(h, (ye - y) << 2), lpx2 = imin(h, (ye - y - th) << 2);
             const int tpx = imin(w, (xe - x) << 2), tpx2 = imin(w, (xe - x - tw) << 2);
@@ -854,6 +870,74 @@ __global__ void __launch_bounds__(kIpT, B200_INTRA_SB_MINB) intra_sb_kernel(cons
     }
 }
 
+// ---- saved intra edge of a band boundary ---------------------------------------------------------------------
+// The last row of each plane of a band, copied at the end of the band's reconstruction (before any post filter of the
+// band can run) into the slot of the boundary below it: what intra_top_row reads for the next band's first row.
+struct EdgeSaveArgs {
+    const void *pic;
+    void *slot;
+    uint32_t src_off[3], dst_off[3];      // pixels
+    int32_t n[3];                         // pixels per row
+};
+constexpr int kEdgeSaveThreads = 256;
+template <bool HBD>
+__global__ void __launch_bounds__(kEdgeSaveThreads) intra_edge_save_kernel(const __grid_constant__ EdgeSaveArgs a)
+{
+    typedef typename Bd<HBD>::pixel pixel;
+    const int tid = blockIdx.x * kEdgeSaveThreads + threadIdx.x, nt = gridDim.x * kEdgeSaveThreads;
+    for (int p = 0; p < 3; p++) {
+        const pixel *src = (const pixel *)a.pic + a.src_off[p];
+        pixel *dst = (pixel *)a.slot + a.dst_off[p];
+        for (int i = tid; i < a.n[p]; i += nt) dst[i] = src[i];
+    }
+}
+
+int intra_launch(int bdmax, const B200IntraFrame *frames, const B200IntraTx *const *d_tx, const int32_t *n_tx,
+                 int n_frames, const IntraBandEdge *band, void *stream);
+
+// the bytes of one boundary's slot in a job's edge buffer (slot k - 1 holds the rows above luma row 64 k): stride[0] +
+// stride[1] + stride[2] pixels
+static size_t edge_slot_bytes(const B200IntraFrame *f, int bdmax)
+{
+    return (size_t)(f->stride[0] + f->stride[1] + f->stride[2]) * (bdmax > 255 ? 2 : 1);
+}
+
+int intra_band(int bdmax, const B200IntraFrame *f, const B200IntraTx *d_tx, int n, int y0, const void *edge, cudaStream_t stream)
+{
+    if (y0 == 0 && n <= 0) {            // the first band initialises the done map even when it has no record of its own
+        if (int r = check_bdmax(bdmax, "b200_frame_run_band")) return r;
+        const IntraScratch L = intra_scratch_layout(f);
+        if (f->done_init) B200_CUDA_OK(cudaMemcpyAsync(f->scratch, f->done_init, L.total, cudaMemcpyDeviceToDevice, stream));
+        else B200_CUDA_OK(cudaMemsetAsync(f->scratch, 0, L.total, stream));
+        return 0;
+    }
+    if (n <= 0) return 0;
+    IntraBandEdge band;
+    band.rows = y0 > 0 ? (const uint8_t *)edge + (size_t)(y0 / 64 - 1) * edge_slot_bytes(f, bdmax) : nullptr;
+    band.y0 = y0; band.pad = 0;
+    const int32_t nn = n;
+    return intra_launch(bdmax, f, &d_tx, &nn, 1, &band, stream);
+}
+
+int intra_edge_save(int bdmax, const B200IntraFrame *f, int y1, void *edge, cudaStream_t stream)
+{
+    EdgeSaveArgs a;
+    memset(&a, 0, sizeof(a));
+    a.pic = f->pic;
+    a.slot = (uint8_t *)edge + (size_t)(y1 / 64 - 1) * edge_slot_bytes(f, bdmax);
+    int widest = 0;
+    for (int p = 0; p < 3; p++) {
+        const int row = (y1 >> (p ? f->ss_ver : 0)) - 1;
+        a.src_off[p] = f->plane_off[p] + (uint32_t)row * f->stride[p];
+        a.dst_off[p] = p ? f->stride[0] + (p > 1 ? f->stride[1] : 0) : 0;
+        a.n[p] = f->h4[p] > 0 ? imin(f->w4[p] * 4, f->stride[p]) : 0;
+        widest = imax(widest, a.n[p]);
+    }
+    const int grid = imax(1, (widest + kEdgeSaveThreads - 1) / kEdgeSaveThreads);
+    return launch_hbd(bdmax, Launch::plain, dim3(grid), dim3(kEdgeSaveThreads), 0, stream,
+                      [&](auto hbd) { return std::make_tuple(intra_edge_save_kernel<hbd>, a); });
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -875,6 +959,23 @@ static size_t intra_canvas_bytes(const B200IntraFrame *f, size_t px)
 int b200_intra_frames(int bdmax, const B200IntraFrame *frames, const B200IntraTx *const *d_tx, const int32_t *n_tx,
                       int n_frames, void *stream)
 {
+    return intra_launch(bdmax, frames, d_tx, n_tx, n_frames, nullptr, stream);
+}
+
+int b200_intra_frame(int bdmax, const B200IntraFrame *f, const B200IntraTx *d_tx, int n, void *stream)
+{
+    if (n <= 0) return 0;
+    const int32_t nn = n;
+    return b200_intra_frames(bdmax, f, &d_tx, &nn, 1, stream);
+}
+
+}  // extern "C"
+
+// band == nullptr: whole frames. Otherwise one frame, a band of it: a band below the first one keeps the done map that the
+// bands above it left and only resets the ticket counter.
+int b200::intra_launch(int bdmax, const B200IntraFrame *frames, const B200IntraTx *const *d_tx, const int32_t *n_tx,
+                       int n_frames, const IntraBandEdge *band, void *stream)
+{
     if (int r = check_bdmax(bdmax, "b200_intra_frames")) return r;
     const size_t px = bdmax > 255 ? 2 : 1;
     static const bool use_cta_kernel = getenv("B200_INTRA_CTA") != nullptr;      // round-1 CTA-per-block kernel (A/B measurements)
@@ -882,6 +983,7 @@ int b200_intra_frames(int bdmax, const B200IntraFrame *frames, const B200IntraTx
     for (int base = 0; base < n_frames; ) {
         IntraBatch B;
         memset(&B, 0, sizeof(B));
+        if (band) B.band = *band;
         int nb = 0, grid = 0, i = base;
         size_t dyn = 0;
         for (; i < n_frames && nb < kIntraMaxBatch; i++) {
@@ -899,7 +1001,9 @@ int b200_intra_frames(int bdmax, const B200IntraFrame *frames, const B200IntraTx
             uint8_t *base_p = (uint8_t *)f->scratch;
             P.scratch = base_p;
             for (int p = 0; p < 3; p++) P.done_off[p] = (uint32_t)L.done_off[p];
-            if (!mode && f->done_init)
+            if (band && band->y0 > 0)
+                B200_CUDA_OK(cudaMemsetAsync(base_p, 0, 256, (cudaStream_t)stream));
+            else if (!mode && f->done_init)
                 B200_CUDA_OK(cudaMemcpyAsync(base_p, f->done_init, L.total, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
             else
                 B200_CUDA_OK(cudaMemsetAsync(base_p, 0, mode ? 256 + (size_t)f->sb_w * f->sb_h : L.total, (cudaStream_t)stream));
@@ -945,12 +1049,3 @@ int b200_intra_frames(int bdmax, const B200IntraFrame *frames, const B200IntraTx
     }
     return 0;
 }
-
-int b200_intra_frame(int bdmax, const B200IntraFrame *f, const B200IntraTx *d_tx, int n, void *stream)
-{
-    if (n <= 0) return 0;
-    const int32_t nn = n;
-    return b200_intra_frames(bdmax, f, &d_tx, &nn, 1, stream);
-}
-
-}  // extern "C"

@@ -78,7 +78,8 @@ def band_plan(S, band_rows, compact=False, fused=False):
     order is kept inside a band), bands = list of dicts {y0, y1, last, <record list>: (first, count)} and need[k][ref] =
     (luma rows, chroma rows) of reference `ref` that band k's predictions read — the `lowest_pixel` of dav1d's
     check_tile (reference src/thread_task.c:415, src/decode.c lowest_pixel bookkeeping); expand = the compact coefficient
-    stream and its band-sorted B200CoefBlock records when `compact`."""
+    stream and its band-sorted B200CoefBlock records when `compact`. Intra records (S["intra_tx"]) are sorted by band too
+    (bands[k]["intra"]); see check_intra_bands for what they may read."""
     assert band_rows % 64 == 0 and band_rows > 0
     H, off, stride = S["H"], S["off"], S["stride"]
     ssv = [0, S["ss_ver"], S["ss_ver"]]
@@ -142,16 +143,26 @@ def band_plan(S, band_rows, compact=False, fused=False):
         a = S["itx"][tx]
         S2["itx"][tx], f, c, _ = sort_by_band(a, luma_y(a["dst_off"], a["plane"]) if len(a) else np.zeros(0, np.int64))
         itx_ranges[tx] = (f, c)
+    # intra-machine records (intra, CFL, palette, inter-intra, intra block copy) by the luma row of their top: the stable sort
+    # keeps the wavefront order, so the records of every band stay in a topological order
+    iband = None
+    it = S.get("intra_tx")
+    if it is not None and len(it):
+        S2["intra_tx"], f, c, iband = sort_by_band(it, luma_y(it["dst_off"], it["plane"]))
+        ranges["intra"] = (f, c)
+        check_intra_bands(S, S2["intra_tx"], iband, band_rows, nb)
     expand = None
     if compact:
         from . import synth
         cc, ex = synth.compact_coefs(S2)
         # compact_coefs emits its records size class after size class, each in the (band-sorted) order of S2["itx"][tx]
         per_tx = [np.repeat(np.arange(nb), itx_ranges[tx][1]) for tx in range(19) if len(S2["itx"][tx])]       # empty: every inter block skipped
-        eb = np.concatenate(per_tx) if per_tx else np.zeros(0, np.int64)
-        # ... followed by the intra records' blocks (mixed frames: a single band only, see b200_frame_run_band)
-        assert len(eb) == len(ex) or (nb == 1 and len(eb) < len(ex))
-        eb = np.concatenate([eb, np.zeros(len(ex) - len(eb), np.int64)]).astype(np.int64)
+        # ... followed by the coded intra records, size class after size class, in the (band-sorted) order of S2["intra_tx"]
+        if iband is not None:
+            it2 = S2["intra_tx"]
+            per_tx += [iband[(it2["tx"] == tx) & (it2["eob"] >= 0)] for tx in range(19)]
+        eb = np.concatenate(per_tx).astype(np.int64) if per_tx else np.zeros(0, np.int64)
+        assert len(eb) == len(ex)
         order = np.argsort(eb, kind="stable")
         cnt = np.bincount(eb, minlength=nb)
         expand = (cc, ex[order])
@@ -174,6 +185,35 @@ def band_plan(S, band_rows, compact=False, fused=False):
     ph = [H, (H + ssv[1]) >> ssv[1]]
     need[:, :, 0] = np.minimum(need[:, :, 0], ph[0]); need[:, :, 1] = np.minimum(need[:, :, 1], ph[1])
     return S2, bands, need, expand
+
+
+def check_intra_bands(S, tx, band, band_rows, nb):
+    """No intra record of a band may read a row at or below the band's bottom: those rows are reconstructed by a later
+    band, so the intra kernel would wait for their cells forever (or, for cells of inter blocks, which the done map marks
+    final from the start, read pixels that are not there yet). Checks the cells the kernel waits for: bottom-left edges,
+    intra block copy sources and the luma blocks of CFL records. The bottom band reads nothing below itself."""
+    from . import levels as L, synth
+    if nb == 1 or not len(tx):
+        return
+    ssv = np.where(tx["plane"] > 0, S["ss_ver"], 0).astype(np.int64)
+    th = (np.asarray(L.TX_H)[tx["tx"]] // 4).astype(np.int64)
+    y, ye = tx["y4"].astype(np.int64), tx["yend4"].astype(np.int64)
+    h4 = np.where(tx["plane"] > 0, S["h4"] >> S["ss_ver"], S["h4"])
+    mode, fl = tx["mode"], tx["flags"].astype(np.int64)
+    reach = y + th                                                   # end of the rows read, plane 4-sample units
+    edges = (mode != synth.MODE_RESID) & (mode != synth.MODE_IBC)
+    bl = edges & ((fl & 9) == 9) & (y + th < ye)                    # HAVE_LEFT | LEFT_HAS_BOTTOM
+    reach = np.where(bl, y + th + np.minimum(th, ye - y - th), reach)
+    ibc = mode == synth.MODE_IBC
+    sy = (tx["luma_off"] >> 16).astype(np.int64)
+    reach = np.where(ibc, np.minimum((sy + 4 * th - 1 + (tx["cfl_h_pad"] != 0)) >> 2, h4 - 1) + 1, reach)
+    cfl = (mode == synth.MODE_CFL) & (tx["cfl_alpha"] != 0)          # CFL: end of the luma block, luma 4-sample units
+    ly4 = y << ssv
+    lum = np.where(cfl, ly4 + np.minimum((th - tx["cfl_h_pad"].astype(np.int64)) << ssv, S["h4"] - ly4), 0)
+    y1 = (band + 1) * band_rows
+    bad = (band < nb - 1) & (((reach * 4) << ssv > y1) | (lum * 4 > y1))
+    assert not bad.any(), "intra record %d (plane %d, y4 %d, mode %d) reads rows below its band [.., %d)" % (
+        int(np.argmax(bad)), int(tx["plane"][bad][0]), int(y[bad][0]), int(mode[bad][0]), int(y1[bad][0]))
 
 
 def run_batch(fbs, stream=None):
@@ -229,7 +269,7 @@ class FrameBuffers:
             for k, b in enumerate(plan):
                 fbn = self.bands[k]
                 fbn.y0, fbn.y1, fbn.last = b["y0"], b["y1"], b["last"]
-                for name in ("pred", "warp", "comp", "comp2", "blend", "blend2", "cfused", "cfused2", "expand"):
+                for name in ("pred", "warp", "comp", "comp2", "blend", "blend2", "cfused", "cfused2", "expand", "intra"):
                     if name in b:
                         getattr(fbn, name)[0], getattr(fbn, name)[1] = b[name]
                 for tx in range(19):
@@ -306,6 +346,7 @@ class FrameBuffers:
             for p in range(3):
                 it.stride[p] = S["stride"][p]
                 it.w4[p] = S["w4"] >> ssh[p]; it.h4[p] = S["h4"] >> ssv[p]
+                it.plane_off[p] = S["off"][p]
             nb = self.lib.b200_intra_scratch_bytes(C.byref(it)) if hasattr(self.lib, "b200_intra_scratch_bytes") else 1 << 22
             it.scratch = zeros("intra_scratch", nb)
             if intra_sb:     # superblock-granular schedule (records grouped by 64x64 superblock)
@@ -314,8 +355,6 @@ class FrameBuffers:
                 it.sb = up("intra_sb", S["intra_sb"]); it.n_sb = len(S["intra_sb"])
                 it.sb_w, it.sb_h = S["intra_sb_grid"]
                 self.uploads.append(("intra_sb", S["intra_sb"]))
-                for p in range(3):
-                    it.plane_off[p] = S["off"][p]
             else:
                 j.d_intra = up("intra_tx", S["intra_tx"]); j.n_intra = len(S["intra_tx"])
                 self.uploads.append(("intra_tx", S["intra_tx"]))
@@ -355,6 +394,11 @@ class FrameBuffers:
         lr.unit_size_log2[0], lr.unit_size_log2[1] = S["us"]
         lr.restore_planes, lr.lr_mask = S["rp"], d_lrm
         self.out_name = "p2" if run_lr else ("p1" if run_cdef else "p0")
+        if self.bands is not None and len(self.bands) > 1 and j.n_intra:
+            # the pre-filter bottom rows of the bands, which the first row of intra records of the next band reads
+            edge = zeros("intra_edge", self.lib.b200_band_edge_bytes(C.byref(j)))
+            for b in self.bands:
+                b.intra_edge = edge
         n_fg = 0
         self.ref_name = self.out_name          # the picture later frames predict from (never the grained copy)
         if S.get("fg") is not None:

@@ -6,6 +6,8 @@ src/picture.h:52-63). Here a frame job is cut into horizontal bands (b200_frame_
 producer PUTS the rows that became final into the consumers' landing buffers over NVLink peer memory and raises their
 progress flag; the consumer's stream waits for exactly the flag value its band needs. No collective, no host
 synchronisation on the data path; `torch.distributed` only exchanges the IPC handles (and carries the CPU tests).
+Frames with intra blocks (mixed inter frames, key frames) are banded like pure inter frames: FrameBuffers(band_rows=...) gives
+their bands the buffer in which each band saves its pre-filter bottom rows for the next band's intra prediction.
 
     PeerExchange   CUDA IPC peer pointers + copy engine puts + stream-ordered flags (the product path on GPUs)
     DistExchange   the same schedule over torch.distributed isend / recv (gloo, in the CPU tests on the host emulator)

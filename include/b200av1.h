@@ -546,7 +546,7 @@ typedef struct B200IntraFrame {
     int32_t zero_coefs;
     int32_t grid;                  /* CTAs to launch; 0 = default */
     void *scratch;                 /* device, >= b200_intra_scratch_bytes(frame) */
-    uint32_t plane_off[3];         /* superblock mode: sample offset of each plane in pic */
+    uint32_t plane_off[3];         /* sample offset of each plane in pic: superblock mode, band-sliced jobs (B200FrameBand) */
     int32_t n_sb, sb_w, sb_h;      /* superblock mode: number of B200IntraSb, superblock grid */
     const B200IntraSb *sb;         /* device; NULL = per-transform-block dataflow */
     const uint8_t *mask;           /* device or NULL: blend masks of B200_INTRA_MODE_II records (per-transform-block mode only) */
@@ -654,7 +654,21 @@ B200_API int b200_struct_size(int which);
  *       CDEF tile rows (32 luma rows) below y1 - 32, loop-restoration tile rows whose stripe ends at or above y1 - 8,
  *     and, for the last band, everything down to the bottom edge + film grain.
  * After band k the restored picture is final down to b200_band_progress(): the rows a dependent frame may predict from.
- * Bands must be run in order, top to bottom, on one stream; the result is bit-identical to b200_frame_run. */
+ * Bands must be run in order, top to bottom, on one stream; the result is bit-identical to b200_frame_run.
+ *
+ * Intra records (job->d_intra: intra, filter-intra, CFL, palette, inter-intra, intra block copy) are band-sliced too.
+ * Intra prediction reads the UNFILTERED reconstruction of the row above a block, but the post filters of band k may run
+ * before or beside the reconstruction of band k+1 and rewrite band k's bottom rows. So, like dav1d's saved intra edge
+ * (backup_ipred_edge / f->ipred_edge, reference src/recon_tmpl.c `top_sb_edge`), the end of every band's RECON phase
+ * but the last copies the band's bottom row of each plane into `intra_edge`, and the records on the first row of the
+ * next band read their top, top-right and top-left pixels from that copy. Rules for banded intra jobs:
+ *   - band.intra = [first, count) of job->d_intra; the records of a band must be in a topological order, and no record may
+ *     read a row at or below its band's y1 (bottom-left edges, intra block copy sources, CFL luma blocks);
+ *   - the RECON phases of a job's bands run in order on one stream (the first band, y0 = 0, initialises the done map);
+ *   - job->intra.plane_off must be set (the edge copy addresses the planes with it);
+ *   - superblock-mode intra (B200IntraFrame.sb) is not band-sliced (one band that is the whole frame, or b200_frame_run);
+ *   - jobs with intra block copy must have deblock, CDEF and loop restoration off, as AV1 requires (a copy reads rows of
+ *     earlier bands from the picture, not from the saved edge). */
 typedef struct B200FrameBand {
     int32_t y0, y1;                 /* luma rows reconstructed by this band */
     int32_t last;                   /* 1: bottom band (y1 = picture height; sweeps run to the bottom edge) */
@@ -662,7 +676,13 @@ typedef struct B200FrameBand {
     /* [first, count) of the job's record arrays that belong to this band */
     int32_t pred[2], warp[2], comp[2], comp2[2], blend[2], blend2[2], scaled[2], cfused[2], cfused2[2], expand[2];
     int32_t itx[B200_N_RECT_TX_SIZES][2];
+    int32_t intra[2];               /* [first, count) of job->d_intra that belong to this band */
+    void *intra_edge;               /* device, >= b200_band_edge_bytes(job): pre-filter bottom rows of the bands, one buffer
+                                       shared by every band of the job (may be NULL when the band is the whole frame) */
 } B200FrameBand;
+/* bytes of B200FrameBand.intra_edge for a job: one saved row per plane (the plane's stride in pixels) per 64-row band
+ * boundary inside the picture */
+B200_API size_t b200_band_edge_bytes(const B200FrameJob *job);
 B200_API int b200_frame_run_band(const B200FrameJob *job, const B200FrameBand *band, void *stream);
 /* The two halves of a band for callers that pipeline them on two streams: B200_BAND_RECON = coefficient expansion,
  * prediction, compound, blends, transforms (reads the references, writes the band's rows of the reconstruction);

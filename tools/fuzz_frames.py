@@ -2,7 +2,8 @@
 """Fuzz the frame job against the oracle on the CPU: random synthetic frames (dav1d_b200/synth.py: bit depth, chroma layout, frame
 size, compound / skip / intra / OBMC / warp / inter-intra rates, film grain; intra-only frames with intra block copy) through the
 host-emulator build of the CUDA sources — whole-frame job, compact coefficient upload, fused compound prediction, band-sliced
-execution with random band heights — compared with oracle/*.c stage by stage (tests/test_frame.py::check_frame).
+execution with random band heights (inter, mixed and intra-only frames; bands in order or with the reconstruction of the next
+band before the post filters of the previous one) — compared with oracle/*.c stage by stage (tests/test_frame.py::check_frame).
 usage: tools/fuzz_frames.py [n_frames] [first_seed]"""
 import os
 import sys
@@ -16,6 +17,19 @@ import refs                                   # noqa: E402
 from dav1d_b200 import frame, synth           # noqa: E402
 import test_frame as TF                       # noqa: E402
 import test_intra as TI                       # noqa: E402
+
+
+def run_banded(fb, interleave):
+    """band after band, or RECON 0, RECON 1, POST 0, RECON 2, POST 1, ... (the reconstruction of band k+1 before the post
+    filters of band k, as the two-stream frame pipeline may run them)"""
+    if not interleave:
+        return fb.run_bands()
+    n = fb.n_bands()
+    fb.run_band_phase(0, 1)
+    for k in range(n):
+        if k + 1 < n:
+            fb.run_band_phase(k + 1, 1)
+        fb.run_band_phase(k, 2)
 
 
 def main():
@@ -34,6 +48,12 @@ def main():
                 got = TI.run_lib(lib, frame.NumpyAlloc(), S, order=str(rng.choice(["intra_tx", "intra_tx_decode_order"])), compact=bool(rng.integers(0, 2)))
                 ok, where = TI.planes_equal(S, exp, got)
                 assert ok, where
+                # ... and band by band (filters off, as intra block copy requires): random band height, band or phase order
+                fb = frame.FrameBuffers(S, lib=lib, alloc=frame.NumpyAlloc(), run_lf=False, run_cdef=False, run_lr=False,
+                                        band_rows=64 * int(rng.integers(1, 4)), compact=bool(rng.integers(0, 2)))
+                run_banded(fb, bool(rng.integers(0, 2)))
+                ok, where = TI.planes_equal(S, exp, fb.output("p0"))
+                assert ok, ("bands", where)
                 kind = "intra"
             else:
                 mixed = rng.random() < 0.5
@@ -43,14 +63,12 @@ def main():
                               p_ii=float(rng.choice([0, 0.2])))
                 S = synth.make_inter_frame(rng, bpc, W, H, ssh, ssv, **kw)
                 exp = TF.oracle_frame(S)
-                has_intra = S.get("intra_tx") is not None and len(S["intra_tx"]) > 0
                 whole = -(-H // 64) * 64
-                variants = [dict(), dict(compact=True), dict(fused=True), dict(band_rows=whole, compact=True)]
-                if not has_intra:
-                    variants += [dict(band_rows=64 * int(rng.integers(1, 4)), compact=bool(rng.integers(0, 2)), fused=bool(rng.integers(0, 2)))]
+                variants = [dict(), dict(compact=True), dict(fused=True), dict(band_rows=whole, compact=True),
+                            dict(band_rows=64 * int(rng.integers(1, 4)), compact=bool(rng.integers(0, 2)), fused=bool(rng.integers(0, 2)))]
                 for v in variants:
                     fb = frame.FrameBuffers(S, lib=lib, alloc=frame.NumpyAlloc(), **v)
-                    fb.run_bands() if v.get("band_rows") else fb.run()
+                    run_banded(fb, bool(rng.integers(0, 2))) if v.get("band_rows") else fb.run()
                     TF.check_frame(S, fb, exp)
                 kind = "mixed" if mixed else "inter"
             kinds[kind] = kinds.get(kind, 0) + 1
