@@ -20,6 +20,9 @@
 // The done map therefore has three states per 4x4 cell: 0 = not written, 2 = predicted (PAL / II with residual records to
 // come), 1 = final. Neighbours wait for 1, a RESID record waits for 2 on its own cells. In frames with inter blocks the map
 // starts from `done_init` (every cell that no intra record covers is already final when the kernel starts).
+// The two per-transform-block kernels (CTA per block, warp per block) share one per-record front end: record decode
+// (intra_blk), mode conversion (intra_mode), dependency poll (intra_wait), edge gather with the Z2 corner (intra_edges), CFL
+// luma gather (intra_cfl_gather) and the prediction of a tile (intra_predict).
 // Integer, bit-exact with the reference C path.
 #include "ipred_body.cuh"
 #include "itx_body.cuh"
@@ -141,11 +144,202 @@ __device__ __forceinline__ int ibc_sample(const Frame &f, const B200IntraTx &r, 
     return iclip((16 * m0 + my * (m1 - m0) + ((1 << (4 + ib)) >> 1)) >> (4 + ib), 0, bdmax);
 }
 
-template <bool HBD>
+// ---- the per-record front end of the per-transform-block kernels ----------------------------------------------
+// what a record says about its transform block
+struct IntraBlk {
+    int pl, x, y, xe, ye;                   // plane; position and tile end in 4-sample units
+    int tw, th, w, h;                       // size in 4-sample units and in samples
+    int flags;                              // B200_INTRA_* availability bits
+    bool have_left, have_top;
+    bool is_cfl, is_ii, is_resid, is_pal, is_ibc;
+    // evaluated where they are used: held from the decode on, they cost the 10-bit warp kernel spills across its transform
+    B200_DEV bool have_tr() const { return have_top && x + tw < xe && (flags & B200_INTRA_TOP_HAS_RIGHT); }
+    B200_DEV bool have_bl() const { return have_left && y + th < ye && (flags & B200_INTRA_LEFT_HAS_BOTTOM); }
+};
+B200_DEV IntraBlk intra_blk(const B200IntraTx &r)
+{
+    IntraBlk b;
+    b.pl = r.plane; b.x = r.x4; b.y = r.y4; b.xe = r.xend4; b.ye = r.yend4;
+    b.tw = c_tx_w4[r.tx]; b.th = c_tx_h4[r.tx];
+    b.w = b.tw * 4; b.h = b.th * 4;
+    b.flags = r.flags;
+    b.have_left = r.flags & B200_INTRA_HAVE_LEFT; b.have_top = r.flags & B200_INTRA_HAVE_TOP;
+    b.is_cfl = r.mode == B200_INTRA_MODE_CFL && r.cfl_alpha != 0;
+    b.is_ii = r.mode == B200_INTRA_MODE_II; b.is_resid = r.mode == B200_INTRA_MODE_RESID;
+    b.is_pal = r.mode == B200_INTRA_MODE_PAL; b.is_ibc = r.mode == B200_INTRA_MODE_IBC;
+    return b;
+}
+
+// dav1d_prepare_intra_edges: mode conversion (:97-120). The predictor and the angle argument of ipred_pred_body (dav1d's
+// edge flags included; FILTER_PRED: the taps index).
+struct IntraPred { int mode, angle; };
+B200_DEV IntraPred intra_mode(const B200IntraTx &r, const IntraBlk &b)
+{
+    int mode = r.mode, angle = r.angle;
+    if (b.is_ii) { mode = r.angle; angle = 0; }                            // inter-intra: the predictor is in `angle`
+    if (b.is_resid || b.is_pal || b.is_ibc) mode = 0;
+    if (mode == B200_INTRA_MODE_CFL) mode = 0;                             // DC_PRED (:1446, :1373)
+    if (mode >= 1 && mode <= 8) {                                          // VERT_PRED .. VERT_LEFT_PRED
+        const int base = mode == 1 ? 90 : mode == 2 ? 180 : mode == 3 ? 45 : mode == 4 ? 135 : mode == 5 ? 113
+                       : mode == 6 ? 157 : mode == 7 ? 203 : 67;
+        angle = base + 3 * angle;
+        if (angle <= 90) mode = angle < 90 && b.have_top ? B200_Z1_PRED : B200_VERT_PRED;
+        else if (angle < 180) mode = B200_Z2_PRED;
+        else mode = angle > 180 && b.have_left ? B200_Z3_PRED : B200_HOR_PRED;
+    } else if (mode == 0) {
+        mode = b.have_left ? (b.have_top ? B200_DC_PRED : B200_LEFT_DC_PRED) : (b.have_top ? B200_TOP_DC_PRED : B200_DC_128_PRED);
+    } else if (mode == 12) {
+        mode = b.have_left ? (b.have_top ? B200_PAETH_PRED : B200_HOR_PRED) : (b.have_top ? B200_VERT_PRED : B200_DC_128_PRED);
+    }
+    return { mode, (mode == B200_FILTER_PRED ? r.angle : angle) | r.angle_flags };
+}
+
 #ifndef B200_POLL_NS0
 #define B200_POLL_NS0 32
 #define B200_POLL_NSMAX 256
 #endif
+// Waits until every done-map cell whose pixels the record reads is final: left, top, top-left, the CFL luma block, the
+// source rectangle of an intra block copy; a residual-only record waits for its own cells to be "predicted" (2).
+// Cells lane, lane + 32, ... of that list, then the acquire fence of the calling lanes.
+B200_DEV void intra_wait(const IntraParams &P, const B200IntraTx &r, const IntraBlk &b, const int lane)
+{
+    const IntraFrameDev &f = P.f;
+    const uint8_t *const dmap = P.scratch + P.done_off[b.pl];
+    const int x = b.x, y = b.y, tw = b.tw, th = b.th, mw = f.w4[b.pl];
+    const bool no_edges = b.is_resid || b.is_ibc;
+    const int n_left = no_edges ? 0 : b.have_left ? imin(th, b.ye - y) + (b.have_bl() ? imin(th, b.ye - y - th) : 0) : 0;
+    const int n_top = no_edges ? 0 : b.have_top ? imin(tw, b.xe - x) + (b.have_tr() ? imin(tw, b.xe - x - tw) : 0) : 0;
+    const int n_tl = !no_edges && b.have_left && b.have_top;
+    // intra block copy: every cell of the source rectangle (one sample more where the bilinear phase is not 0)
+    int n_src = 0, sc_x0 = 0, sc_y0 = 0, sc_w = 1;
+    if (b.is_ibc) {
+        const int sx = r.luma_off & 0xffff, sy = r.luma_off >> 16;
+        sc_x0 = imin(sx >> 2, mw - 1); sc_y0 = imin(sy >> 2, f.h4[b.pl] - 1);
+        sc_w = imin((sx + b.w - 1 + (r.cfl_w_pad != 0)) >> 2, mw - 1) - sc_x0 + 1;
+        n_src = sc_w * (imin((sy + b.h - 1 + (r.cfl_h_pad != 0)) >> 2, f.h4[b.pl] - 1) - sc_y0 + 1);
+    }
+    const int self_w = imin(tw, mw - x), n_self = b.is_resid ? self_w * imin(th, f.h4[b.pl] - y) : 0;
+    const int want = b.is_resid ? 2 : 1;
+    int n_luma = 0, lw4 = 0, lx4 = 0, ly4 = 0;
+    if (b.is_cfl) {
+        lx4 = x << f.ss_hor; ly4 = y << f.ss_ver;
+        lw4 = imin((tw - r.cfl_w_pad) << f.ss_hor, f.w4[0] - lx4);
+        const int lh4 = imin((th - r.cfl_h_pad) << f.ss_ver, f.h4[0] - ly4);
+        n_luma = lw4 * lh4;
+    }
+    for (int c = lane; c < n_left + n_top + n_tl + n_luma + n_self + n_src; c += 32) {
+        const uint8_t *cell;
+        if (c >= n_left + n_top + n_tl + n_luma + n_self) { const int k = c - n_left - n_top - n_tl - n_luma - n_self; cell = dmap + (sc_y0 + k / sc_w) * mw + sc_x0 + k % sc_w; }
+        else if (c >= n_left + n_top + n_tl + n_luma) { const int k = c - n_left - n_top - n_tl - n_luma; cell = dmap + (y + k / self_w) * mw + x + k % self_w; }
+        else if (c < n_left) cell = dmap + (y + c) * mw + x - 1;
+        else if (c < n_left + n_top) cell = dmap + (y - 1) * mw + x + (c - n_left);
+        else if (c < n_left + n_top + n_tl) cell = dmap + (y - 1) * mw + x - 1;
+        else { const int k = c - n_left - n_top - n_tl; cell = (P.scratch + P.done_off[0]) + (ly4 + k / lw4) * f.w4[0] + lx4 + k % lw4; }
+        unsigned ns = B200_POLL_NS0, spins = 0;
+        while (ld_cell(cell) != want) {
+            __nanosleep(ns); if (ns < B200_POLL_NSMAX) ns += ns >> 1;
+            if (++spins > (1u << 23)) intra_stuck();      // seconds: records are not in a valid order
+        }
+    }
+    __threadfence();              // acquire side
+}
+
+// The edge array of dav1d_prepare_intra_edges: tl[-(1+i)] left then bottom-left, tl[1+i] top then top-right, tl[0] the
+// top-left sample, with replication past the tile end, default values without neighbours and the Z2 corner smoothing.
+// Every part is filled; the predictors read only what the reference fills. `dst` is the block, `top` the row above it.
+// The smoothed corner reads only samples that thread 0 itself wrote, so it needs no barrier.
+template <bool HBD, class G>
+B200_DEV void intra_edges(int *tl, const typename Bd<HBD>::pixel *dst, const typename Bd<HBD>::pixel *top, const int st,
+                          const IntraBlk &b, const B200IntraTx &r, const int mode, const int bitdepth)
+{
+    const int w = b.w, h = b.h;
+    const int half = (1 << bitdepth) >> 1;
+    const bool have_tr = b.have_tr(), have_bl = b.have_bl();
+    const int lpx = imin(h, (b.ye - b.y) << 2), lpx2 = imin(h, (b.ye - b.y - b.th) << 2);
+    const int tpx = imin(w, (b.xe - b.x) << 2), tpx2 = imin(w, (b.xe - b.x - b.tw) << 2);
+    const int left_fill = b.have_top ? ld_px<HBD>(top) : half + 1;
+    const int top_fill = b.have_left ? ld_px<HBD>(dst - 1) : half - 1;
+    for (int i = G::tid(); i < 2 * h; i += G::size) {
+        int v;
+        if (i < h) v = b.have_left ? ld_px<HBD>(dst + (ptrdiff_t)imin(i, lpx - 1) * st - 1) : left_fill;
+        else if (have_bl) v = ld_px<HBD>(dst + (ptrdiff_t)(h + imin(i - h, lpx2 - 1)) * st - 1);
+        else v = b.have_left ? ld_px<HBD>(dst + (ptrdiff_t)(lpx - 1) * st - 1) : left_fill;
+        tl[-(1 + i)] = v;
+    }
+    for (int i = G::tid(); i < 2 * w; i += G::size) {
+        int v;
+        if (i < w) v = b.have_top ? ld_px<HBD>(top + imin(i, tpx - 1)) : top_fill;
+        else if (have_tr) v = ld_px<HBD>(top + w + imin(i - w, tpx2 - 1));
+        else v = b.have_top ? ld_px<HBD>(top + tpx - 1) : top_fill;
+        tl[1 + i] = v;
+    }
+    if (G::tid() == 0) {
+        tl[0] = b.have_left ? (b.have_top ? ld_px<HBD>(top - 1) : ld_px<HBD>(dst - 1)) : (b.have_top ? ld_px<HBD>(top) : half);
+        if (mode == B200_Z2_PRED && b.tw + b.th >= 6 && (r.angle_flags & 1024))
+            tl[0] = ((tl[-1] + tl[1]) * 5 + tl[0] * 6 + 8) >> 4;
+    }
+}
+
+// CFL: the (sub-sampled, padded) luma block at ypx (row pitch ys) -> ac, mean not yet removed; returns this thread's sum
+template <bool HBD, class G>
+B200_DEV int intra_cfl_gather(int16_t *ac, const typename Bd<HBD>::pixel *ypx, const int ys, const IntraFrameDev &f,
+                              const IntraBlk &b, const B200IntraTx &r)
+{
+    typedef typename Bd<HBD>::pixel pixel;
+    const int ssh = f.ss_hor, ssv = f.ss_ver, w = b.w, h = b.h;
+    int part = 0;
+    for (int i = G::tid(); i < w * h; i += G::size) {
+        const int yy = i / w, xx = i - yy * w;
+        const int sy = imin(yy, h - 4 * r.cfl_h_pad - 1), sx = imin(xx, w - 4 * r.cfl_w_pad - 1);
+        const pixel *p = ypx + (ptrdiff_t)(sy << ssv) * ys + (sx << ssh);
+        int sacc = ld_px<HBD>(p);
+        if (ssh) sacc += ld_px<HBD>(p + 1);
+        if (ssv) { sacc += ld_px<HBD>(p + ys); if (ssh) sacc += ld_px<HBD>(p + ys + 1); }
+        sacc <<= 1 + !ssv + !ssh;
+        ac[i] = (int16_t)sacc;
+        part += sacc;
+    }
+    return part;
+}
+
+// The prediction of a block into the shared tile s_px (pitch = its width) of the per-transform-block kernels, inter-intra
+// blend included; CFL reads the zero-mean ac in s_ac. `dst` is the block in the picture.
+template <bool HBD, class G>
+B200_DEV void intra_predict(IpShared &S, typename Bd<HBD>::pixel *s_px, const int16_t *s_ac, const typename Bd<HBD>::pixel *dst,
+                            const IntraFrameDev &f, const B200IntraTx &r, const IntraBlk &b, const IntraPred pm,
+                            const int bitdepth, const int bdmax)
+{
+    typedef typename Bd<HBD>::pixel pixel;
+    const int tid = G::tid(), st = f.stride[b.pl], w = b.w, h = b.h;
+    if (b.is_resid) {
+        // residual only: the tile is what the inter-intra record of this block left in the picture (another SM wrote it)
+        for (int i = tid; i < w * h; i += G::size) { const int yy = i / w, xx = i - yy * w; s_px[i] = (pixel)ld_px<HBD>(dst + (ptrdiff_t)yy * st + xx); }
+    } else if (b.is_pal) {
+        // palette: 8 colours, then the index map (two 4-bit indices per byte, low nibble first)
+        const pixel *const colours = (const pixel *)(f.pal + r.luma_off);
+        const uint8_t *const idx = f.pal + r.luma_off + 8 * sizeof(pixel);
+        for (int i = tid; i < w * h; i += G::size) s_px[i] = colours[(idx[i >> 1] >> ((i & 1) * 4)) & 7];
+    } else if (b.is_ibc) {
+        for (int i = tid; i < w * h; i += G::size) s_px[i] = (pixel)ibc_sample<HBD>(f, r, b.pl, i % w, i / w, bitdepth, bdmax);
+    } else if (b.is_cfl) {
+        ipred_cfl_pred_body<HBD, G>(S, s_px, w, w, h, pm.mode, r.cfl_alpha, s_ac, bdmax);
+    } else {
+        ipred_pred_body<HBD, G>(S, s_px, w, w, h, pm.mode, pm.angle, r.max_w, r.max_h, bdmax);
+    }
+    G::sync();
+    if (b.is_ii) {
+        // inter-intra: blend the intra prediction into the inter prediction already in the picture (earlier launch),
+        // dst = (inter * (64 - m) + intra * m + 32) >> 6 (dsp->mc.blend, reference src/mc_tmpl.c:683-694)
+        const uint8_t *const msk = f.mask + r.luma_off;
+        for (int i = tid; i < w * h; i += G::size) {
+            const int yy = i / w, xx = i - yy * w, m = msk[i];
+            s_px[i] = (pixel)(((int)dst[(ptrdiff_t)yy * st + xx] * (64 - m) + (int)s_px[i] * m + 32) >> 6);
+        }
+        G::sync();
+    }
+}
+
+template <bool HBD>
 #ifndef B200_INTRA_MINB
 #define B200_INTRA_MINB 5
 #endif
@@ -181,18 +375,8 @@ __global__ void __launch_bounds__(kIpT, B200_INTRA_MINB) intra_frame_kernel(cons
         for (int k = 0; k < kRecWords; k++) ((uint32_t *)&r)[k] = s_rec[k];
         int nxt = 0;
         if (tid == 0) nxt = atomicAdd(((int *)P.scratch), 1);          // consumed at the end of this iteration
-        const int pl = r.plane, st = f.stride[pl];
-        const int tw = c_tx_w4[r.tx], th = c_tx_h4[r.tx];              // 4-sample units
-        const int w = tw * 4, h = th * 4;
-        const int x = r.x4, y = r.y4, xe = r.xend4, ye = r.yend4;
-        const bool have_left = r.flags & B200_INTRA_HAVE_LEFT, have_top = r.flags & B200_INTRA_HAVE_TOP;
-        const bool have_tr = have_top && x + tw < xe && (r.flags & B200_INTRA_TOP_HAS_RIGHT);
-        const bool have_bl = have_left && y + th < ye && (r.flags & B200_INTRA_LEFT_HAS_BOTTOM);
-        const bool is_cfl = r.mode == B200_INTRA_MODE_CFL && r.cfl_alpha != 0;
-        const bool is_ii = r.mode == B200_INTRA_MODE_II, is_resid = r.mode == B200_INTRA_MODE_RESID, is_pal = r.mode == B200_INTRA_MODE_PAL;
-        const bool is_ibc = r.mode == B200_INTRA_MODE_IBC;
-        const uint8_t *const dmap = (P.scratch + P.done_off[pl]);
-        const int mw = f.w4[pl];
+        const IntraBlk b = intra_blk(r);
+        const int pl = b.pl, st = f.stride[pl], w = b.w, h = b.h;
         // coefficients: loads issued before the wait, parked in shared memory after it (off the dependency chain)
         const int ncf = imin(w, 32) * imin(h, 32);
         coef *const gcf = (coef *)f.d_coef + r.coef_off;
@@ -202,163 +386,41 @@ __global__ void __launch_bounds__(kIpT, B200_INTRA_MINB) intra_frame_kernel(cons
             for (int k = 0; k < 1024 / kIpT; k++) { const int i = tid + k * kIpT; creg[k] = i < ncf ? gcf[i] : (coef)0; }
         }
 
-        // ---- wait for the neighbours whose pixels the edge array reads
-        {
-            // a residual-only record waits for its own cells to be "predicted" (2), everything else for final neighbours (1)
-            const bool no_edges = is_resid || is_ibc;
-            const int n_left = no_edges ? 0 : have_left ? imin(th, ye - y) + (have_bl ? imin(th, ye - y - th) : 0) : 0;
-            const int n_top = no_edges ? 0 : have_top ? imin(tw, xe - x) + (have_tr ? imin(tw, xe - x - tw) : 0) : 0;
-            const int n_tl = !no_edges && have_left && have_top;
-            // intra block copy: every cell of the source rectangle (one sample more where the bilinear phase is not 0)
-            int n_src = 0, sc_x0 = 0, sc_y0 = 0, sc_w = 1;
-            if (is_ibc) {
-                const int sx = r.luma_off & 0xffff, sy = r.luma_off >> 16;
-                sc_x0 = imin(sx >> 2, mw - 1); sc_y0 = imin(sy >> 2, f.h4[pl] - 1);
-                sc_w = imin((sx + w - 1 + (r.cfl_w_pad != 0)) >> 2, mw - 1) - sc_x0 + 1;
-                n_src = sc_w * (imin((sy + h - 1 + (r.cfl_h_pad != 0)) >> 2, f.h4[pl] - 1) - sc_y0 + 1);
-            }
-            const int self_w = imin(tw, mw - x), n_self = is_resid ? self_w * imin(th, f.h4[pl] - y) : 0;
-            const int want = is_resid ? 2 : 1;
-            int n_luma = 0, lw4 = 0, lx4 = 0, ly4 = 0;
-            if (is_cfl) {
-                lx4 = x << f.ss_hor; ly4 = y << f.ss_ver;
-                lw4 = imin((tw - r.cfl_w_pad) << f.ss_hor, f.w4[0] - lx4);
-                const int lh4 = imin((th - r.cfl_h_pad) << f.ss_ver, f.h4[0] - ly4);
-                n_luma = lw4 * lh4;
-            }
-            // only warp 0 polls (the other warps park at the barrier and cost no issue slots)
-            if (tid < 32) {
-                for (int c = tid; c < n_left + n_top + n_tl + n_luma + n_self + n_src; c += 32) {
-                    const uint8_t *cell;
-                    if (c >= n_left + n_top + n_tl + n_luma + n_self) { const int k = c - n_left - n_top - n_tl - n_luma - n_self; cell = dmap + (sc_y0 + k / sc_w) * mw + sc_x0 + k % sc_w; }
-                    else if (c >= n_left + n_top + n_tl + n_luma) { const int k = c - n_left - n_top - n_tl - n_luma; cell = dmap + (y + k / self_w) * mw + x + k % self_w; }
-                    else if (c < n_left) cell = dmap + (y + c) * mw + x - 1;
-                    else if (c < n_left + n_top) cell = dmap + (y - 1) * mw + x + (c - n_left);
-                    else if (c < n_left + n_top + n_tl) cell = dmap + (y - 1) * mw + x - 1;
-                    else { const int k = c - n_left - n_top - n_tl; cell = (P.scratch + P.done_off[0]) + (ly4 + k / lw4) * f.w4[0] + lx4 + k % lw4; }
-                    unsigned ns = B200_POLL_NS0, spins = 0;
-                    while (ld_cell(cell) != want) {
-                        __nanosleep(ns); if (ns < B200_POLL_NSMAX) ns += ns >> 1;
-                        if (++spins > (1u << 23)) intra_stuck();      // seconds: records are not in a valid order
-                    }
-                }
-                __threadfence();          // acquire side, by the polling warp only (the barrier below publishes it)
-            }
-            if (tid == 0) s_next = nxt;
-            if (r.eob >= 0) {
+        // ---- wait for the neighbours whose pixels the edge array reads: only warp 0 polls (the other warps park at the
+        // barrier and cost no issue slots); its acquire fence is published by the barrier
+        if (tid < 32) intra_wait(P, r, b, tid);
+        if (tid == 0) s_next = nxt;
+        if (r.eob >= 0) {
 #pragma unroll
-                for (int k = 0; k < 1024 / kIpT; k++) { const int i = tid + k * kIpT; if (i < ncf) s_cf[i] = creg[k]; }
-            }
-            __syncthreads();
+            for (int k = 0; k < 1024 / kIpT; k++) { const int i = tid + k * kIpT; if (i < ncf) s_cf[i] = creg[k]; }
         }
+        __syncthreads();
 
         pixel *const dst = (pixel *)f.pic + r.dst_off;
-        // ---- dav1d_prepare_intra_edges: mode conversion (:97-120)
-        int mode = r.mode, angle = r.angle;
-        if (is_ii) { mode = r.angle; angle = 0; }                              // inter-intra: the predictor is in `angle`
-        if (is_resid || is_pal || is_ibc) mode = 0;
-        if (mode == B200_INTRA_MODE_CFL) mode = 0;                             // DC_PRED (:1446, :1373)
-        if (mode >= 1 && mode <= 8) {                                          // VERT_PRED .. VERT_LEFT_PRED
-            const int base = mode == 1 ? 90 : mode == 2 ? 180 : mode == 3 ? 45 : mode == 4 ? 135 : mode == 5 ? 113
-                           : mode == 6 ? 157 : mode == 7 ? 203 : 67;
-            angle = base + 3 * angle;
-            if (angle <= 90) mode = angle < 90 && have_top ? B200_Z1_PRED : B200_VERT_PRED;
-            else if (angle < 180) mode = B200_Z2_PRED;
-            else mode = angle > 180 && have_left ? B200_Z3_PRED : B200_HOR_PRED;
-        } else if (mode == 0) {
-            mode = have_left ? (have_top ? B200_DC_PRED : B200_LEFT_DC_PRED) : (have_top ? B200_TOP_DC_PRED : B200_DC_128_PRED);
-        } else if (mode == 12) {
-            mode = have_left ? (have_top ? B200_PAETH_PRED : B200_HOR_PRED) : (have_top ? B200_VERT_PRED : B200_DC_128_PRED);
+        const IntraPred pm = intra_mode(r, b);
+        intra_edges<HBD, IpCta>(tl, dst, intra_top_row(B.band, f, (const pixel *)dst, pl, b.x, b.y, b.have_top), st,
+                                b, r, pm.mode, bitdepth);
+        if (b.is_cfl) S.tile[tid] = intra_cfl_gather<HBD, IpCta>(s_ac, (const pixel *)f.pic + r.luma_off, f.stride[0], f, b, r);
+        __syncthreads();
+        if (b.is_cfl && tid == 0) {
+            const int log2sz = (__ffs(w) - 1) + (__ffs(h) - 1);
+            int sum = (1 << log2sz) >> 1;
+            for (int i = 0; i < kIpT; i++) sum += S.tile[i];
+            S.dc = sum >> log2sz;
         }
-        // ---- edge gather (every part is filled; the predictors read only what the reference fills)
-        {
-            const pixel *const top = intra_top_row(B.band, f, (const pixel *)dst, pl, x, y, have_top);
-            const int half = (1 << bitdepth) >> 1;
-            const int lpx = imin(h, (ye - y) << 2), lpx2 = imin(h, (ye - y - th) << 2);
-            const int tpx = imin(w, (xe - x) << 2), tpx2 = imin(w, (xe - x - tw) << 2);
-            const int left_fill = have_top ? ld_px<HBD>(top) : half + 1;
-            const int top_fill = have_left ? ld_px<HBD>(dst - 1) : half - 1;
-            for (int i = tid; i < 2 * h; i += kIpT) {                           // tl[-(1+i)]: left, then bottom-left
-                int v;
-                if (i < h) v = have_left ? ld_px<HBD>(dst + (ptrdiff_t)imin(i, lpx - 1) * st - 1) : left_fill;
-                else if (have_bl) v = ld_px<HBD>(dst + (ptrdiff_t)(h + imin(i - h, lpx2 - 1)) * st - 1);
-                else v = have_left ? ld_px<HBD>(dst + (ptrdiff_t)(lpx - 1) * st - 1) : left_fill;
-                tl[-(1 + i)] = v;
-            }
-            for (int i = tid; i < 2 * w; i += kIpT) {                           // tl[1+i]: top, then top-right
-                int v;
-                if (i < w) v = have_top ? ld_px<HBD>(top + imin(i, tpx - 1)) : top_fill;
-                else if (have_tr) v = ld_px<HBD>(top + w + imin(i - w, tpx2 - 1));
-                else v = have_top ? ld_px<HBD>(top + tpx - 1) : top_fill;
-                tl[1 + i] = v;
-            }
-            if (tid == 0)
-                tl[0] = have_left ? (have_top ? ld_px<HBD>(top - 1) : ld_px<HBD>(dst - 1)) : (have_top ? ld_px<HBD>(top) : half);
-            // CFL: the (sub-sampled, padded) luma block -> s_ac (mean removed below)
-            int part = 0;
-            if (is_cfl) {
-                const pixel *ypx = (const pixel *)f.pic + r.luma_off;
-                const int ssh = f.ss_hor, ssv = f.ss_ver, ys = f.stride[0];
-                for (int i = tid; i < w * h; i += kIpT) {
-                    const int yy = i / w, xx = i - yy * w;
-                    const int sy = imin(yy, h - 4 * r.cfl_h_pad - 1), sx = imin(xx, w - 4 * r.cfl_w_pad - 1);
-                    const pixel *p = ypx + (ptrdiff_t)(sy << ssv) * ys + (sx << ssh);
-                    int sacc = ld_px<HBD>(p);
-                    if (ssh) sacc += ld_px<HBD>(p + 1);
-                    if (ssv) { sacc += ld_px<HBD>(p + ys); if (ssh) sacc += ld_px<HBD>(p + ys + 1); }
-                    sacc <<= 1 + !ssv + !ssh;
-                    s_ac[i] = (int16_t)sacc;
-                    part += sacc;
-                }
-                S.tile[tid] = part;
-            }
-            __syncthreads();
-            if (tid == 0 && mode == B200_Z2_PRED && tw + th >= 6 && (r.angle_flags & 1024))
-                tl[0] = ((tl[-1] + tl[1]) * 5 + tl[0] * 6 + 8) >> 4;
-            if (is_cfl && tid == 0) {
-                const int log2sz = (__ffs(w) - 1) + (__ffs(h) - 1);
-                int sum = (1 << log2sz) >> 1;
-                for (int i = 0; i < kIpT; i++) sum += S.tile[i];
-                S.dc = sum >> log2sz;
-            }
-            __syncthreads();
-        }
+        __syncthreads();
         // the next record (its ticket has arrived by now): loads issued here, consumed at the end of the iteration
         uint32_t next_word = 0;
         const int nti = s_next;
         if (tid < kRecWords && nti < P.n) next_word = ((const uint32_t *)&P.tx[nti])[tid];
 
         // ---- predict into the shared tile
-        if (is_resid) {
-            // residual only: the tile is what the inter-intra record of this block left in the picture (another SM wrote it)
-            for (int i = tid; i < w * h; i += kIpT) { const int yy = i / w, xx = i - yy * w; s_px[i] = (pixel)ld_px<HBD>(dst + (ptrdiff_t)yy * st + xx); }
-        } else if (is_pal) {
-            // palette: 8 colours, then the index map (two 4-bit indices per byte, low nibble first)
-            const pixel *const colours = (const pixel *)(f.pal + r.luma_off);
-            const uint8_t *const idx = f.pal + r.luma_off + 8 * sizeof(pixel);
-            for (int i = tid; i < w * h; i += kIpT) s_px[i] = colours[(idx[i >> 1] >> ((i & 1) * 4)) & 7];
-        } else if (is_ibc) {
-            for (int i = tid; i < w * h; i += kIpT) s_px[i] = (pixel)ibc_sample<HBD>(f, r, pl, i % w, i / w, bitdepth, bdmax);
-        } else if (is_cfl) {
+        if (b.is_cfl) {
             const int dc = S.dc;
             for (int i = tid; i < w * h; i += kIpT) s_ac[i] = (int16_t)(s_ac[i] - dc);
             __syncthreads();
-            ipred_cfl_pred_body<HBD>(S, s_px, w, w, h, mode, r.cfl_alpha, s_ac, bdmax);
-        } else {
-            const int a = (mode == B200_FILTER_PRED ? r.angle : angle) | r.angle_flags;
-            ipred_pred_body<HBD>(S, s_px, w, w, h, mode, a, r.max_w, r.max_h, bdmax);
         }
-        __syncthreads();
-        if (is_ii) {
-            // inter-intra: blend the intra prediction into the inter prediction already in the picture (earlier launch),
-            // dst = (inter * (64 - m) + intra * m + 32) >> 6 (dsp->mc.blend, reference src/mc_tmpl.c:683-694)
-            const uint8_t *const msk = f.mask + r.luma_off;
-            for (int i = tid; i < w * h; i += kIpT) {
-                const int yy = i / w, xx = i - yy * w, m = msk[i];
-                s_px[i] = (pixel)(((int)dst[(ptrdiff_t)yy * st + xx] * (64 - m) + (int)s_px[i] * m + 32) >> 6);
-            }
-            __syncthreads();
-        }
+        intra_predict<HBD, IpCta>(S, s_px, s_ac, dst, f, r, b, pm, bitdepth, bdmax);
 
         // ---- residual, added in the shared tile
         if (r.eob >= 0) {
@@ -385,9 +447,9 @@ __global__ void __launch_bounds__(kIpT, B200_INTRA_MINB) intra_frame_kernel(cons
             if (tid == 0) __threadfence();
             __syncwarp();
             uint8_t *const dm = (P.scratch + P.done_off[pl]);
-            const int cw = imin(tw, mw - x), chh = imin(th, f.h4[pl] - y);
-            const uint8_t state = (is_ii || is_pal || is_ibc) && r.cfl_alpha ? 2 : 1;   // 2: predicted, the block's residual records follow
-            for (int c = tid; c < cw * chh; c += 32) *(volatile uint8_t *)(dm + (y + c / cw) * mw + x + c % cw) = state;
+            const int mw = f.w4[pl], cw = imin(b.tw, mw - b.x), chh = imin(b.th, f.h4[pl] - b.y);
+            const uint8_t state = (b.is_ii || b.is_pal || b.is_ibc) && r.cfl_alpha ? 2 : 1;   // 2: predicted, the block's residual records follow
+            for (int c = tid; c < cw * chh; c += 32) *(volatile uint8_t *)(dm + (b.y + c / cw) * mw + b.x + c % cw) = state;
         }
         // ---- hand over to the next record
         if (tid < kRecWords) s_rec[tid] = next_word;
@@ -453,18 +515,8 @@ __global__ void __launch_bounds__(kIwWarps * 32) intra_warp_kernel(const __grid_
         ti = __shfl_sync(0xffffffffu, ti, 0);
         if (ti >= P.n) break;
         const B200IntraTx r = P.tx[ti];
-        const int pl = r.plane, st = f.stride[pl];
-        const int tw = c_tx_w4[r.tx], th = c_tx_h4[r.tx];              // 4-sample units
-        const int w = tw * 4, h = th * 4;
-        const int x = r.x4, y = r.y4, xe = r.xend4, ye = r.yend4;
-        const bool have_left = r.flags & B200_INTRA_HAVE_LEFT, have_top = r.flags & B200_INTRA_HAVE_TOP;
-        const bool have_tr = have_top && x + tw < xe && (r.flags & B200_INTRA_TOP_HAS_RIGHT);
-        const bool have_bl = have_left && y + th < ye && (r.flags & B200_INTRA_LEFT_HAS_BOTTOM);
-        const bool is_cfl = r.mode == B200_INTRA_MODE_CFL && r.cfl_alpha != 0;
-        const bool is_ii = r.mode == B200_INTRA_MODE_II, is_resid = r.mode == B200_INTRA_MODE_RESID, is_pal = r.mode == B200_INTRA_MODE_PAL;
-        const bool is_ibc = r.mode == B200_INTRA_MODE_IBC;
-        uint8_t *const dmap = (P.scratch + P.done_off[pl]);
-        const int mw = f.w4[pl];
+        const IntraBlk b = intra_blk(r);
+        const int pl = b.pl, st = f.stride[pl], w = b.w, h = b.h;
         const int ncf = imin(w, 32) * imin(h, 32);
         coef *const gcf = (coef *)f.d_coef + r.coef_off;
         // The residual does not depend on the neighbours: inverse transform NOW, into an int16 tile, off the dependency chain
@@ -483,104 +535,17 @@ __global__ void __launch_bounds__(kIwWarps * 32) intra_warp_kernel(const __grid_
         }
 
         // ---- wait for the neighbours whose pixels the edge array reads
-        {
-            const bool no_edges = is_resid || is_ibc;
-            const int n_left = no_edges ? 0 : have_left ? imin(th, ye - y) + (have_bl ? imin(th, ye - y - th) : 0) : 0;
-            const int n_top = no_edges ? 0 : have_top ? imin(tw, xe - x) + (have_tr ? imin(tw, xe - x - tw) : 0) : 0;
-            const int n_tl = !no_edges && have_left && have_top;
-            // intra block copy: every cell of the source rectangle (one sample more where the bilinear phase is not 0)
-            int n_src = 0, sc_x0 = 0, sc_y0 = 0, sc_w = 1;
-            if (is_ibc) {
-                const int sx = r.luma_off & 0xffff, sy = r.luma_off >> 16;
-                sc_x0 = imin(sx >> 2, mw - 1); sc_y0 = imin(sy >> 2, f.h4[pl] - 1);
-                sc_w = imin((sx + w - 1 + (r.cfl_w_pad != 0)) >> 2, mw - 1) - sc_x0 + 1;
-                n_src = sc_w * (imin((sy + h - 1 + (r.cfl_h_pad != 0)) >> 2, f.h4[pl] - 1) - sc_y0 + 1);
-            }
-            const int self_w = imin(tw, mw - x), n_self = is_resid ? self_w * imin(th, f.h4[pl] - y) : 0;
-            const int want = is_resid ? 2 : 1;       // a residual-only record waits for its own cells to be "predicted" (2)
-            int n_luma = 0, lw4 = 0, lx4 = 0, ly4 = 0;
-            if (is_cfl) {
-                lx4 = x << f.ss_hor; ly4 = y << f.ss_ver;
-                lw4 = imin((tw - r.cfl_w_pad) << f.ss_hor, f.w4[0] - lx4);
-                const int lh4 = imin((th - r.cfl_h_pad) << f.ss_ver, f.h4[0] - ly4);
-                n_luma = lw4 * lh4;
-            }
-            for (int c = lane; c < n_left + n_top + n_tl + n_luma + n_self + n_src; c += 32) {
-                const uint8_t *cell;
-                if (c >= n_left + n_top + n_tl + n_luma + n_self) { const int k = c - n_left - n_top - n_tl - n_luma - n_self; cell = dmap + (sc_y0 + k / sc_w) * mw + sc_x0 + k % sc_w; }
-                else if (c >= n_left + n_top + n_tl + n_luma) { const int k = c - n_left - n_top - n_tl - n_luma; cell = dmap + (y + k / self_w) * mw + x + k % self_w; }
-                else if (c < n_left) cell = dmap + (y + c) * mw + x - 1;
-                else if (c < n_left + n_top) cell = dmap + (y - 1) * mw + x + (c - n_left);
-                else if (c < n_left + n_top + n_tl) cell = dmap + (y - 1) * mw + x - 1;
-                else { const int k = c - n_left - n_top - n_tl; cell = (P.scratch + P.done_off[0]) + (ly4 + k / lw4) * f.w4[0] + lx4 + k % lw4; }
-                unsigned ns = B200_POLL_NS0, spins = 0;
-                while (ld_cell(cell) != want) {
-                    __nanosleep(ns); if (ns < B200_POLL_NSMAX) ns += ns >> 1;
-                    if (++spins > (1u << 23)) intra_stuck();      // seconds: records are not in a valid order
-                }
-            }
-            __threadfence();              // acquire side
-            __syncwarp();
-        }
+        intra_wait(P, r, b, lane);
+        __syncwarp();
 
         pixel *const dst = (pixel *)f.pic + r.dst_off;
-        // ---- dav1d_prepare_intra_edges: mode conversion (:97-120)
-        int mode = r.mode, angle = r.angle;
-        if (is_ii) { mode = r.angle; angle = 0; }                              // inter-intra: the predictor is in `angle`
-        if (is_resid || is_pal || is_ibc) mode = 0;
-        if (mode == B200_INTRA_MODE_CFL) mode = 0;                             // DC_PRED (:1446, :1373)
-        if (mode >= 1 && mode <= 8) {                                          // VERT_PRED .. VERT_LEFT_PRED
-            const int base = mode == 1 ? 90 : mode == 2 ? 180 : mode == 3 ? 45 : mode == 4 ? 135 : mode == 5 ? 113
-                           : mode == 6 ? 157 : mode == 7 ? 203 : 67;
-            angle = base + 3 * angle;
-            if (angle <= 90) mode = angle < 90 && have_top ? B200_Z1_PRED : B200_VERT_PRED;
-            else if (angle < 180) mode = B200_Z2_PRED;
-            else mode = angle > 180 && have_left ? B200_Z3_PRED : B200_HOR_PRED;
-        } else if (mode == 0) {
-            mode = have_left ? (have_top ? B200_DC_PRED : B200_LEFT_DC_PRED) : (have_top ? B200_TOP_DC_PRED : B200_DC_128_PRED);
-        } else if (mode == 12) {
-            mode = have_left ? (have_top ? B200_PAETH_PRED : B200_HOR_PRED) : (have_top ? B200_VERT_PRED : B200_DC_128_PRED);
-        }
-        // ---- edge gather (every part is filled; the predictors read only what the reference fills)
-        if (!is_resid && !is_pal && !is_ibc) {
-            const pixel *const top = intra_top_row(B.band, f, (const pixel *)dst, pl, x, y, have_top);
-            const int half = (1 << bitdepth) >> 1;
-            const int lpx = imin(h, (ye - y) << 2), lpx2 = imin(h, (ye - y - th) << 2);
-            const int tpx = imin(w, (xe - x) << 2), tpx2 = imin(w, (xe - x - tw) << 2);
-            const int left_fill = have_top ? ld_px<HBD>(top) : half + 1;
-            const int top_fill = have_left ? ld_px<HBD>(dst - 1) : half - 1;
-            for (int i = lane; i < 2 * h; i += 32) {                            // tl[-(1+i)]: left, then bottom-left
-                int v;
-                if (i < h) v = have_left ? ld_px<HBD>(dst + (ptrdiff_t)imin(i, lpx - 1) * st - 1) : left_fill;
-                else if (have_bl) v = ld_px<HBD>(dst + (ptrdiff_t)(h + imin(i - h, lpx2 - 1)) * st - 1);
-                else v = have_left ? ld_px<HBD>(dst + (ptrdiff_t)(lpx - 1) * st - 1) : left_fill;
-                tl[-(1 + i)] = v;
-            }
-            for (int i = lane; i < 2 * w; i += 32) {                            // tl[1+i]: top, then top-right
-                int v;
-                if (i < w) v = have_top ? ld_px<HBD>(top + imin(i, tpx - 1)) : top_fill;
-                else if (have_tr) v = ld_px<HBD>(top + w + imin(i - w, tpx2 - 1));
-                else v = have_top ? ld_px<HBD>(top + tpx - 1) : top_fill;
-                tl[1 + i] = v;
-            }
-            if (lane == 0)
-                tl[0] = have_left ? (have_top ? ld_px<HBD>(top - 1) : ld_px<HBD>(dst - 1)) : (have_top ? ld_px<HBD>(top) : half);
+        const IntraPred pm = intra_mode(r, b);
+        if (!b.is_resid && !b.is_pal && !b.is_ibc) {
+            intra_edges<HBD, G>(tl, dst, intra_top_row(B.band, f, (const pixel *)dst, pl, b.x, b.y, b.have_top), st,
+                                b, r, pm.mode, bitdepth);
             // CFL: the (sub-sampled, padded) luma block -> s_ac, mean removed
-            if (is_cfl) {
-                const pixel *ypx = (const pixel *)f.pic + r.luma_off;
-                const int ssh = f.ss_hor, ssv = f.ss_ver, ys = f.stride[0];
-                int part = 0;
-                for (int i = lane; i < w * h; i += 32) {
-                    const int yy = i / w, xx = i - yy * w;
-                    const int sy = imin(yy, h - 4 * r.cfl_h_pad - 1), sx = imin(xx, w - 4 * r.cfl_w_pad - 1);
-                    const pixel *p = ypx + (ptrdiff_t)(sy << ssv) * ys + (sx << ssh);
-                    int sacc = ld_px<HBD>(p);
-                    if (ssh) sacc += ld_px<HBD>(p + 1);
-                    if (ssv) { sacc += ld_px<HBD>(p + ys); if (ssh) sacc += ld_px<HBD>(p + ys + 1); }
-                    sacc <<= 1 + !ssv + !ssh;
-                    s_ac[i] = (int16_t)sacc;
-                    part += sacc;
-                }
+            if (b.is_cfl) {
+                int part = intra_cfl_gather<HBD, G>(s_ac, (const pixel *)f.pic + r.luma_off, f.stride[0], f, b, r);
 #pragma unroll
                 for (int o = 16; o; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
                 const int log2sz = (__ffs(w) - 1) + (__ffs(h) - 1);
@@ -589,39 +554,8 @@ __global__ void __launch_bounds__(kIwWarps * 32) intra_warp_kernel(const __grid_
                 for (int i = lane; i < w * h; i += 32) s_ac[i] = (int16_t)(s_ac[i] - dc);
             }
             __syncwarp();
-            if (lane == 0 && mode == B200_Z2_PRED && tw + th >= 6 && (r.angle_flags & 1024))
-                tl[0] = ((tl[-1] + tl[1]) * 5 + tl[0] * 6 + 8) >> 4;
-            __syncwarp();
         }
-
-        // ---- predict into the shared tile
-        if (is_resid) {
-            // residual only: the tile is what the inter-intra record of this block left in the picture (another SM wrote it)
-            for (int i = lane; i < w * h; i += 32) { const int yy = i / w, xx = i - yy * w; s_px[i] = (pixel)ld_px<HBD>(dst + (ptrdiff_t)yy * st + xx); }
-        } else if (is_pal) {
-            // palette: 8 colours, then the index map (two 4-bit indices per byte, low nibble first)
-            const pixel *const colours = (const pixel *)(f.pal + r.luma_off);
-            const uint8_t *const idx = f.pal + r.luma_off + 8 * sizeof(pixel);
-            for (int i = lane; i < w * h; i += 32) s_px[i] = colours[(idx[i >> 1] >> ((i & 1) * 4)) & 7];
-        } else if (is_ibc) {
-            for (int i = lane; i < w * h; i += 32) s_px[i] = (pixel)ibc_sample<HBD>(f, r, pl, i % w, i / w, bitdepth, bdmax);
-        } else if (is_cfl) {
-            ipred_cfl_pred_body<HBD, G>(S, s_px, w, w, h, mode, r.cfl_alpha, s_ac, bdmax);
-        } else {
-            const int a = (mode == B200_FILTER_PRED ? r.angle : angle) | r.angle_flags;
-            ipred_pred_body<HBD, G>(S, s_px, w, w, h, mode, a, r.max_w, r.max_h, bdmax);
-        }
-        __syncwarp();
-        if (is_ii) {
-            // inter-intra: blend the intra prediction into the inter prediction already in the picture (earlier launch),
-            // dst = (inter * (64 - m) + intra * m + 32) >> 6 (dsp->mc.blend, reference src/mc_tmpl.c:683-694)
-            const uint8_t *const msk = f.mask + r.luma_off;
-            for (int i = lane; i < w * h; i += 32) {
-                const int yy = i / w, xx = i - yy * w, m = msk[i];
-                s_px[i] = (pixel)(((int)dst[(ptrdiff_t)yy * st + xx] * (64 - m) + (int)s_px[i] * m + 32) >> 6);
-            }
-            __syncwarp();
-        }
+        intra_predict<HBD, G>(S, s_px, s_ac, dst, f, r, b, pm, bitdepth, bdmax);
 
         // ---- prediction + residual -> picture, publish
         if (r.eob >= 0) {
@@ -637,10 +571,11 @@ __global__ void __launch_bounds__(kIwWarps * 32) intra_warp_kernel(const __grid_
         }
         __syncwarp();
         {
-            const int cw = imin(tw, mw - x), chh = imin(th, f.h4[pl] - y);
-            const uint8_t state = (is_ii || is_pal || is_ibc) && r.cfl_alpha ? 2 : 1;   // 2: predicted, the block's residual records follow
+            uint8_t *const dmap = (P.scratch + P.done_off[pl]);
+            const int mw = f.w4[pl], cw = imin(b.tw, mw - b.x), chh = imin(b.th, f.h4[pl] - b.y);
+            const uint8_t state = (b.is_ii || b.is_pal || b.is_ibc) && r.cfl_alpha ? 2 : 1;   // 2: predicted, the block's residual records follow
             if (lane < cw * chh || lane == 0) __threadfence();                  // the warp barrier above ordered every lane's stores before it
-            for (int c = lane; c < cw * chh; c += 32) *(volatile uint8_t *)(dmap + (y + c / cw) * mw + x + c % cw) = state;
+            for (int c = lane; c < cw * chh; c += 32) *(volatile uint8_t *)(dmap + (b.y + c / cw) * mw + b.x + c % cw) = state;
         }
         __syncwarp();
     }

@@ -107,7 +107,7 @@ IBC_CASES = [(8, 328, 264, 1, 1), (10, 264, 200, 1, 1), (12, 200, 264, 0, 0), (8
 def test_intra_block_copy_oracle_reference_and_kernel(bpc, W, H, ssh, ssv):
     """intra block copy records (B200_INTRA_MODE_IBC + RESID): blocks copied with the bilinear put from arbitrary (unaligned,
     odd-vector) positions in the superblock rows above; the oracle's restatement, dav1d's own emu_edge + mc[BILINEAR] and the
-    intra machine (wavefront order and decode order, both kernels) give the same picture"""
+    intra machine (wavefront order and decode order) give the same picture"""
     S = synth.make_intra_frame(np.random.default_rng(740 + bpc + W), bpc, W, H, ssh, ssv, p_ibc=0.3)
     t = S["intra_tx"]
     assert (t["mode"] == synth.MODE_IBC).sum() > 12 and (t["mode"] == synth.MODE_RESID).sum() > 12
@@ -123,13 +123,40 @@ def test_intra_block_copy_oracle_reference_and_kernel(bpc, W, H, ssh, ssv):
         got = run_lib(refs.emu_lib(), frame.NumpyAlloc(), S, order=order, compact=order == "intra_tx")
         ok, where = planes_equal(S, exp, got)
         assert ok, (order, where)
-    os.environ["B200_INTRA_CTA"] = "1"                                       # the CTA-per-block kernel (read once per process:
-    try:                                                                     # effective only if this is the first intra launch)
-        got = run_lib(refs.emu_lib(), frame.NumpyAlloc(), S)
-    finally:
-        del os.environ["B200_INTRA_CTA"]
-    ok, where = planes_equal(S, exp, got)
-    assert ok, ("cta", where)
+
+
+def check_cta_kernel():
+    """The CTA-per-block kernel against the oracle: an intra block copy frame, an intra frame in wavefront and in decode
+    order, a mixed PAL / II / RESID frame. Runs in a process started with B200_INTRA_CTA=1 (test_emu_intra_cta_kernel)."""
+    emu = refs.emu_lib()
+    bpc, W, H, ssh, ssv = IBC_CASES[0]
+    S = synth.make_intra_frame(np.random.default_rng(740 + bpc + W), bpc, W, H, ssh, ssv, p_ibc=0.3)
+    ok, where = planes_equal(S, oracle_intra(S), run_lib(emu, frame.NumpyAlloc(), S))
+    assert ok, ("ibc", where)
+    bpc, W, H, ssh, ssv = CASES[1]
+    S = synth.make_intra_frame(np.random.default_rng(720 + bpc + W), bpc, W, H, ssh, ssv)
+    exp = oracle_intra(S)
+    for order in ("intra_tx", "intra_tx_decode_order"):
+        ok, where = planes_equal(S, exp, run_lib(emu, frame.NumpyAlloc(), S, order=order))
+        assert ok, (order, where)
+    bpc, W, H, ssh, ssv = CASES[0]
+    rng = np.random.default_rng(900 + bpc + W)
+    S = make_mixed(synth.make_intra_frame(rng, bpc, W, H, ssh, ssv), rng)
+    ok, where = planes_equal(S, run_mixed(refs.oracle().oracle_intra_frame, S), run_mixed(None, S, emu=emu))
+    assert ok, ("mixed", where)
+
+
+@pytest.mark.emu
+def test_emu_intra_cta_kernel():
+    """the CTA-per-block kernel is chosen once per process from B200_INTRA_CTA, so it is checked in a process of its own"""
+    import subprocess, sys
+    code = ("import sys; sys.path[:0] = [%r, %r]\n"
+            "import test_intra\n"
+            "test_intra.check_cta_kernel()\n"
+            "print('RESULT ok')\n") % (refs.ROOT, os.path.dirname(os.path.abspath(__file__)))
+    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=1800,
+                         env=dict(os.environ, B200_INTRA_CTA="1"))
+    assert "RESULT ok" in out.stdout, out.stdout[-2000:] + out.stderr[-4000:]
 
 
 def check_batch(lib, alloc_fn, n, bpc=8, W=136, H=72, with_lf=True):
