@@ -115,7 +115,7 @@ class McScaledBlock(C.Structure):
 
 
 class CoefBlock(C.Structure):
-    _fields_ = [("dense_off", C.c_uint32), ("compact_off", C.c_uint32), ("eob", C.c_int16), ("tx", C.c_uint8), ("pad", C.c_uint8)]
+    _fields_ = [("dense_off", C.c_uint32), ("compact_off", C.c_uint32), ("eob", C.c_int16), ("tx", C.c_uint8), ("tx_class", C.c_uint8)]
 
 
 class IntraTx(C.Structure):

@@ -70,8 +70,14 @@ __device__ __noinline__ void itx_col_pass_shared(const int *tcol, int pitch, typ
     for (int y = 0; y < H; y++) c[y] = y < SH ? tcol[y * pitch] : 0;
     tx1d_apply<H>(c, t_second, col_lo, col_hi);
     if (resid) {
+        // high bit depth: saturated, as in itx_add_warp's DC and WHT paths (|residual| >= 2^15 clips the 12-bit sum exactly
+        // like the full value; 12-bit IDTX with 32-sample columns reaches (131071 * 4 + 8) >> 4 = 32768). The 8-bit column
+        // clip keeps the residual within (32767 * 4 + 8) >> 4 = 8192.
 #pragma unroll
-        for (int y = 0; y < H; y++) resid[y * stride] = (int16_t)((c[y] + 8) >> 4);
+        for (int y = 0; y < H; y++) {
+            if constexpr (HBD) resid[y * stride] = (int16_t)iclip((c[y] + 8) >> 4, -32768, 32767);
+            else resid[y * stride] = (int16_t)((c[y] + 8) >> 4);
+        }
         return;
     }
 #pragma unroll

@@ -950,35 +950,48 @@ def make_intra_frame(rng, bpc, W, H, ss_hor=1, ss_ver=1, p_skip=0.2, p_cfl=0.25,
 
 
 # ---------------------------------------------------------------------------------------------------------
-COEF_BLOCK_DT = np.dtype([("dense_off", "<u4"), ("compact_off", "<u4"), ("eob", "<i2"), ("tx", "u1"), ("pad", "u1")])
+COEF_BLOCK_DT = np.dtype([("dense_off", "<u4"), ("compact_off", "<u4"), ("eob", "<i2"), ("tx", "u1"), ("tx_class", "u1")])
+# TxClass per TxfmType (reference src/tables.c dav1d_tx_type_class): 0 2-D, 1 H_* (TX_CLASS_H), 2 V_* (TX_CLASS_V)
+TX_CLASS = np.array([0] * 10 + [2, 1, 2, 1, 2, 1] + [0], np.int64)
+
+
+def class_scan(tx, cls):
+    """coefficient index of scan position k for a block of TxClass cls, as decode_coefs walks it (reference
+    src/recon_tmpl.c:458-467, 548-576): dav1d_scans[tx] (2-D), k (H), x * sh + y with x = k % sw, y = k / sw (V)"""
+    if cls == 0:
+        return scan_table(tx)
+    sw, sh = _L.tx_coef_dims(tx)
+    k = np.arange(sw * sh, dtype=np.int64)
+    return k if cls == 1 else (k % sw) * sh + k // sw
 
 
 def compact_coefs(S):
     """What a record emitter would ship instead of the dense coefficient plane: per coded transform block the
-    coefficients 0 .. eob in scan order, plus one B200CoefBlock record each (include/b200av1.h). Returns
+    coefficients 0 .. eob in the scan order of its class, plus one B200CoefBlock record each (include/b200av1.h). Returns
     (compact stream, records)."""
     dense = S["coefs"]
     recs, chunks, pos = [], [], 0
-    groups = [(tx, S["itx"][tx]["coef_off"].astype(np.int64), S["itx"][tx]["eob"].astype(np.int64)) for tx in range(19) if len(S["itx"][tx])]
+    groups = [(tx, S["itx"][tx]["coef_off"].astype(np.int64), S["itx"][tx]["eob"].astype(np.int64), TX_CLASS[S["itx"][tx]["txtp"]])
+              for tx in range(19) if len(S["itx"][tx])]
     it = S.get("intra_tx")
     if it is not None and len(it):
         for tx in range(19):
             sel = (it["tx"] == tx) & (it["eob"] >= 0)
             if sel.any():
-                groups.append((tx, it["coef_off"][sel].astype(np.int64), it["eob"][sel].astype(np.int64)))
-    for tx, offs, eobs in groups:
-        scan = scan_table(tx)
+                groups.append((tx, it["coef_off"][sel].astype(np.int64), it["eob"][sel].astype(np.int64), TX_CLASS[it["txtp"][sel]]))
+    for tx, offs, eobs, cls in groups:
+        scans = np.stack([class_scan(tx, c) for c in range(3)])
         n = len(offs)
         cnt = eobs + 1
         # gather dense[off + scan[k]] for k <= eob, block after block
         k = np.arange(int(cnt.max()))[None, :]
         valid = k < cnt[:, None]
-        idx = offs[:, None] + scan[np.minimum(k, len(scan) - 1)]
+        idx = offs[:, None] + scans[cls[:, None], np.minimum(k, scans.shape[1] - 1)]
         chunks.append(dense[idx[valid]])
         a = np.zeros(n, COEF_BLOCK_DT)
         a["dense_off"] = offs
         a["compact_off"] = pos + np.concatenate([[0], np.cumsum(cnt)[:-1]])
-        a["eob"] = eobs; a["tx"] = tx
+        a["eob"] = eobs; a["tx"] = tx; a["tx_class"] = cls
         recs.append(a)
         pos += int(cnt.sum())
     if not recs:

@@ -566,15 +566,17 @@ B200_API int b200_intra_frames(int bitdepth_max, const B200IntraFrame *frames, c
                                const int32_t *n_tx, int n_frames, void *stream);
 
 /* ==== compact coefficient upload ============================================================= */
-/* Per coded transform block the emitter may ship only coefficients 0 .. eob in scan order (dav1d_scans[tx],
- * reference src/scan.c) instead of the dense block: b200_coef_expand scatters them into the (zeroed) dense buffer
- * the transform kernels read. In a B200FrameJob: d_expand / n_expand / d_ccoef / coef_bytes; b200_frame_run then
- * zeroes d_coef[0 .. coef_bytes) and expands before anything else. */
+/* Per coded transform block the emitter may ship only coefficients 0 .. eob in the scan order decode_coefs walks
+ * (reference src/recon_tmpl.c:548-576) instead of the dense block: b200_coef_expand scatters them into the (zeroed)
+ * dense buffer the transform kernels read. In a B200FrameJob: d_expand / n_expand / d_ccoef / coef_bytes; b200_frame_run
+ * then zeroes d_coef[0 .. coef_bytes) and expands before anything else. */
 typedef struct B200CoefBlock {
     uint32_t dense_off;            /* coefficient index of the block in the dense buffer (= its coef_off) */
     uint32_t compact_off;          /* coefficient index of its first value in the compact stream */
     int16_t eob;
-    uint8_t tx, pad;
+    uint8_t tx;
+    uint8_t tx_class;              /* dav1d_tx_type_class[txtp]: 0 2-D (dav1d_scans[tx]), 1 H_* (position k is coefficient
+                                    * k), 2 V_* (position k is coefficient (k % sw) * sh + k / sw; sw, sh = min(w|h, 32)) */
 } B200CoefBlock;
 B200_API int b200_coef_expand(int bitdepth_max, const B200CoefBlock *d_blocks, int n_blocks, const void *d_compact,
                               void *d_dense, void *stream);
