@@ -67,57 +67,63 @@ B200_DEV int cdef_pixel(const typename Bd<HBD>::pixel *__restrict__ plane, int s
     return v;
 }
 
-// direction search over an 8x8 block held in shared memory as (px >> (bitdepth-8)) - 128;
-// lanes 0..7 each own one direction's cost. Returns dir in all lanes, *var likewise.
-B200_DEV int cdef_find_dir(const int *v, int lane, unsigned *var)
+// Direction search (cdef_find_dir_c) of one 8x8 block by an aligned group of 8 lanes of one warp; lane y supplies row y
+// as v[x] = (px >> (bitdepth - 8)) - 128. bins is the block's zeroed 8 x 16 int scratch in shared memory: bins[d * 16 + n]
+// collects the sum along line n of direction d. The slanted lines are accumulated with shared-memory integer atomics
+// (the order does not change a sum), the row sums (d = 2) and column sums (d = 6) are formed in registers. Lane d then
+// evaluates direction d's cost as sum_n w(d, n) * s(d, n)^2, which equals the reference's grouped form modulo 2^32, and the
+// argmax (first index on ties), the opposite cost and var are reduced over the 8 lanes. Returns dir in all 8 lanes, *var likewise.
+B200_HD constexpr unsigned cdef_w04(int n) { return n < 7 ? 840u / (n + 1) : n == 7 ? 105u : 840u / (15 - n); }
+B200_HD constexpr unsigned cdef_wodd(int n) { return n < 3 ? 420u / (n + 1) : n < 8 ? 105u : n < 11 ? 420u / (11 - n) : 0u; }
+B200_DEV int cdef_dir8(const int (&v)[8], int y, int *bins, unsigned *var)
 {
-    unsigned cost = 0;
-    if (lane < 8) {
-        int sums[15];
+    int rs = 0;
 #pragma unroll
-        for (int i = 0; i < 15; i++) sums[i] = 0;
-        for (int i = 0; i < 64; i++) {
-            const int y = i >> 3, x = i & 7, p = v[i];
-            int idx;
-            switch (lane) {
-            case 0: idx = y + x; break;
-            case 1: idx = y + (x >> 1); break;
-            case 2: idx = y; break;
-            case 3: idx = 3 + y - (x >> 1); break;
-            case 4: idx = 7 + y - x; break;
-            case 5: idx = 3 - (y >> 1) + x; break;
-            case 6: idx = x; break;
-            default: idx = (y >> 1) + x; break;
-            }
+    for (int x = 0; x < 8; x++) rs += v[x];
+    bins[2 * 16 + y] = rs;
+    int c[8];                                      // column sums: reduce-scatter over the 8 lanes, lane y ends with column y
 #pragma unroll
-            for (int k = 0; k < 15; k++) if (k == idx) sums[k] += p;
+    for (int x = 0; x < 8; x++) c[x] = v[x];
+#pragma unroll
+    for (int h = 4; h; h >>= 1)
+#pragma unroll
+        for (int k = 0; k < h; k++) {
+            const bool hi = y & h;
+            const int send = hi ? c[k] : c[k + h], keep = hi ? c[k + h] : c[k];
+            c[k] = keep + __shfl_xor_sync(0xffffffffu, send, h, 8);
         }
-        if (lane == 2 || lane == 6) {
+    bins[6 * 16 + y] = c[0];
 #pragma unroll
-            for (int n = 0; n < 8; n++) cost += sums[n] * sums[n];
-            cost *= 105;
-        } else if (lane == 0 || lane == 4) {
-#pragma unroll
-            for (int n = 0; n < 7; n++) cost += (sums[n] * sums[n] + sums[14 - n] * sums[14 - n]) * c_cdef_div[n];
-            cost += sums[7] * sums[7] * 105;
-        } else {
-#pragma unroll
-            for (int m = 0; m < 5; m++) cost += sums[3 + m] * sums[3 + m];
-            cost *= 105;
-#pragma unroll
-            for (int m = 0; m < 3; m++) cost += (sums[m] * sums[m] + sums[10 - m] * sums[10 - m]) * c_cdef_div[2 * m + 1];
-        }
+    for (int x = 0; x < 8; x++) {
+        atomicAdd(&bins[0 * 16 + y + x], v[x]);
+        atomicAdd(&bins[4 * 16 + 7 + y - x], v[x]);
+        atomicAdd(&bins[5 * 16 + 3 - (y >> 1) + x], v[x]);
+        atomicAdd(&bins[7 * 16 + (y >> 1) + x], v[x]);
     }
-    unsigned c[8];
 #pragma unroll
-    for (int n = 0; n < 8; n++) c[n] = __shfl_sync(0xffffffffu, cost, n);
-    int best = 0; unsigned bc = c[0];
+    for (int j = 0; j < 4; j++) {
+        const int q = v[2 * j] + v[2 * j + 1];
+        atomicAdd(&bins[1 * 16 + y + j], q);
+        atomicAdd(&bins[3 * 16 + 3 + y - j], q);
+    }
+    __syncwarp();
+    const int d = y;
+    unsigned cost = 0;
 #pragma unroll
-    for (int n = 1; n < 8; n++) if (c[n] > bc) { bc = c[n]; best = n; }
-    unsigned opp = c[0];
+    for (int n = 0; n < 15; n++) {
+        const int s = bins[d * 16 + n];
+        const unsigned w = (d & 1) ? cdef_wodd(n) : (d & 2) ? (n < 8 ? 105u : 0u) : cdef_w04(n);
+        cost += (unsigned)(s * s) * w;
+    }
+    unsigned bc = cost;
+    int best = d;
 #pragma unroll
-    for (int n = 1; n < 8; n++) if (n == (best ^ 4)) opp = c[n];
-    if ((best ^ 4) == 0) opp = c[0];
+    for (int m = 1; m < 8; m <<= 1) {
+        const unsigned oc = __shfl_xor_sync(0xffffffffu, bc, m, 8);
+        const int ob = __shfl_xor_sync(0xffffffffu, best, m, 8);
+        if (oc > bc || (oc == bc && ob < best)) { bc = oc; best = ob; }
+    }
+    const unsigned opp = __shfl_sync(0xffffffffu, cost, best ^ 4, 8);
     *var = (bc - opp) >> 10;
     return best;
 }
@@ -146,45 +152,14 @@ constexpr unsigned kCdefSentinel = 0xC000u;
 struct CdefBlockInfo { int16_t y_pri, y_sec, uv_pri, uv_sec; int8_t y_dir, uv_dir, inside, pad;
                        uint8_t y_pri_shift, y_sec_shift, uv_pri_shift, uv_sec_shift; };   // constrain shifts, computed once per block
 
+constexpr int kCdefBins = 8 * 16 + 8;           // per-block direction-search scratch (ints); the pad staggers the blocks' banks
+
 struct CdefShared {
     uint32_t tile[3][kCdefRows * kCdefPitch];   // pair rows -2 .. TH, columns -4 .. TW+3
+    int bins[32][kCdefBins];
     CdefBlockInfo info[32];
     int16_t off[8][2];                          // word offset of direction d, tap k (filled per plane pitch: constant pitch)
 };
-
-template <int D> B200_DEV unsigned cdef_dir_cost(const int (&v)[8][8])
-{
-    constexpr int NB = (D == 2 || D == 6) ? 8 : (D == 0 || D == 4) ? 15 : 11;
-    int sums[NB];
-#pragma unroll
-    for (int i = 0; i < NB; i++) sums[i] = 0;
-#pragma unroll
-    for (int y = 0; y < 8; y++)
-#pragma unroll
-        for (int x = 0; x < 8; x++) {
-            constexpr int dummy = 0; (void)dummy;
-            const int idx = D == 0 ? y + x : D == 1 ? y + (x >> 1) : D == 2 ? y : D == 3 ? 3 + y - (x >> 1)
-                          : D == 4 ? 7 + y - x : D == 5 ? 3 - (y >> 1) + x : D == 6 ? x : (y >> 1) + x;
-            sums[idx] += v[y][x];
-        }
-    unsigned cost = 0;
-    if (D == 2 || D == 6) {
-#pragma unroll
-        for (int n = 0; n < 8; n++) cost += sums[n] * sums[n];
-        cost *= 105;
-    } else if (D == 0 || D == 4) {
-#pragma unroll
-        for (int n = 0; n < 7; n++) cost += (sums[n] * sums[n] + sums[14 - n] * sums[14 - n]) * c_cdef_div[n];
-        cost += sums[7] * sums[7] * 105;
-    } else {
-#pragma unroll
-        for (int m = 0; m < 5; m++) cost += sums[3 + m] * sums[3 + m];
-        cost *= 105;
-#pragma unroll
-        for (int m = 0; m < 3; m++) cost += (sums[m] * sums[m] + sums[10 - m] * sums[10 - m]) * c_cdef_div[2 * m + 1];
-    }
-    return cost;
-}
 
 // one tap pair (+off / -off) on two packed pixels
 B200_DEV void cdef_tap2(const uint32_t *t, int idx, int off, unsigned negpx, unsigned thr1, int shift, unsigned smask, int tap,
@@ -204,6 +179,11 @@ B200_DEV void cdef_tap2(const uint32_t *t, int idx, int off, unsigned negpx, uns
     }
 }
 
+// 8-bit: the low bytes of four packed pairs' halves as one row word (sel 0x0040 / 0x0062 picks the low / high halves)
+B200_DEV unsigned cdef_row8(const unsigned (&o)[4], unsigned sel) {
+    return __byte_perm(__byte_perm(o[0], o[1], sel), __byte_perm(o[2], o[3], sel), 0x5410);
+}
+
 template <bool HBD>
 #ifndef B200_CDEF_MINB
 #define B200_CDEF_MINB 4
@@ -218,161 +198,175 @@ __global__ void __launch_bounds__(kCdefThreads, B200_CDEF_MINB) cdef_frame_kerne
     const int b8 = HBD ? (32 - __clz(bdmax)) - 8 : 0;
     const pixel *const src = (const pixel *)f.src;
     pixel *const dst = (pixel *)f.dst;
+    const int ssh = f.ss_hor, ssv = f.ss_ver;
 
-    // ---- stage the three planes (4 samples of two consecutive rows per thread and step)
-#pragma unroll 1
-    for (int pl = 0; pl < 3; pl++) {
-        const int sh = pl ? f.ss_hor : 0, sv = pl ? f.ss_ver : 0;
-        const int tw = kCdefTW >> sh, th = kCdefTH >> sv;
-        const int availw = ((f.bw + 1) >> 1) * 8 >> sh, availh = ((f.bh + 1) >> 1) * 8 >> sv;
-        const int x0 = bx0 * 4 >> sh, y0 = by0 * 4 >> sv;
-        const int groups = (tw + 8) >> 2, rows = th + 3;
-        const pixel *sp = src + f.plane_off[pl];
-        const int st = f.stride[pl];
-        const unsigned magic = recip16(groups);            // exact i / groups for i < 36 * 18
-        for (int i = tid; i < groups * rows; i += kCdefThreads) {
-            const int r = (int)((i * magic) >> 16), g = i - r * groups;
-            const int x = x0 - 4 + g * 4, y = y0 - 2 + r;
-            uint4 w;
-            w.x = w.y = w.z = w.w = kCdefSentinel * 0x00010001u;
-            if (x >= 0 && x < availw) {
-                const bool ha = y >= 0 && y < availh, hb = y + 1 >= 0 && y + 1 < availh;
+    // the 8 lanes of 8x8 block b = tid / 8 look up its strengths; the loads are in flight during the staging
+    const int blk = tid >> 3, brow = tid & 7, bxi = blk & 7, byi = blk >> 3;
+    const int bx = bx0 + bxi * 2, by = by0 + byi * 2;
+    const bool inside = bx < f.bw && by < f.bh;
+    int y_lvl = 0, uv_lvl = 0;
+    if (inside) {
+        const B200Av1Filter &m = f.mask[(by >> 5) * f.sb128w + (bx >> 5)];
+        const int cdef_idx = m.cdef_idx[((by & 16) >> 3) + ((bx & 16) >> 4)];
+        const uint16_t *nr = m.noskip_mask[(by & 30) >> 1];
+        const unsigned noskip = (unsigned)nr[1] << 16 | nr[0];
+        if (cdef_idx != -1 && (noskip & (3u << (bx & 30)))) { y_lvl = f.y_strength[cdef_idx]; uv_lvl = f.uv_strength[cdef_idx]; }
+    }
+
+    // ---- stage the three planes: one flat list of items (4 samples of two consecutive rows); a thread issues the
+    // loads of up to 4 items before it stores any of them, so a 4:2:0 tile is staged with all its loads in flight
+    {
+        const int cw = kCdefTW >> ssh, ch = kCdefTH >> ssv;
+        const int g0 = (kCdefTW + 8) >> 2, n0 = g0 * (kCdefTH + 3);
+        const int gc = (cw + 8) >> 2, nc = gc * (ch + 3);
+        const unsigned magic0 = recip16(g0), magicc = recip16(gc);   // exact i / groups for i < 36 * 18
+        const int total = n0 + 2 * nc;
+        for (int base = 0; base < total; base += 4 * kCdefThreads) {
+            unsigned qa[4][HBD ? 2 : 1], qb[4][HBD ? 2 : 1];
+            int dsti[4]; bool ha[4], hb[4];
+#pragma unroll
+            for (int u = 0; u < 4; u++) {
+                int i = base + u * kCdefThreads + tid, pl = 0;
+                if (i >= n0) { i -= n0; pl = 1; if (i >= nc) { i -= nc; pl = 2; } }
+                const int sh = pl ? ssh : 0, sv = pl ? ssv : 0, groups = pl ? gc : g0;
+                const int r = (int)((i * (pl ? magicc : magic0)) >> 16), g = i - r * groups;
+                const int availw = ((f.bw + 1) >> 1) * 8 >> sh, availh = ((f.bh + 1) >> 1) * 8 >> sv;
+                const int x = (bx0 * 4 >> sh) - 4 + g * 4, y = (by0 * 4 >> sv) - 2 + r;
+                const bool ok = base + u * kCdefThreads + tid < total && x >= 0 && x < availw;
+                dsti[u] = base + u * kCdefThreads + tid < total ? pl * (kCdefRows * kCdefPitch) + r * kCdefPitch + g * 4 : -1;
+                ha[u] = ok && y >= 0 && y < availh;
+                hb[u] = ok && y + 1 >= 0 && y + 1 < availh;
+                const pixel *sp = src + f.plane_off[pl] + x;
+                const int st = f.stride[pl];
+#pragma unroll
+                for (int k = 0; k < (HBD ? 2 : 1); k++) qa[u][k] = qb[u][k] = HBD ? kCdefSentinel * 0x00010001u : 0u;
                 if (HBD) {
-                    uint2 qa, qb;
-                    qa.x = qa.y = qb.x = qb.y = kCdefSentinel * 0x00010001u;
-                    if (ha) qa = *(const uint2 *)(sp + (ptrdiff_t)y * st + x);
-                    if (hb) qb = *(const uint2 *)(sp + (ptrdiff_t)(y + 1) * st + x);
-                    // (a0 a1 | a2 a3) x (b0 b1 | b2 b3) -> (a0 b0) (a1 b1) (a2 b2) (a3 b3): one byte permute each
-                    w.x = __byte_perm(qa.x, qb.x, 0x5410); w.y = __byte_perm(qa.x, qb.x, 0x7632);
-                    w.z = __byte_perm(qa.y, qb.y, 0x5410); w.w = __byte_perm(qa.y, qb.y, 0x7632);
+                    if (ha[u]) { const uint2 q = *(const uint2 *)(sp + (ptrdiff_t)y * st); qa[u][0] = q.x; qa[u][HBD] = q.y; }
+                    if (hb[u]) { const uint2 q = *(const uint2 *)(sp + (ptrdiff_t)(y + 1) * st); qb[u][0] = q.x; qb[u][HBD] = q.y; }
                 } else {
-                    const unsigned sent4 = 0;         // per-byte sentinel impossible: handled after the permutes
-                    unsigned qa = sent4, qb = sent4;
-                    if (ha) qa = *(const unsigned *)(sp + (ptrdiff_t)y * st + x);
-                    if (hb) qb = *(const unsigned *)(sp + (ptrdiff_t)(y + 1) * st + x);
-                    // bytes a_k, b_k -> halfwords (a_k | b_k << 16): two byte permutes per word
-                    const unsigned t01 = __byte_perm(qa, qb, 0x5140), t23 = __byte_perm(qa, qb, 0x7362);   // a0 b0 a1 b1 | a2 b2 a3 b3
-                    w.x = __byte_perm(t01, 0, 0x4140); w.y = __byte_perm(t01, 0, 0x4342);
-                    w.z = __byte_perm(t23, 0, 0x4140); w.w = __byte_perm(t23, 0, 0x4342);
-                    if (!ha) { w.x = (w.x & 0xffff0000u) | kCdefSentinel; w.y = (w.y & 0xffff0000u) | kCdefSentinel; w.z = (w.z & 0xffff0000u) | kCdefSentinel; w.w = (w.w & 0xffff0000u) | kCdefSentinel; }
-                    if (!hb) { w.x = (w.x & 0xffffu) | kCdefSentinel << 16; w.y = (w.y & 0xffffu) | kCdefSentinel << 16; w.z = (w.z & 0xffffu) | kCdefSentinel << 16; w.w = (w.w & 0xffffu) | kCdefSentinel << 16; }
+                    if (ha[u]) qa[u][0] = *(const unsigned *)(sp + (ptrdiff_t)y * st);
+                    if (hb[u]) qb[u][0] = *(const unsigned *)(sp + (ptrdiff_t)(y + 1) * st);
                 }
             }
-            *(uint4 *)&S.tile[pl][r * kCdefPitch + g * 4] = w;
+#pragma unroll
+            for (int u = 0; u < 4; u++) {
+                if (dsti[u] < 0) continue;
+                uint4 w;
+                if (HBD) {
+                    // (a0 a1 | a2 a3) x (b0 b1 | b2 b3) -> (a0 b0) (a1 b1) (a2 b2) (a3 b3): one byte permute each
+                    w.x = __byte_perm(qa[u][0], qb[u][0], 0x5410); w.y = __byte_perm(qa[u][0], qb[u][0], 0x7632);
+                    w.z = __byte_perm(qa[u][HBD], qb[u][HBD], 0x5410); w.w = __byte_perm(qa[u][HBD], qb[u][HBD], 0x7632);
+                } else {
+                    // bytes a_k, b_k -> halfwords (a_k | b_k << 16): two byte permutes per word; the sentinel replaces
+                    // missing rows afterwards (a per-byte sentinel is impossible)
+                    const unsigned t01 = __byte_perm(qa[u][0], qb[u][0], 0x5140), t23 = __byte_perm(qa[u][0], qb[u][0], 0x7362);
+                    w.x = __byte_perm(t01, 0, 0x4140); w.y = __byte_perm(t01, 0, 0x4342);
+                    w.z = __byte_perm(t23, 0, 0x4140); w.w = __byte_perm(t23, 0, 0x4342);
+                    if (!ha[u]) { w.x = (w.x & 0xffff0000u) | kCdefSentinel; w.y = (w.y & 0xffff0000u) | kCdefSentinel; w.z = (w.z & 0xffff0000u) | kCdefSentinel; w.w = (w.w & 0xffff0000u) | kCdefSentinel; }
+                    if (!hb[u]) { w.x = (w.x & 0xffffu) | kCdefSentinel << 16; w.y = (w.y & 0xffffu) | kCdefSentinel << 16; w.z = (w.z & 0xffffu) | kCdefSentinel << 16; w.w = (w.w & 0xffffu) | kCdefSentinel << 16; }
+                }
+                *(uint4 *)&S.tile[0][dsti[u]] = w;
+            }
         }
     }
+    for (int i = tid; i < 32 * kCdefBins / 4; i += kCdefThreads) ((uint4 *)S.bins)[i] = make_uint4(0, 0, 0, 0);
     if (tid < 16) {
         const int d = tid >> 1, k = tid & 1;
         S.off[d][k] = (int16_t)(c_cdef_off[d][k][0] * kCdefPitch + c_cdef_off[d][k][1]);
     }
     __syncthreads();
 
-    // ---- per-8x8 parameters: one thread per block (direction search over all 8 directions)
-    if (tid < 32) {
-        const int bxi = tid & 7, byi = tid >> 3;
-        const int bx = bx0 + bxi * 2, by = by0 + byi * 2;
-        CdefBlockInfo bi; bi.y_pri = bi.y_sec = bi.uv_pri = bi.uv_sec = 0; bi.y_dir = bi.uv_dir = 0; bi.pad = 0;
-        bi.inside = bx < f.bw && by < f.bh;
-        if (bi.inside) {
-            int y_lvl = 0, uv_lvl = 0;
-            const B200Av1Filter &m = f.mask[(by >> 5) * f.sb128w + (bx >> 5)];
-            const int cdef_idx = m.cdef_idx[((by & 16) >> 3) + ((bx & 16) >> 4)];
-            const uint16_t *nr = m.noskip_mask[(by & 30) >> 1];
-            const unsigned noskip = (unsigned)nr[1] << 16 | nr[0];
-            if (cdef_idx != -1 && (noskip & (3u << (bx & 30)))) { y_lvl = f.y_strength[cdef_idx]; uv_lvl = f.uv_strength[cdef_idx]; }
+    // ---- per-8x8 parameters: 8 lanes per block, lane y supplies the block's row y to the direction search
+    {
+        const uint32_t *t = &S.tile[0][(2 + byi * 8 + brow) * kCdefPitch + 4 + bxi * 8];
+        const uint4 w0 = *(const uint4 *)t, w1 = *(const uint4 *)(t + 4);
+        const unsigned wr[8] = { w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w };
+        int v[8];
+#pragma unroll
+        for (int x = 0; x < 8; x++) v[x] = (int)((wr[x] & 0xffff) >> b8) - 128;
+        unsigned var;
+        const int dir = cdef_dir8(v, brow, S.bins[blk], &var);
+        if (brow == 0) {
+            CdefBlockInfo bi; bi.y_pri = bi.y_sec = bi.uv_pri = bi.uv_sec = 0; bi.y_dir = bi.uv_dir = 0; bi.pad = 0;
+            bi.inside = inside;
             const int y_pri = (y_lvl >> 2) << b8;
             int y_sec = y_lvl & 3; y_sec += y_sec == 3; y_sec <<= b8;
             const int uv_pri = (uv_lvl >> 2) << b8;
             int uv_sec = uv_lvl & 3; uv_sec += uv_sec == 3; uv_sec <<= b8;
-            int dir = 0; unsigned var = 0;
-            if (y_pri || uv_pri) {
-                int v[8][8];
-                const uint32_t *t = &S.tile[0][(2 + byi * 8) * kCdefPitch + 4 + bxi * 8];
-#pragma unroll
-                for (int y = 0; y < 8; y += 2)
-#pragma unroll
-                    for (int x = 0; x < 8; x++) {
-                        const unsigned w = t[y * kCdefPitch + x];
-                        v[y][x] = (int)((w & 0xffff) >> b8) - 128;
-                        v[y + 1][x] = (int)((w >> 16) >> b8) - 128;
-                    }
-                unsigned c[8];
-                c[0] = cdef_dir_cost<0>(v); c[1] = cdef_dir_cost<1>(v); c[2] = cdef_dir_cost<2>(v); c[3] = cdef_dir_cost<3>(v);
-                c[4] = cdef_dir_cost<4>(v); c[5] = cdef_dir_cost<5>(v); c[6] = cdef_dir_cost<6>(v); c[7] = cdef_dir_cost<7>(v);
-                unsigned bc = c[0];
-#pragma unroll
-                for (int n = 1; n < 8; n++) if (c[n] > bc) { bc = c[n]; dir = n; }
-                unsigned opp = 0;
-#pragma unroll
-                for (int n = 0; n < 8; n++) if (n == (dir ^ 4)) opp = c[n];
-                var = (bc - opp) >> 10;
-            }
             if (y_pri) { bi.y_pri = (int16_t)cdef_adjust_strength(y_pri, var); bi.y_sec = (int16_t)y_sec; bi.y_dir = (int8_t)dir; }
             else bi.y_sec = (int16_t)y_sec;
             if (uv_lvl) {
                 bi.uv_pri = (int16_t)uv_pri; bi.uv_sec = (int16_t)uv_sec;
-                bi.uv_dir = (int8_t)(uv_pri ? ((f.ss_hor && !f.ss_ver) ? c_uv_dir422[dir] : dir) : 0);
+                bi.uv_dir = (int8_t)(uv_pri ? ((ssh && !ssv) ? c_uv_dir422[dir] : dir) : 0);
             }
-        }
-        {   // shift = max(0, damping - ulog2(strength)) per class (luma damping, chroma damping - 1)
+            // shift = max(0, damping - ulog2(strength)) per class (luma damping, chroma damping - 1)
             const int dl = f.damping + b8, dc = dl - 1;
             bi.y_pri_shift = (uint8_t)(bi.y_pri ? imax(0, dl - ulog2(bi.y_pri)) : 0);
             bi.y_sec_shift = (uint8_t)(bi.y_sec ? dl - ulog2(bi.y_sec) : 0);
             bi.uv_pri_shift = (uint8_t)(bi.uv_pri ? imax(0, dc - ulog2(bi.uv_pri)) : 0);
             bi.uv_sec_shift = (uint8_t)(bi.uv_sec ? dc - ulog2(bi.uv_sec) : 0);
+            S.info[blk] = bi;
         }
-        S.info[tid] = bi;
     }
     __syncthreads();
 
-    // ---- filter: one thread per vertical pixel pair
-#pragma unroll 1
-    for (int pl = 0; pl < 3; pl++) {
-        const int sh = pl ? f.ss_hor : 0, sv = pl ? f.ss_ver : 0;
-        const int tw = kCdefTW >> sh, th = kCdefTH >> sv;
-        const int x0 = bx0 * 4 >> sh, y0 = by0 * 4 >> sv;
-        pixel *dp = dst + f.plane_off[pl];
-        const int st = f.stride[pl];
+    // ---- filter: a thread takes 4 adjacent columns of one vertical pixel pair (a group never straddles an 8x8 block, so
+    // the block's parameters and tap offsets are decoded once) and writes each of the two rows with one store.
+    // Items: the luma tile's 16 x 16 groups, then each chroma plane's (16 >> ss_hor) x (16 >> ss_ver).
+    const int cgl = 4 - ssh, nc = 1 << (cgl + 4 - ssv);
+    for (int i = tid; i < 256 + 2 * nc; i += kCdefThreads) {
+        int pl = 0, li = i;
+        if (li >= 256) { li -= 256; pl = 1; if (li >= nc) { li -= nc; pl = 2; } }
+        const int sh = pl ? ssh : 0, sv = pl ? ssv : 0, gl = pl ? cgl : 4;
+        const int y = (li >> gl) * 2, x = (li & ((1 << gl) - 1)) * 4;
+        const CdefBlockInfo bi = S.info[(y >> (3 - sv)) * 8 + (x >> (3 - sh))];
+        if (!bi.inside) continue;
         const uint32_t *t = S.tile[pl];
-        const int twl = 6 - sh;                                   // tw = 64 >> sh is a power of two
-        for (int i = tid; i < tw * (th >> 1); i += kCdefThreads) {
-            const int yp = i >> twl, x = i & (tw - 1), y = yp * 2;
-            const CdefBlockInfo bi = S.info[(y >> (3 - sv)) * 8 + (x >> (3 - sh))];
-            if (!bi.inside) continue;
-            const int idx = (y + 2) * kCdefPitch + x + 4;
-            const unsigned px2 = t[idx];
-            int o0 = px2 & 0xffff, o1 = px2 >> 16;
-            const int pri = pl ? bi.uv_pri : bi.y_pri, sec = pl ? bi.uv_sec : bi.y_sec, dir = pl ? bi.uv_dir : bi.y_dir;
-            if (pri | sec) {
+        const int idx = (y + 2) * kCdefPitch + x + 4;
+        const uint4 pw = *(const uint4 *)&t[idx];
+        unsigned o[4] = { pw.x, pw.y, pw.z, pw.w };              // (row y | row y + 1 << 16) per column
+        const int pri = pl ? bi.uv_pri : bi.y_pri, sec = pl ? bi.uv_sec : bi.y_sec, dir = pl ? bi.uv_dir : bi.y_dir;
+        if (pri | sec) {
+            const int pshift = pl ? bi.uv_pri_shift : bi.y_pri_shift, sshift = pl ? bi.uv_sec_shift : bi.y_sec_shift;
+            const unsigned pthr1 = (unsigned)(pri + 1) * 0x00010001u, psmask = (0xffffu >> pshift) * 0x00010001u;
+            const unsigned sthr1 = (unsigned)(sec + 1) * 0x00010001u, ssmask = (0xffffu >> sshift) * 0x00010001u;
+            const int tap0 = 4 - ((pri >> b8) & 1);
+            const int d2 = (dir + 2) & 7, d6 = (dir + 6) & 7;
+            const int op0 = S.off[dir][0], op1 = S.off[dir][1];
+            const int os20 = S.off[d2][0], os60 = S.off[d6][0], os21 = S.off[d2][1], os61 = S.off[d6][1];
+#pragma unroll
+            for (int c = 0; c < 4; c++) {
+                const unsigned px2 = o[c];
                 const unsigned negpx = __vadd2(~px2, 0x00010001u);
                 unsigned sumP = 0, sumN = 0, mx = px2, mn = px2;
                 if (pri) {
-                    const int shift = pl ? bi.uv_pri_shift : bi.y_pri_shift;
-                    const unsigned thr1 = (unsigned)(pri + 1) * 0x00010001u, smask = (0xffffu >> shift) * 0x00010001u;
-                    const int tap0 = 4 - ((pri >> b8) & 1);
-                    cdef_tap2(t, idx, S.off[dir][0], negpx, thr1, shift, smask, tap0, sumP, sumN, mx, mn);
-                    cdef_tap2(t, idx, S.off[dir][1], negpx, thr1, shift, smask, (tap0 & 3) | 2, sumP, sumN, mx, mn);
+                    cdef_tap2(t, idx + c, op0, negpx, pthr1, pshift, psmask, tap0, sumP, sumN, mx, mn);
+                    cdef_tap2(t, idx + c, op1, negpx, pthr1, pshift, psmask, (tap0 & 3) | 2, sumP, sumN, mx, mn);
                 }
                 if (sec) {
-                    const int shift = pl ? bi.uv_sec_shift : bi.y_sec_shift;
-                    const unsigned thr1 = (unsigned)(sec + 1) * 0x00010001u, smask = (0xffffu >> shift) * 0x00010001u;
-                    const int d2 = (dir + 2) & 7, d6 = (dir + 6) & 7;
-                    cdef_tap2(t, idx, S.off[d2][0], negpx, thr1, shift, smask, 2, sumP, sumN, mx, mn);
-                    cdef_tap2(t, idx, S.off[d6][0], negpx, thr1, shift, smask, 2, sumP, sumN, mx, mn);
-                    cdef_tap2(t, idx, S.off[d2][1], negpx, thr1, shift, smask, 1, sumP, sumN, mx, mn);
-                    cdef_tap2(t, idx, S.off[d6][1], negpx, thr1, shift, smask, 1, sumP, sumN, mx, mn);
+                    cdef_tap2(t, idx + c, os20, negpx, sthr1, sshift, ssmask, 2, sumP, sumN, mx, mn);
+                    cdef_tap2(t, idx + c, os60, negpx, sthr1, sshift, ssmask, 2, sumP, sumN, mx, mn);
+                    cdef_tap2(t, idx + c, os21, negpx, sthr1, sshift, ssmask, 1, sumP, sumN, mx, mn);
+                    cdef_tap2(t, idx + c, os61, negpx, sthr1, sshift, ssmask, 1, sumP, sumN, mx, mn);
                 }
                 const int s0 = (int)(sumP & 0xffff) - (int)(sumN & 0xffff), s1 = (int)(sumP >> 16) - (int)(sumN >> 16);
-                o0 += (s0 - (s0 < 0) + 8) >> 4;
-                o1 += (s1 - (s1 < 0) + 8) >> 4;
+                int o0 = (int)(px2 & 0xffff) + ((s0 - (s0 < 0) + 8) >> 4);
+                int o1 = (int)(px2 >> 16) + ((s1 - (s1 < 0) + 8) >> 4);
                 if (pri && sec) {
                     o0 = iclip(o0, (int)(mn & 0xffff), (int)(mx & 0xffff));
                     o1 = iclip(o1, (int)(mn >> 16), (int)(mx >> 16));
                 }
+                o[c] = (unsigned)o0 | (unsigned)o1 << 16;
             }
-            pixel *o = dp + (ptrdiff_t)(y0 + y) * st + x0 + x;
-            o[0] = (pixel)o0;
-            o[st] = (pixel)o1;
+        }
+        const int st = f.stride[pl];
+        pixel *op = dst + f.plane_off[pl] + (ptrdiff_t)((by0 * 4 >> sv) + y) * st + (bx0 * 4 >> sh) + x;
+        if (HBD) {
+            *(uint2 *)op = make_uint2(__byte_perm(o[0], o[1], 0x5410), __byte_perm(o[2], o[3], 0x5410));
+            *(uint2 *)(op + st) = make_uint2(__byte_perm(o[0], o[1], 0x7632), __byte_perm(o[2], o[3], 0x7632));
+        } else {
+            *(unsigned *)op = cdef_row8(o, 0x0040);
+            *(unsigned *)(op + st) = cdef_row8(o, 0x0062);
         }
     }
 }
@@ -398,12 +392,17 @@ __global__ void cdef_fb_kernel(const typename Bd<HBD>::pixel *win, typename Bd<H
 template <bool HBD>
 __global__ void cdef_dir_kernel(const typename Bd<HBD>::pixel *img, int *out, int bdmax)
 {
-    __shared__ int v[64];
+    // the four 8-lane groups of the warp each search the same block
+    __shared__ int bins[4][8 * 16];
     const int b8 = HBD ? (32 - __clz(bdmax)) - 8 : 0;
-    for (int i = threadIdx.x; i < 64; i += 32) v[i] = ((int)img[i] >> b8) - 128;
+    const int g = threadIdx.x >> 3, y = threadIdx.x & 7;
+    for (int i = y; i < 8 * 16; i += 8) bins[g][i] = 0;
+    int v[8];
+#pragma unroll
+    for (int x = 0; x < 8; x++) v[x] = ((int)img[y * 8 + x] >> b8) - 128;
     __syncwarp();
     unsigned var;
-    const int d = cdef_find_dir(v, threadIdx.x, &var);
+    const int d = cdef_dir8(v, y, bins[g], &var);
     if (threadIdx.x == 0) { out[0] = d; out[1] = (int)var; }
 }
 
@@ -412,13 +411,14 @@ __global__ void cdef_dir_kernel(const typename Bd<HBD>::pixel *img, int *out, in
 using namespace b200;
 
 namespace b200 {
-// tile rows [t0, t1) of the sweep: a tile row is 32 luma rows (16 subsampled chroma rows) and reads 2 rows beyond each side
+// tile rows [t0, t1) of the sweep: a tile row is 32 luma rows (16 subsampled chroma rows) and reads 2 rows beyond each side;
+// the tile loader reads and the filter writes 4 samples at a time
 int cdef_frame_rows(int bdmax, const B200CdefFrame *f, int t0, int t1, cudaStream_t stream)
 {
     if (int r = check_bdmax(bdmax, "b200_cdef_frame")) return r;
     const size_t px = bdmax > 255 ? 2 : 1;
-    for (int pl = 0; pl < 3; pl++)   // the tile loader reads 4 samples at a time
-        if ((f->stride[pl] & 3) || (f->plane_off[pl] & 3) || ((uintptr_t)f->src * 1 % (4 * px))) { b200_set_error("b200_cdef_frame: planes must be 4-sample aligned"); return -2; }
+    for (int pl = 0; pl < 3; pl++)
+        if ((f->stride[pl] & 3) || (f->plane_off[pl] & 3) || ((uintptr_t)f->src % (4 * px)) || ((uintptr_t)f->dst % (4 * px))) { b200_set_error("b200_cdef_frame: planes must be 4-sample aligned"); return -2; }
     t0 = imax(t0, 0); t1 = imin(t1, (f->bh + 7) / 8);
     if (t1 <= t0) return 0;
     return launch_hbd(bdmax, Launch::pdl, dim3((f->bw + 15) / 16, t1 - t0), dim3(kCdefThreads), 0, stream,

@@ -173,18 +173,35 @@ B200_DEV void lr_tile_compute(LrShared &sm, const LrTileParams &P, int tw, int t
                 t3b[k] = (mb[k + 1] + mb[k] + mb[k + 2] + vb[k + 1]) * 4 + (vb[k] + vb[k + 2]) * 3;
             }
         }
+        int out[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) {
-            if (x + k >= tw) break;
             const int src = sm.src[y + 3][x + k + 3];
             int t5 = 0, t3 = 0;
             if (P.s0) t5 = !(y & 1) ? (t5b[k] - t5a[k] * src + (1 << 8)) >> 9 : (t5b[k] - t5a[k] * src + (1 << 7)) >> 8;
             if (P.s1) t3 = (t3b[k] - t3a[k] * src + (1 << 8)) >> 9;
             const int v = P.w0 * t5 + P.w1 * t3;     // the unused term is zero (w0 = 0 without s0; t3 = 0 without s1)
-            store(x + k, y, iclip(src + ((v + (1 << 10)) >> 11), 0, bdmax));
+            out[k] = iclip(src + ((v + (1 << 10)) >> 11), 0, bdmax);
         }
+        store.row4(x, y, out, imin(4, tw - x));
     }
 }
+
+// where lr_tile_compute writes: sample (x, y) of the tile, or 4 consecutive samples of a row of which the first n are inside
+template <class pixel> struct LrStore {
+    pixel *o; ptrdiff_t st;   // tile origin and row pitch
+    B200_DEV void operator()(int x, int y, int v) const { o[y * st + x] = (pixel)v; }
+    B200_DEV void row4(int x, int y, const int (&v)[4], int n) const {
+        pixel *p = o + y * st + x;
+        if (n == 4 && !((uintptr_t)p & (4 * sizeof(pixel) - 1))) {
+            if (sizeof(pixel) == 1) *(unsigned *)p = (unsigned)v[0] | (unsigned)v[1] << 8 | (unsigned)v[2] << 16 | (unsigned)v[3] << 24;
+            else *(uint2 *)p = make_uint2((unsigned)v[0] | (unsigned)v[1] << 16, (unsigned)v[2] | (unsigned)v[3] << 16);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++) if (k < n) p[k] = (pixel)v[k];
+        }
+    }
+};
 
 B200_DEV void lr_unit_params(const B200RestorationUnit &u, bool hbd, LrTileParams &P)
 {
@@ -238,13 +255,22 @@ __global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __gri
     pixel *O = (pixel *)f.dst + f.plane_off[pl];
     const int st = f.stride[pl];
 
-    // the unit lookup and the tap / weight set-up are per-tile work: one thread does them, the tile reads them from
-    // shared memory (they used to be a quarter of the kernel's instructions, executed by all 256 threads)
+    const bool have_top = y0s > 0, have_bot = y1s < h;
+    constexpr int PPW = HBD ? 2 : 4;                                 // samples per 32-bit word
+    // interior tiles are staged from aligned words over picture columns x0-4 .. x0+tw+3 (one more column on each
+    // side than needed); the copy of an unrestored interior tile writes the same words
+    const bool interior = x0 >= 4 && x0 + tw + 4 <= w && !(tw & 3) && !(x0 & 3) && !(st & (PPW - 1)) &&
+                          !(((uintptr_t)C | (uintptr_t)D | (uintptr_t)O) & 3);
+    const int NW = (tw + 8) / PPW;
+    const unsigned magic = recip16(NW);                   // exact i / NW for i < 38 * 36
+
+    // The unit lookup and the tap / weight set-up are per-tile work: thread 0 starts them, the loads of the interior
+    // staging are issued by every thread while its lr_mask load is in flight, and the tile reads the parameters from
+    // shared memory after one barrier.
     __shared__ LrTileParams sP;
-    if (threadIdx.x == 0) {
-    LrTileParams P;
-    P.type = 0;
-    if (f.restore_planes & (1 << pl)) {
+    B200RestorationUnit u;
+    u.type = 0;
+    if (threadIdx.x == 0 && (f.restore_planes & (1 << pl))) {
         // unit lookup: reference src/lr_apply_tmpl.c:107-148
         int n_full = 0;
         { const int max_unit = unit + half; if (w >= max_unit) n_full = (w - max_unit) / unit + 1; }
@@ -256,14 +282,44 @@ __global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __gri
         aligned <<= ssv;
         const int sb_idx = (aligned >> 7) * f.sr_sb128w, unit_idx = ((aligned >> 6) & 1) << 1;
         const int shift_hor = 7 - ssh;
-        const B200RestorationUnit u = f.lr_mask[sb_idx + (xu >> shift_hor)].lr[pl][unit_idx + ((xu >> (shift_hor - 1)) & 1)];
-        lr_unit_params(u, HBD, P);
+        u = f.lr_mask[sb_idx + (xu >> shift_hor)].lr[pl][unit_idx + ((xu >> (shift_hor - 1)) & 1)];
     }
-    sP = P;
+    constexpr int NI = HBD ? 6 : 3;                       // ceil(38 * 72 / PPW / 256) words per thread
+    unsigned wv[NI];
+    if (interior) {
+#pragma unroll
+        for (int n = 0; n < NI; n++) {
+            const int i = threadIdx.x + n * 256;
+            const int yy = (int)((i * magic) >> 16), g = i - yy * NW;
+            if (yy >= th + 6) break;
+            int Y = ty0 - 3 + yy;
+            const pixel *base = C;
+            if (Y < y0s) {
+                if (have_top) { base = D; Y = imax(Y, y0s - 2); } else Y = y0s;
+            } else if (Y >= y1s) {
+                if (have_bot) { base = D; Y = imin(imin(Y, y1s + 1), h - 1); } else Y = y1s - 1;
+            }
+            wv[n] = *(const unsigned *)(base + (ptrdiff_t)Y * st + x0 - 4 + g * PPW);
+        }
+    }
+    if (threadIdx.x == 0) {
+        LrTileParams P;
+        lr_unit_params(u, HBD, P);
+        sP = P;
     }
     __syncthreads();
     const LrTileParams &P = sP;
     if (P.type == 0) {
+        if (interior) {
+#pragma unroll
+            for (int n = 0; n < NI; n++) {
+                const int i = threadIdx.x + n * 256;
+                const int yy = (int)((i * magic) >> 16), g = i - yy * NW;
+                if (yy >= th + 6) break;
+                if (yy >= 3 && yy < th + 3 && g * PPW >= 4 && g * PPW < tw + 4)
+                    *(unsigned *)(O + (ptrdiff_t)(ty0 - 3 + yy) * st + x0 - 4 + g * PPW) = wv[n];
+            }
+        } else
         for (int i = threadIdx.x; i < kTW * th; i += blockDim.x) {
             const int y = i / kTW, x = i - y * kTW;
             if (x >= tw) continue;
@@ -272,29 +328,17 @@ __global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __gri
         return;
     }
     // stage the virtual source: rows ty0-3 .. ty0+th+2, cols x0-3 .. x0+tw+2
-    const bool have_top = y0s > 0, have_bot = y1s < h;
-    constexpr int PPW = HBD ? 2 : 4;                                 // samples per 32-bit word
-    const bool interior = x0 >= 4 && x0 + tw + 4 <= w && !(tw & 3) && !(x0 & 3) && !(st & (PPW - 1)) &&
-                          !(((uintptr_t)C | (uintptr_t)D) & 3);
     if (interior) {
-        // aligned words over picture columns x0-4 .. x0+tw+3 (one more column on each side than needed)
-        const int NW = (tw + 8) / PPW;
-        const unsigned magic = recip16(NW);               // exact i / NW for i < 38 * 36
-        for (int i = threadIdx.x; i < (th + 6) * NW; i += blockDim.x) {
+#pragma unroll
+        for (int n = 0; n < NI; n++) {
+            const int i = threadIdx.x + n * 256;
             const int yy = (int)((i * magic) >> 16), g = i - yy * NW;
-            int Y = ty0 - 3 + yy;
-            const pixel *base = C;
-            if (Y < y0s) {
-                if (have_top) { base = D; Y = imax(Y, y0s - 2); } else Y = y0s;
-            } else if (Y >= y1s) {
-                if (have_bot) { base = D; Y = imin(imin(Y, y1s + 1), h - 1); } else Y = y1s - 1;
-            }
-            const unsigned wv = *(const unsigned *)(base + (ptrdiff_t)Y * st + x0 - 4 + g * PPW);
+            if (yy >= th + 6) break;
             const int c0 = g * PPW - 1;                              // tile column of the word's first sample
 #pragma unroll
             for (int k = 0; k < PPW; k++) {
                 const int c = c0 + k;
-                if (c >= 0 && c < tw + 6) sm.src[yy][c] = (uint16_t)(HBD ? (wv >> (16 * k)) & 0xffff : (wv >> (8 * k)) & 0xff);
+                if (c >= 0 && c < tw + 6) sm.src[yy][c] = (uint16_t)(HBD ? (wv[n] >> (16 * k)) & 0xffff : (wv[n] >> (8 * k)) & 0xff);
             }
         }
     } else
@@ -312,8 +356,7 @@ __global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __gri
         sm.src[yy][xx] = base[(ptrdiff_t)Y * st + X];
     }
     __syncthreads();
-    lr_tile_compute<HBD>(sm, P, tw, th, bdmax,
-                         [&](int x, int y, int v) { O[(ptrdiff_t)(ty0 + y) * st + x0 + x] = (pixel)v; });
+    lr_tile_compute<HBD>(sm, P, tw, th, bdmax, LrStore<pixel>{ O + (ptrdiff_t)ty0 * st + x0, st });
 }
 
 // Level 1: window = host-assembled (w + 6) x (h + 6) virtual source; out = dense w x h
@@ -330,8 +373,7 @@ __global__ void __launch_bounds__(256) lr_window_kernel(const typename Bd<HBD>::
         sm.src[yy][xx] = win[(size_t)(y0 + yy) * (w + 6) + x0 + xx];
     }
     __syncthreads();
-    lr_tile_compute<HBD>(sm, P, tw, th, bdmax,
-                         [&](int x, int y, int v) { out[(size_t)(y0 + y) * w + x0 + x] = (typename Bd<HBD>::pixel)v; });
+    lr_tile_compute<HBD>(sm, P, tw, th, bdmax, LrStore<typename Bd<HBD>::pixel>{ out + (size_t)y0 * w + x0, w });
 }
 
 // tile rows [r0, r1) of the sweep, counted in half stripes: tile row r is rows 32 r - 8 .. 32 r + 23 of the luma plane
