@@ -1,10 +1,12 @@
 // CDEF (dav1d Dav1dCdefDSPContext; reference src/cdef_tmpl.c:37-305, driver src/cdef_apply_tmpl.c).
 //
-// Frame-wide and out of place: one warp owns one 8x8 luma block and its chroma blocks. The warp
-// finds the block's direction/variance from the (pre-CDEF) luma samples, derives the strengths
-// exactly like dav1d_cdef_brow, then every lane filters its pixels reading taps straight from the
-// source picture; taps outside the block's available rectangle (picture edges) are skipped, which is
-// what the reference's INT16_MIN padding achieves. Unfiltered blocks are copied through.
+// Frame-wide and out of place: one CTA owns a 64x32 luma tile and its chroma tiles, staged once in shared
+// memory as vertical pixel pairs with a sentinel for samples outside the picture (see the frame kernel).
+// Eight lanes per 8x8 block find its direction / variance from the (pre-CDEF) luma samples and derive the
+// strengths exactly like dav1d_cdef_brow; the filter then reads every tap from the tile. Unfiltered blocks
+// are copied through. The Level-1 direction search runs the same cdef_dir8; the Level-1 block filter
+// (cdef_fb_kernel) is still a scalar restatement that skips the taps outside the block's available
+// rectangle, which is what the reference's INT16_MIN padding achieves.
 #include "host_util.h"
 
 namespace b200 {

@@ -244,6 +244,41 @@ B200_DEV int fg_pixel_grain(const B200FilmGrainData &d, const int16_t *lut, cons
     return g;
 }
 
+// Writes out[k] = sample s[k] of plane pl (0: luma) with grain value g[k] applied, k < n <= N (reference :181-226,
+// :292-352). The scaling index is s[k] for luma; for chroma it is the co-located luma sample luma(k, 0), averaged with its
+// right neighbour luma(k, 1) when subsampled horizontally, and unless chroma scaling comes from luma combined with s[k].
+// luma(k, j) is the caller's load, so the caller decides how a missing right neighbour (odd widths) is replicated.
+template <int N, class pixel, class Luma>
+B200_DEV void fg_apply_samples(const B200FilmGrainData &d, const uint8_t *scaling, int pl, int is_id, int sx, int b8, int bdmax,
+                               int n, const int (&s)[N], const int (&g)[N], Luma luma, pixel *out)
+{
+    int mn, mx;
+    if (d.clip_to_restricted_range) { mn = 16 << b8; mx = (pl && !is_id ? 240 : 235) << b8; }
+    else { mn = 0; mx = bdmax; }
+    int val[N];
+#pragma unroll
+    for (int k = 0; k < N; k++) val[k] = s[k];
+    if (pl) {
+#pragma unroll
+        for (int k = 0; k < N; k++) {
+            if (k >= n) break;
+            int avg = luma(k, 0);
+            if (sx) avg = (avg + luma(k, 1) + 1) >> 1;
+            val[k] = avg;
+            if (!d.chroma_scaling_from_luma) {
+                const int combined = avg * d.uv_luma_mult[pl - 1] + s[k] * d.uv_mult[pl - 1];
+                val[k] = iclip((combined >> 6) + d.uv_offset[pl - 1] * (1 << b8), 0, bdmax);
+            }
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < N; k++) {
+        if (k >= n) break;
+        const int noise = fg_round2((int)scaling[val[k]] * g[k], d.scaling_shift);
+        out[k] = (pixel)iclip(s[k] + noise, mn, mx);
+    }
+}
+
 // grid: (ceil(w / 128), ceil(h / 8), 3 planes); block (32, 8); a thread owns 4 consecutive samples of one row
 // (always inside one 32-wide grain block: 4 divides the block width of every layout)
 template <bool HBD>
@@ -288,36 +323,13 @@ __global__ void __launch_bounds__(256) fg_apply_kernel(const __grid_constant__ B
 #pragma unroll
         for (int k = 0; k < 4; k++) g[k] = gp[k];
     }
-    int mn, mx;
-    if (d.clip_to_restricted_range) { mn = 16 << b8; mx = (pl && !f.is_id ? 240 : 235) << b8; }
-    else { mn = 0; mx = bdmax; }
     const uint8_t *scaling = S->scaling[0];
-    int val[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) val[k] = s[k];
-    if (pl) {
+    if (pl && !d.chroma_scaling_from_luma) scaling = S->scaling[pl];
+    fg_apply_samples(d, scaling, pl, f.is_id, sx, b8, bdmax, nx, s, g, [&](int k, int j) {
         const pixel *luma = (const pixel *)f.in + f.plane_off[0] + (ptrdiff_t)(yp << sy) * f.stride[0];
-        const bool mix = !d.chroma_scaling_from_luma;
-        if (mix) scaling = S->scaling[pl];
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            if (k >= nx) break;
-            const int lx = (x0 + k) << sx;
-            int avg = luma[lx];
-            if (sx) avg = (avg + (int)luma[imin(lx + 1, f.w - 1)] + 1) >> 1;   // odd widths: replicate the last column (:196-203)
-            val[k] = avg;
-            if (mix) {
-                const int combined = avg * d.uv_luma_mult[pl - 1] + s[k] * d.uv_mult[pl - 1];
-                val[k] = iclip((combined >> 6) + d.uv_offset[pl - 1] * (1 << b8), 0, bdmax);
-            }
-        }
-    }
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        if (k >= nx) break;
-        const int noise = fg_round2((int)scaling[val[k]] * g[k], d.scaling_shift);
-        out[k] = (pixel)iclip(s[k] + noise, mn, mx);
-    }
+        const int lx = (x0 + k) << sx;
+        return j ? (int)luma[imin(lx + 1, f.w - 1)] : (int)luma[lx];   // odd widths: replicate the last column (:196-203)
+    }, out);
 }
 
 // ---- Level-1 kernels ----
@@ -343,24 +355,13 @@ __global__ void fg_strip_l1_kernel(typename Bd<HBD>::pixel *dst, const typename 
         for (int k = 0; k < nbx; k++) off[threadIdx.x][k] = (uint8_t)fg_rnd(8, &s);
     }
     __syncthreads();
-    int mn, mx;
-    if (d.clip_to_restricted_range) { mn = 16 << b8; mx = (uv >= 0 && !is_id ? 240 : 235) << b8; } else { mn = 0; mx = bdmax; }
     for (int i = threadIdx.x; i < pw * bh; i += blockDim.x) {
         const int y = i / pw, x = i - y * pw;
         const int g = fg_pixel_grain(d, lut, off[0], off[1], b8, row_num, x, y, pw, bh, sx, sy);
-        const int s = src[i];
-        int val = s;
-        if (uv >= 0) {
-            const int lx = x << sx;
-            int avg = luma[(y << sy) * lw + lx];
-            if (sx) avg = (avg + (int)luma[(y << sy) * lw + lx + 1] + 1) >> 1;
-            val = avg;
-            if (!d.chroma_scaling_from_luma) {
-                const int combined = avg * d.uv_luma_mult[uv] + s * d.uv_mult[uv];
-                val = iclip((combined >> 6) + d.uv_offset[uv] * (1 << b8), 0, bdmax);
-            }
-        }
-        dst[i] = (typename Bd<HBD>::pixel)iclip(s + fg_round2((int)scaling[val] * g, d.scaling_shift), mn, mx);
+        // dav1d pads an odd-width luma row, so the right neighbour of the last column is always there
+        const int lx = (y << sy) * lw + (x << sx);
+        const int s[1] = { src[i] }, gr[1] = { g };
+        fg_apply_samples(d, scaling, uv + 1, is_id, sx, b8, bdmax, 1, s, gr, [&](int, int j) { return (int)luma[lx + j]; }, dst + i);
     }
 }
 

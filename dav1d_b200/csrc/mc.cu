@@ -9,7 +9,8 @@
 //   mc_comp_kernel   avg / w_avg / mask / w_mask{444,422,420} (:628-681, 724-781)
 //   mc_blend_kernel  blend / blend_v / blend_h (:683-722)
 //   mc_warp_kernel   warp_affine_8x8 / 8x8t (:799-866), one warp per 8x8 block
-//   emu_edge / resize kernels (:868-944) for the Level-1 table
+//   resize_frame_kernel  super-resolution upscaling of whole planes (:918-944)
+//   emu_edge_kernel  (:868-916) for the Level-1 table only: the prediction kernels fold emu_edge into their loads
 // Integer only; bit-exact with the reference C path.
 #include "host_util.h"
 #define B200_TBL __constant__
@@ -630,24 +631,8 @@ __global__ void emu_edge_kernel(int bw, int bh, int iw, int ih, int x0, int y0,
     }
 }
 
-template <bool HBD>
-__global__ void resize_kernel(typename Bd<HBD>::pixel *dst, const typename Bd<HBD>::pixel *src, int dst_w,
-                              int h, int src_w, int dx, int mx0, int bdmax)
-{
-    // the x position recurrence (mx += dx; src_x += mx >> 14; mx &= 0x3fff) has the closed form below
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < dst_w * h; i += gridDim.x * blockDim.x) {
-        const int y = i / dst_w, x = i - y * dst_w;
-        const long long pos = (long long)mx0 + (long long)x * dx;
-        const int src_x = -1 + (int)(pos >> 14), mx = (int)(pos & 0x3fff);
-        const int8_t *F = b200_resize_filter[mx >> 8];
-        int s = 0;
-#pragma unroll
-        for (int k = 0; k < 8; k++) s += F[k] * (int)src[y * src_w + iclip(src_x - 3 + k, 0, src_w - 1)];
-        dst[i] = (typename Bd<HBD>::pixel)iclip((-s + 64) >> 7, 0, bdmax);
-    }
-}
-
-// whole planes, strided (the frame job's super-resolution stage): one thread per output sample, grid.y = plane
+// whole planes, strided (the frame job's super-resolution stage): one thread per output sample, grid.y = plane.
+// The x position recurrence (mx += dx; src_x += mx >> 14; mx &= 0x3fff) has the closed form below.
 template <bool HBD>
 __global__ void __launch_bounds__(256) resize_frame_kernel(const __grid_constant__ B200ResizeFrame fr, int bdmax)
 {
@@ -911,14 +896,14 @@ int b200_mc_resize(void *dst, ptrdiff_t dst_stride, const void *src, ptrdiff_t s
     if (dst_w < 1 || h < 1 || src_w < 1 || (size_t)dst_w * h > (1u << 26)) { b200_set_error("b200_mc_resize: bad geometry"); return -2; }
     Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
-    void *s, *d;
-    if (!(s = L.upload_rect(REF, src, src_stride, src_w, h, px)) || !(d = L.dev(DST, (size_t)dst_w * h * px))) return -1;
-    const int n = dst_w * h, grid = imin((n + 255) / 256, 1184);
-    if (int r = launch_hbd(bdmax, Launch::plain, dim3(grid), dim3(256), 0, 0, [&](auto hbd) {
-            typedef typename Bd<hbd>::pixel pixel;
-            return std::make_tuple(resize_kernel<hbd>, (pixel *)d, (const pixel *)s, dst_w, h, src_w, dx, mx, bdmax);
-        }))
-        return r;
+    B200ResizeFrame fr;
+    memset(&fr, 0, sizeof(fr));
+    if (!(fr.src = L.upload_rect(REF, src, src_stride, src_w, h, px)) || !(fr.dst = L.dev(DST, (size_t)dst_w * h * px))) return -1;
+    fr.n_planes = 1;
+    fr.src_stride[0] = fr.src_w[0] = src_w; fr.dst_stride[0] = fr.dst_w[0] = dst_w; fr.h[0] = h;
+    fr.dx[0] = dx; fr.mx0[0] = mx;
+    // the frame entry point launches with PDL; on stream 0 after the staging copies that orders like a plain launch (as mc_l1)
+    if (int r = b200_resize_frame(bdmax, &fr, 0)) return r;
     return L.download_rect(DST, dst, dst_stride, dst_w, h, px);
 }
 
