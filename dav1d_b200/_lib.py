@@ -297,6 +297,9 @@ _SIGS = {
     "b200_event_destroy": (None, [C.c_void_p]),
     "b200_event_record": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_stream_wait_event": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "b200_event_sync": (C.c_int, [C.c_void_p]),
+    # ---- export of a decoded picture
+    "b200_export_picture": (C.c_int, [C.c_void_p, C.c_void_p]),
     # ---- ipred
     "b200_ipred_batch": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "b200_ipred": (C.c_int, [C.c_int, C.c_void_p, C.c_ssize_t, C.c_void_p] + [C.c_int] * 6),
@@ -363,5 +366,14 @@ class Av1Restoration(C.Structure):
     _fields_ = [("lr", C.c_uint8 * 108)]
 
 
+class ExportJob(C.Structure):
+    """B200ExportJob: export of a decoded picture (format 0 planes, 1 RGB) into caller memory"""
+    _fields_ = [("src", C.c_void_p), ("plane_off", C.c_uint32 * 3), ("stride", C.c_int32 * 3), ("w", C.c_int32), ("h", C.c_int32),
+                ("ss_hor", C.c_int32), ("ss_ver", C.c_int32), ("mono", C.c_int32), ("bitdepth_max", C.c_int32), ("format", C.c_int32),
+                ("full_range", C.c_int32), ("identity", C.c_int32), ("cy", C.c_int32), ("rv", C.c_int32), ("gu", C.c_int32),
+                ("gv", C.c_int32), ("bu", C.c_int32), ("dst", C.c_void_p * 3), ("dst_pitch", C.c_int32 * 3), ("pad2", C.c_int32)]
+
+
 ABI_STRUCTS = [McFrame, McBlock, CompBlock, BlendBlock, WarpBlock, ItxBlock, LfFrame, CdefFrame, LrFrame, FrameJob,
-               Av1Filter, Av1Restoration, FgFrame, FilmGrainData, IntraTx, IntraFrame, McScaledBlock, CoefBlock, IntraSb, CompFusedBlock, FrameBand, ResizeFrame]
+               Av1Filter, Av1Restoration, FgFrame, FilmGrainData, IntraTx, IntraFrame, McScaledBlock, CoefBlock, IntraSb, CompFusedBlock, FrameBand, ResizeFrame,
+               ExportJob]

@@ -173,9 +173,13 @@ def main(argv=None):
     ap.add_argument("--one-job-at-a-time", action="store_true", help="serialise the device jobs (for back ends that are not re-entrant)")
     ap.add_argument("--frametimes", metavar="FILE", help="write one line per output frame: nanoseconds since the previous one (like `dav1d --frametimes`)")
     ap.add_argument("-q", "--quiet", action="store_true", help="no progress / speed line")
+    ap.add_argument("--output-path", choices=["host", "device"], default="host",
+                    help="device: pictures stay in device memory and are exported as planes (stream.DeviceDecoder); md5 / null only")
     args = ap.parse_args(argv)
     if bool(args.input) == bool(args.synth):
         ap.error("give exactly one of -i / --synth")
+    if args.output_path == "device" and (args.output or args.muxer == "y4m" or args.frametimes):
+        ap.error("--output-path device supports --muxer md5 / null and --verify")
     tus = synth_stream(args.synth, args.seed) if args.synth else demux(open(args.input, "rb").read(), args.demuxer)
     if args.write_stream:
         with open(args.write_stream, "wb") as fh:
@@ -183,6 +187,8 @@ def main(argv=None):
         if not (args.output or args.muxer or args.verify):
             print("wrote %d temporal units, %d bytes" % (len(tus), sum(map(len, tus))))
             return 0
+    if args.output_path == "device":
+        return _main_device(args, tus)
     kw = dict(n_threads=max(2, args.threads), max_frame_delay=max(2, args.framedelay), apply_grain=args.filmgrain, max_pics=len(tus) + 8)
     t0 = time.perf_counter()
     dec = stream.HookedDecoder(backend=None if args.backend == "b200" else args.backend, serialize=args.one_job_at_a_time)
@@ -217,6 +223,37 @@ def main(argv=None):
         # tools/dav1d.c print_stats(): "Decoded n/num frames (100.0%) - x fps" (the decoder's own clock: first byte in to last frame out)
         d_fps = 1e9 * n / times[-1] if times and times[-1] else n / dt
         print("Decoded %d/%d frames (100.0%%) - %.2f fps (%.1f Mpixels/s; %.3f s incl. start-up)" % (n, n, d_fps, px * d_fps / max(n, 1) / 1e6, dt), file=sys.stderr)
+    return 0
+
+
+def _main_device(args, tus):
+    """--output-path device: the md5 / --verify digest is taken over the planes the export kernel wrote. A --backend other
+    than the CUDA library is a host build of the C ABI (the emulator), whose device memory is host memory: numpy planes."""
+    alloc = None if args.backend == "b200" else (lambda shape, dtype: np.empty(shape, dtype))
+    dec = stream.DeviceDecoder(backend=None if args.backend == "b200" else args.backend, n_threads=max(2, args.threads),
+                               max_frame_delay=max(2, args.framedelay), apply_grain=args.filmgrain, serialize=args.one_job_at_a_time)
+    t0 = time.perf_counter()
+    m, n, px = hashlib.md5(), 0, 0
+    try:
+        for planes in dec.pictures(tus, alloc=alloc):
+            for p in planes:
+                m.update(np.ascontiguousarray(p.cpu().numpy() if hasattr(p, "cpu") else p).tobytes())
+            n += 1
+            px += planes[0].shape[0] * planes[0].shape[1]
+    except RuntimeError as e:
+        print(e, file=sys.stderr)
+        return 1
+    finally:
+        dec.release()
+    dt = time.perf_counter() - t0
+    digest = m.hexdigest()
+    if (args.muxer or "md5") == "md5":
+        print(digest)
+    if args.verify and digest != args.verify.lower():
+        print("md5 mismatch: %s != %s" % (digest, args.verify), file=sys.stderr)
+        return 2
+    if not args.quiet:
+        print("Decoded %d/%d frames (100.0%%) - %.2f fps (%.1f Mpixels/s; %.3f s incl. start-up, device output)" % (n, n, n / dt, px / dt / 1e6, dt), file=sys.stderr)
     return 0
 
 

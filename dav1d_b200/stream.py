@@ -1,17 +1,40 @@
 """Host glue for decoding AV1 elementary streams with the B200 back end behind a real dav1d front end.
 
-`oracle/_ref/libdav1d_b200.so` is the unmodified dav1d library whose `f->bd_fn` hooks are the record emitters of
-integration/dav1d/ (built by oracle/hooked.mk where the reference sources exist; elsewhere the prebuilt oracle/_ref/ is
-used). This module binds its stream driver (dav1d's public API: dav1d_open / dav1d_send_data / dav1d_get_picture)
+`oracle/_ref/hooked-<digest>/libdav1d_b200.so` is the unmodified dav1d library whose `f->bd_fn` hooks are the record
+emitters of integration/dav1d/ (built by oracle/hooked.mk where the reference sources exist; elsewhere the prebuilt
+oracle/_ref/ is used). This module binds its stream driver (dav1d's public API: dav1d_open / dav1d_send_data / dav1d_get_picture)
 and points the hooks at dav1d_b200/libb200av1.so. No CPU fallback: without the CUDA library the decode fails."""
 import ctypes as C
 import os
 
 import numpy as np
 
+from ._lib import ExportJob  # noqa: F401  (B200ExportJob, filled by DeviceDecoder)
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HOOKED_SO = os.path.join(ROOT, "oracle", "_ref", "libdav1d_b200.so")
-LEVEL1_SO = os.path.join(ROOT, "oracle", "_ref", "libdav1d_b200_l1.so")
+
+
+def _hooked_dir():
+    """oracle/_ref/hooked-<digest>: the hooked libraries are compiled from this tree's own sources (integration/dav1d/, the C
+    ABI header, the recipe), so the directory they are built into is named by a digest of those sources. A library built
+    from other sources (an older checkout, a build directory restored from elsewhere, objects make judged up to date by
+    their times) is then never loaded in their place: its symbols and struct layouts would not be the ones this module
+    binds."""
+    import hashlib
+    h = hashlib.sha256()
+    hk = os.path.join(ROOT, "integration", "dav1d")
+    files = [os.path.join(hk, f) for f in sorted(os.listdir(hk))] + [os.path.join(ROOT, "include", "b200av1.h"),
+                                                                    os.path.join(ROOT, "oracle", "hooked.mk")]
+    for f in files:
+        if os.path.isfile(f):
+            with open(f, "rb") as fh:
+                h.update(os.path.relpath(f, ROOT).encode()); h.update(fh.read())
+    return os.path.join(ROOT, "oracle", "_ref", "hooked-" + h.hexdigest()[:16])
+
+
+HOOKED_DIR = _hooked_dir()
+HOOKED_SO = os.path.join(HOOKED_DIR, "libdav1d_b200.so")
+LEVEL1_SO = os.path.join(HOOKED_DIR, "libdav1d_b200_l1.so")
 # hooked library -> the back end its hooks are bound to: the binding and everything the hooks hold (device pictures, frame
 # slots, page-locked pictures) is process-wide state of the library, shared by every HookedDecoder of the process
 _bound = {}
@@ -26,9 +49,10 @@ class HookStats(C.Structure):
 
 
 def build_hooked(verbose=False):
-    """(Re)build oracle/_ref/libdav1d_b200.so (+ the Level-1 variant) where the reference sources exist; otherwise a no-op."""
+    """(Re)build HOOKED_SO (+ the Level-1 variant) where the reference sources exist; otherwise a no-op."""
     import subprocess
-    r = subprocess.run(["make", "-j8", "-C", os.path.join(ROOT, "oracle"), "hooked"], capture_output=True, text=True)
+    oracle = os.path.join(ROOT, "oracle")
+    r = subprocess.run(["make", "-j8", "-C", oracle, "hooked", "OUT=" + os.path.relpath(HOOKED_DIR, oracle)], capture_output=True, text=True)
     if r.returncode:
         raise RuntimeError("oracle/hooked.mk build failed:\n" + r.stderr[-3000:])
     if verbose:
@@ -78,7 +102,7 @@ class HookedDecoder:
         if not os.path.exists(HOOKED_SO):
             build_hooked()
             if not os.path.exists(HOOKED_SO):
-                raise RuntimeError("oracle/_ref/libdav1d_b200.so missing (it is built where the reference sources exist)")
+                raise RuntimeError("%s missing (it is built where the reference sources exist)" % HOOKED_SO)
         if backend is None:
             from . import _lib
             _lib.get_lib()                       # builds / loads the CUDA library or raises
@@ -118,6 +142,167 @@ class HookedDecoder:
         self.dll.b200hook_release()
 
 
+EXPORT_FORMATS = {"planes": 0, "rgb": 1}
+# (Kr, Kb) of the YCbCr matrices the RGB export knows; the sequence header's matrix_coefficients (enum Dav1dMatrixCoefficients)
+# -> one of them ("identity": R = V, G = Y, B = U)
+MATRICES = {"bt601": (0.299, 0.114), "bt709": (0.2126, 0.0722), "bt2020": (0.2627, 0.0593)}
+MTRX_TO_MATRIX = {0: "identity", 1: "bt709", 5: "bt601", 6: "bt601", 9: "bt2020", 10: "bt2020"}
+
+
+def rgb_coefficients(matrix, full_range):
+    """(cy, rv, gu, gv, bu) of the RGB export, 1.0 = 1 << 14: R = cy*Y' + rv*Cr', G = cy*Y' - gu*Cb' - gv*Cr', B = cy*Y' + bu*Cb'.
+    Limited range stretches luma by 255/219 and chroma by 255/224 (whatever the bit depth)."""
+    kr, kb = MATRICES[matrix]
+    kg = 1.0 - kr - kb
+    ys, cs = (1.0, 1.0) if full_range else (255.0 / 219.0, 255.0 / 224.0)
+    f = [ys, 2 * (1 - kr) * cs, 2 * kb * (1 - kb) / kg * cs, 2 * kr * (1 - kr) / kg * cs, 2 * (1 - kb) * cs]
+    return tuple(int(round(v * (1 << 14))) for v in f)
+
+
+def rgb_reference(planes, bpc, layout, matrix, full_range):
+    """numpy statement of the RGB export (include/b200av1.h B200ExportJob) for one picture's planes: [3, h, w] int64"""
+    y = planes[0].astype(np.int64)
+    h, w = y.shape
+    if layout == 0:
+        u = v = None
+    else:
+        ssh, ssv = int(layout != 3), int(layout == 1)
+        yi, xi = np.arange(h)[:, None] >> ssv, np.arange(w)[None, :] >> ssh
+        u, v = planes[1].astype(np.int64)[yi, xi], planes[2].astype(np.int64)[yi, xi]
+    if matrix == "identity":
+        return np.stack([v, y, u])
+    s, bdmax = bpc - 8, (1 << bpc) - 1
+    cy, rv, gu, gv, bu = rgb_coefficients(matrix, full_range)
+    yy = cy * (y - (0 if full_range else 16 << s)) + 8192
+    cb, cr = (0, 0) if u is None else (u - (128 << s), v - (128 << s))
+    return np.clip(np.stack([(yy + rv * cr) >> 14, (yy - gu * cb - gv * cr) >> 14, (yy + bu * cb) >> 14]), 0, bdmax)
+
+
+class DeviceDecoder:
+    """dav1d front end + B200 back end whose output pictures never leave the device: each one is exported by one kernel from
+    its HBM copy into memory the caller allocates, and released at once.
+
+        dec = DeviceDecoder()
+        for y, u, v in dec.pictures(tus):                      # torch.uint8 (8 bit) / torch.int16 (10, 12 bit) CUDA tensors
+            ...
+        for rgb in dec.pictures(tus, format="rgb"):             # [3, h, w], same dtype rule, stream bit depth
+
+    `backend` = path of the C-ABI library the hooks bind (default: the CUDA library); `serialize` = one device job at a time
+    (for back ends that are not re-entrant, like the host emulator)."""
+
+    def __init__(self, backend=None, n_threads=4, max_frame_delay=2, apply_grain=1, serialize=False):
+        self._hooked = HookedDecoder(backend=backend, serialize=serialize)
+        self.dll = self._hooked.dll
+        self.n_threads, self.max_frame_delay, self.apply_grain = n_threads, max_frame_delay, apply_grain
+        d = self.dll
+        d.refdrv_stream_open.restype = C.c_void_p
+        d.refdrv_stream_open.argtypes = [C.c_int, C.c_int, C.c_int]
+        for fn in ("refdrv_stream_context", "refdrv_stream_picture"):
+            getattr(d, fn).restype = C.c_void_p
+            getattr(d, fn).argtypes = [C.c_void_p]
+        d.refdrv_stream_send.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64]
+        d.refdrv_stream_get.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        d.refdrv_stream_release.argtypes = [C.c_void_p]
+        d.refdrv_stream_close.argtypes = [C.c_void_p]
+        d.b200hook_set_device_only.argtypes = [C.c_void_p, C.c_int]
+        d.b200hook_export_picture.argtypes = [C.c_void_p, C.POINTER(ExportJob), C.c_void_p]
+
+    def stats(self, reset=False):
+        return self._hooked.stats(reset)
+
+    def release(self):
+        self._hooked.release()
+
+    def pictures(self, tus, format="planes", matrix="auto", full_range=None, alloc=None, stream=None):
+        """Decodes the temporal units `tus` and yields one item per output picture: a tuple of planes (Y, U, V; Y alone for
+        4:0:0) for format="planes", a [3, h, w] array of R, G, B for format="rgb".
+        matrix: "auto" (the sequence header's matrix_coefficients; BT.709 when unspecified), "bt601", "bt709", "bt2020" or
+        "identity" (4:4:4 only); full_range: None = the sequence header's color_range.
+        alloc(shape, dtype) returns the destination (dtype "uint8" at 8 bit, "int16" above, holding the sample values): by
+        default torch.empty(..., device="cuda") on the current device. The export runs on `stream` (a torch.cuda.Stream or a
+        cudaStream_t handle), by default torch.cuda.current_stream() with the default alloc and the legacy default stream
+        otherwise."""
+        if format not in EXPORT_FORMATS:
+            raise ValueError("format must be 'planes' or 'rgb'")
+        if matrix != "auto" and matrix != "identity" and matrix not in MATRICES:
+            raise ValueError("unknown matrix %r" % (matrix,))
+        if alloc is None:
+            import torch
+            alloc = lambda shape, dtype: torch.empty(shape, dtype=getattr(torch, dtype), device="cuda")
+            if stream is None:
+                stream = torch.cuda.current_stream()
+        stream = getattr(stream, "cuda_stream", stream) or 0
+        self._hooked._bind()
+        d = self.dll
+        h = d.refdrv_stream_open(self.n_threads, self.max_frame_delay, self.apply_grain)
+        if not h:
+            raise RuntimeError("dav1d_open failed")
+        ctx = d.refdrv_stream_context(h)
+        try:
+            if d.b200hook_set_device_only(ctx, 1):
+                raise RuntimeError("too many decoders with device output open")
+            info = np.zeros(6, np.int32)
+            for tu in list(tus) + [None]:
+                pending = 1 if tu is not None else 0
+                if tu is not None:
+                    pending = d.refdrv_stream_send(h, tu, len(tu))
+                while True:
+                    while True:
+                        r = d.refdrv_stream_get(h, info.ctypes.data, 0 if tu is not None else 1)
+                        if r == _EAGAIN:
+                            break
+                        if r < 0:
+                            raise RuntimeError("decoding failed: dav1d error %d" % r)
+                        try:
+                            out = self._export(h, info, format, matrix, full_range, alloc, stream)
+                        finally:
+                            d.refdrv_stream_release(h)
+                        yield out
+                    if pending < 0:
+                        raise RuntimeError("decoding failed: dav1d error %d" % pending)
+                    if pending == 0:
+                        break
+                    pending = d.refdrv_stream_send(h, None, 0)
+        finally:
+            d.refdrv_stream_close(h)                # frames still in flight are flushed as device-output frames
+            d.b200hook_set_device_only(ctx, 0)
+
+    def _export(self, h, info, format, matrix, full_range, alloc, stream):
+        w, hh, bpc, layout, mtrx, color_range = (int(v) for v in info)
+        dtype = "uint8" if bpc == 8 else "int16"
+        job = ExportJob()
+        job.format = EXPORT_FORMATS[format]
+        if format == "planes":
+            outs = [alloc((ph, pw), dtype) for pw, ph in plane_dims(w, hh, layout)]
+            for k, o in enumerate(outs):
+                job.dst[k], job.dst_pitch[k] = _data_ptr(o), plane_dims(w, hh, layout)[k][0]
+            result = tuple(outs)
+        else:
+            name = MTRX_TO_MATRIX.get(mtrx, "bt709") if matrix == "auto" else matrix
+            if name == "identity" and layout != 3:
+                if matrix == "identity":
+                    raise ValueError("the identity matrix needs a 4:4:4 picture")
+                name = "bt709"
+            job.identity = name == "identity"
+            job.full_range = int(bool(color_range if full_range is None else full_range))
+            if not job.identity:
+                job.cy, job.rv, job.gu, job.gv, job.bu = rgb_coefficients(name, job.full_range)
+            result = alloc((3, hh, w), dtype)
+            base = _data_ptr(result)
+            for k in range(3):
+                job.dst[k], job.dst_pitch[k] = base + k * hh * w * (1 if bpc == 8 else 2), w
+        if self.dll.b200hook_export_picture(self.dll.refdrv_stream_picture(h), C.byref(job), C.c_void_p(stream)) != 0:
+            raise RuntimeError("exporting a picture failed (see stderr)")
+        return result
+
+
+_EAGAIN = -11
+
+
+def _data_ptr(a):
+    return a.data_ptr() if hasattr(a, "data_ptr") else a.ctypes.data
+
+
 class Level1Decoder:
     """dav1d with its own reconstruction code, but every DSP table slot (`Dav1dDSPContext`: itx, mc, ipred, loopfilter,
     cdef, looprestoration, filmgrain) overridden by libb200av1's Level-1 functions — the architecture-hook form of the
@@ -128,7 +313,7 @@ class Level1Decoder:
         if not os.path.exists(LEVEL1_SO):
             build_hooked()
             if not os.path.exists(LEVEL1_SO):
-                raise RuntimeError("oracle/_ref/libdav1d_b200_l1.so missing (it is built where the reference sources exist)")
+                raise RuntimeError("%s missing (it is built where the reference sources exist)" % LEVEL1_SO)
         if backend is None:
             from . import _lib
             backend = _lib.get_lib().path

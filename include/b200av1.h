@@ -641,7 +641,7 @@ B200_API int b200_frame_run_batch(const B200FrameJob *const *jobs, int n_jobs, v
 /* sizeof() of the ABI structs as compiled into the library (binding self-check): 0 McFrame, 1 McBlock, 2 CompBlock,
  * 3 BlendBlock, 4 WarpBlock, 5 ItxBlock, 6 LfFrame, 7 CdefFrame, 8 LrFrame, 9 FrameJob, 10 Av1Filter, 11 Av1Restoration,
  * 12 FgFrame, 13 FilmGrainData, 14 IntraTx, 15 IntraFrame, 16 McScaledBlock, 17 CoefBlock, 18 IntraSb, 19 CompFusedBlock,
- * 20 FrameBand, 21 ResizeFrame */
+ * 20 FrameBand, 21 ResizeFrame, 22 ExportJob */
 B200_API int b200_struct_size(int which);
 
 /* ==== band-sliced frame job + cross-GPU reference exchange (SURVEY.md §8e) ===================== */
@@ -750,6 +750,36 @@ B200_API int b200_frame_submit_host(const B200FrameJob *job, const B200Xfer *upl
 B200_API int b200_frame_submit_host_batch(const B200FrameJob *const *jobs, int n_jobs, const B200Xfer *uploads,
                                           int n_uploads, const B200Xfer *downloads, int n_downloads, void *stream);
 B200_API int b200_frame_wait(void *stream);
+/* blocks the host until the work recorded by `event` (b200_event_record) has completed */
+B200_API int b200_event_sync(void *event);
+
+/* ==== export of a decoded picture into caller-owned device memory ============================ */
+/* Reads the device copy of a decoded picture (planes at src + plane_off[p], strides in samples) and writes, cropped to
+ * the visible w x h and tightly packed at the destination pitches:
+ *   B200_EXPORT_PLANES: dst[0] = Y [h, w], dst[1] / dst[2] = U / V [(h + ss_ver) >> ss_ver, (w + ss_hor) >> ss_hor];
+ *                       mono: Y only
+ *   B200_EXPORT_RGB:    dst[0] / dst[1] / dst[2] = R / G / B [h, w] at the stream's bit depth. Chroma is taken at
+ *                       (x >> ss_hor, y >> ss_ver); with s = bitdepth - 8, Y' = Y - (full_range ? 0 : 16 << s),
+ *                       C' = C - (128 << s) (mono: Cb' = Cr' = 0), and
+ *                         R = clip((cy * Y' + rv * Cr' + 8192) >> 14)
+ *                         G = clip((cy * Y' - gu * Cb' - gv * Cr' + 8192) >> 14)
+ *                         B = clip((cy * Y' + bu * Cb' + 8192) >> 14)
+ *                       in int32 with a flooring shift, clip to [0, bitdepth_max]. identity (4:4:4 only): R = V, G = Y, B = U.
+ * Samples are uint8 at 8 bit and 16-bit words holding the sample values above. One launch on `stream`. */
+enum { B200_EXPORT_PLANES = 0, B200_EXPORT_RGB = 1 };
+typedef struct B200ExportJob {
+    const void *src;               /* device picture */
+    uint32_t plane_off[3];         /* samples */
+    int32_t stride[3];             /* samples */
+    int32_t w, h, ss_hor, ss_ver, mono, bitdepth_max;
+    int32_t format;                /* B200_EXPORT_* */
+    int32_t full_range, identity;  /* RGB only */
+    int32_t cy, rv, gu, gv, bu;    /* RGB only: the matrix, 1.0 = 1 << 14 */
+    void *dst[3];                 /* device */
+    int32_t dst_pitch[3];          /* samples */
+    int32_t pad2;
+} B200ExportJob;
+B200_API int b200_export_picture(const B200ExportJob *job, void *stream);
 
 #ifdef __cplusplus
 }

@@ -70,10 +70,12 @@ API int b200hook_set_backend(const char *path)
     SYM(event_create, "b200_event_create"); SYM(event_destroy, "b200_event_destroy");
     SYM(event_record, "b200_event_record"); SYM(stream_wait_event, "b200_stream_wait_event");
     SYM(struct_size, "b200_struct_size");
+    SYM(event_sync, "b200_event_sync"); SYM(export_picture, "b200_export_picture");
 #undef SYM
     /* binding self-check: the structs this file was compiled with are the ones the library was compiled with */
     if (be.struct_size(9) != (int)sizeof(B200FrameJob) || be.struct_size(14) != (int)sizeof(B200IntraTx) ||
-        be.struct_size(10) != (int)sizeof(B200Av1Filter) || be.struct_size(11) != (int)sizeof(B200Av1Restoration)) {
+        be.struct_size(10) != (int)sizeof(B200Av1Filter) || be.struct_size(11) != (int)sizeof(B200Av1Restoration) ||
+        be.struct_size(22) != (int)sizeof(B200ExportJob)) {
         fprintf(stderr, "b200hook: ABI struct size mismatch with %s\n", path);
         dlclose(h);
         return -1;
@@ -282,7 +284,8 @@ HookRefPic *b200hook_refpic(const void *key, size_t bytes, int create)
             if (!r)                              /* only pictures of abandoned frames (never completed) are left: oldest one */
                 for (int i = 0; i < 64; i++)
                     if (!r || g_refs[i].last_use < r->last_use) r = &g_refs[i];
-            r->key = key; r->ready = 0; r->submitted = 0;
+            if (r->exported) be->event_sync(r->export_event);
+            r->key = key; r->ready = 0; r->submitted = 0; r->exported = 0;
         }
     }
     if (r && create && !r->event) r->event = be->event_create();      /* NULL = no events: consumers then wait for `ready` on the host */
@@ -299,10 +302,72 @@ HookRefPic *b200hook_refpic(const void *key, size_t bytes, int create)
 void b200hook_refpic_forget(const void *const key)
 {
     if (!key) return;
+    /* an export still reading the picture's device copy must complete before the entry (and its buffer) is free; the entry
+     * keeps its key until then, so nobody takes it over */
+    void *export_done = NULL;
     pthread_mutex_lock(&g_lock);
     for (int i = 0; i < 64; i++)
-        if (g_refs[i].key == key) { g_refs[i].key = NULL; g_refs[i].ready = 0; g_refs[i].submitted = 0; }
+        if (g_refs[i].key == key && g_refs[i].exported) export_done = g_refs[i].export_event;
     pthread_mutex_unlock(&g_lock);
+    if (export_done) g_be.event_sync(export_done);
+    pthread_mutex_lock(&g_lock);
+    for (int i = 0; i < 64; i++)
+        if (g_refs[i].key == key) { g_refs[i].key = NULL; g_refs[i].ready = 0; g_refs[i].submitted = 0; g_refs[i].exported = 0; }
+    pthread_mutex_unlock(&g_lock);
+}
+
+int b200hook_export_submit(HookRefPic *const r, const B200ExportJob *const job, void *const stream)
+{
+    const B200Backend *const be = b200hook_backend();
+    if (!be) return -1;
+    pthread_mutex_lock(&g_lock);
+    if (!r->export_event) r->export_event = be->event_create();
+    void *const done = r->export_event;
+    pthread_mutex_unlock(&g_lock);
+    b200hook_job_enter();
+    int rc = r->event ? be->stream_wait_event(stream, r->event) : 0;
+    if (!rc) rc = be->export_picture(job, stream);
+    if (!rc) rc = done ? be->event_record(done, stream) : be->frame_wait(stream);      /* no event: the export completes here */
+    b200hook_job_leave();
+    if (rc) { fprintf(stderr, "b200hook: export failed (%d): %s\n", rc, be->last_error()); return rc; }
+    pthread_mutex_lock(&g_lock);
+    r->exported = done != NULL;
+    pthread_mutex_unlock(&g_lock);
+    return 0;
+}
+
+/* decoder contexts opened for device output (b200hook_set_device_only); a context is registered between its dav1d_open and
+ * its dav1d_close */
+static const void *g_device_only[64];
+API int b200hook_set_device_only(const void *const ctx, const int on)
+{
+    int rc = on ? -1 : 0;
+    pthread_mutex_lock(&g_lock);
+    for (int i = 0; i < 64; i++)
+        if (g_device_only[i] == ctx) g_device_only[i] = NULL;
+    for (int i = 0; i < 64 && on && rc; i++)
+        if (!g_device_only[i]) { g_device_only[i] = ctx; rc = 0; }
+    pthread_mutex_unlock(&g_lock);
+    return rc;
+}
+int b200hook_device_only(const void *const ctx)
+{
+    int on = 0;
+    pthread_mutex_lock(&g_lock);
+    for (int i = 0; i < 64 && !on; i++) on = ctx && g_device_only[i] == ctx;
+    pthread_mutex_unlock(&g_lock);
+    return on;
+}
+
+int b200hook_export_picture_8bpc(const Dav1dPicture *p, const B200ExportJob *tmpl, void *stream);
+int b200hook_export_picture_16bpc(const Dav1dPicture *p, const B200ExportJob *tmpl, void *stream);
+/* Exports a picture dav1d output (the caller holds a reference to it) from its device copy into caller memory: `tmpl`
+ * carries the format, destinations and matrix, the source geometry is the picture's own. Error when the picture has no
+ * device copy (there is no host path). */
+API int b200hook_export_picture(const Dav1dPicture *const p, const B200ExportJob *const tmpl, void *const stream)
+{
+    if (!p || !tmpl || !p->data[0]) return -1;
+    return p->p.bpc > 8 ? b200hook_export_picture_16bpc(p, tmpl, stream) : b200hook_export_picture_8bpc(p, tmpl, stream);
 }
 void b200hook_refpic_set_ready(HookRefPic *r, int ready)
 {
@@ -579,8 +644,10 @@ API void b200hook_release(void)
         memset(h, 0, sizeof(*h));
     }
     for (int i = 0; i < 64; i++) {
+        if (g_refs[i].exported && g_be_ok) g_be.event_sync(g_refs[i].export_event);
         if (g_refs[i].dev && g_be_ok) g_be.dev_free(g_refs[i].dev);
         if (g_refs[i].event && g_be_ok) g_be.event_destroy(g_refs[i].event);
+        if (g_refs[i].export_event && g_be_ok) g_be.event_destroy(g_refs[i].export_event);
         memset(&g_refs[i], 0, sizeof(g_refs[i]));
     }
     pthread_mutex_unlock(&g_lock);

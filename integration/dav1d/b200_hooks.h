@@ -34,6 +34,8 @@ typedef struct B200Backend {
     int (*event_record)(void *, void *);
     int (*stream_wait_event)(void *, void *);
     int (*struct_size)(int);
+    int (*event_sync)(void *);
+    int (*export_picture)(const B200ExportJob *, void *);
 } B200Backend;
 const B200Backend *b200hook_backend(void);   /* NULL (after logging) when no back end is loaded: the decode fails */
 
@@ -129,8 +131,16 @@ static inline void *b200hook_tile_append(HookFrame *const hf, const int tile, co
 /* submitted: the picture's job is enqueued on its frame context's stream and `event` marks the end of its kernels — later
  * frames order their own jobs behind it on the device (b200_stream_wait_event) without waiting on the host; ready: the job
  * and the copy into the host picture are complete */
-typedef struct HookRefPic { const void *key; void *dev; size_t bytes; int ready, submitted; void *event; uint64_t last_use; } HookRefPic;
+/* exported: an export into caller memory was enqueued and `export_event` marks its end — the entry's device buffer is not
+ * handed to another picture before that event has completed */
+typedef struct HookRefPic { const void *key; void *dev; size_t bytes; int ready, submitted; void *event; uint64_t last_use;
+                            void *export_event; int exported; } HookRefPic;
 HookRefPic *b200hook_refpic(const void *key, size_t bytes, int create);
+/* enqueues the export of a resident picture on `stream` behind the picture's own job, and records its export-done event */
+int b200hook_export_submit(HookRefPic *r, const B200ExportJob *job, void *stream);
+/* a decoder context (Dav1dContext *) opened for device output: its frame jobs and film grain leave the pictures in device
+ * memory and copy nothing back into the host pictures */
+int b200hook_device_only(const void *ctx);
 void b200hook_refpic_set_ready(HookRefPic *r, int ready);
 void b200hook_refpic_wait(HookRefPic *r);
 void b200hook_refpic_set_submitted(HookRefPic *r, int submitted);

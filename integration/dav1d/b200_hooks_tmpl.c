@@ -1058,7 +1058,8 @@ static int bitfn(run_frame)(HookFrame *const hf, const Dav1dFrameContext *const 
     uint8_t *const out = outp->dev;
     B200Xfer down[3];
     uint64_t d2h = 0, h2d = 0;
-    const int n_down = mono ? 1 : 3;
+    /* a context opened for device output keeps its pictures in HBM: nothing is copied into the host picture */
+    const int n_down = b200hook_device_only(f->c) ? 0 : mono ? 1 : 3;
     for (int p = 0; p < n_down; p++) {
         const int rows = p ? (f->cur.p.h + ss_ver) >> ss_ver : f->cur.p.h;
         down[p].host = f->sr_cur.p.data[p];
@@ -1137,7 +1138,14 @@ void bitfn(b200hook_filter_sbrow_lr)(Dav1dFrameContext *const f, const int sby) 
  * The decoded picture is still in HBM (keyed by its host buffer), so the whole job — grain LUTs, scaling LUTs, every
  * strip of every plane — runs as one b200 frame job when `prep` is called; the per-row calls have nothing left to do. */
 #include "src/fg_apply.h"
-static void bitfn(fg_whole_picture)(Dav1dPicture *const out, const Dav1dPicture *const in)
+/* the context whose dsp table the film-grain call came through (lib.c and thread_task.c pass &c->dsp[bpc index].fg) */
+static const Dav1dContext *bitfn(fg_context)(const Dav1dFilmGrainDSPContext *const dsp, const int bpc)
+{
+    const int idx = BITDEPTH == 8 ? 0 : (bpc >> 1) - 4;
+    return (const Dav1dContext *)((const char *)dsp - offsetof(Dav1dDSPContext, fg) - (size_t)idx * sizeof(Dav1dDSPContext) -
+                                  offsetof(Dav1dContext, dsp));
+}
+static void bitfn(fg_whole_picture)(const Dav1dFilmGrainDSPContext *const dsp, Dav1dPicture *const out, const Dav1dPicture *const in)
 {
     const B200Backend *const be = b200hook_backend();
     if (!be) { fprintf(stderr, "b200hook: film grain: no back end\n"); abort(); }      /* no error channel here (void, like dav1d's), no CPU fallback */
@@ -1155,6 +1163,14 @@ static void bitfn(fg_whole_picture)(Dav1dPicture *const out, const Dav1dPicture 
     const int resident = src && src->dev && src->bytes >= bytes && !(force && atoi(force));
     if (resident) b200hook_refpic_wait(src);
     const int same_pitch = out->stride[0] == in->stride[0] && (mono || out->stride[1] == in->stride[1]);
+    /* device output: the grained picture gets a resident device copy of its own, keyed by its host buffer like every decoded
+     * picture (the slot's pic[0] is overwritten by the next grained picture), and nothing is copied into the host picture */
+    HookRefPic *dst = NULL;
+    if (b200hook_device_only(bitfn(fg_context)(dsp, in->p.bpc))) {
+        /* (the host picture holds no pixels to upload) */
+        if (!resident || !same_pitch || !(dst = b200hook_refpic(out->data[0], bytes, 1))) { fprintf(stderr, "b200hook: film grain: no device picture\n"); abort(); }
+        b200hook_refpic_set_ready(dst, 0);
+    }
     static const char fg_slot_key = 0;
     HookFrame *const hf = b200hook_frame(&fg_slot_key);                  /* a slot of its own for the output stage */
     if (!hf) { fprintf(stderr, "b200hook: film grain: no slot\n"); abort(); }
@@ -1174,7 +1190,7 @@ static void bitfn(fg_whole_picture)(Dav1dPicture *const out, const Dav1dPicture 
     j.bitdepth_max = (1 << in->p.bpc) - 1;
 #endif
     j.run_fg = 1;
-    j.fg.in = resident ? src->dev : hf->pic[1].dev; j.fg.out = hf->pic[0].dev; j.fg.scratch = hf->scratch.dev;
+    j.fg.in = resident ? src->dev : hf->pic[1].dev; j.fg.out = dst ? dst->dev : hf->pic[0].dev; j.fg.scratch = hf->scratch.dev;
     j.fg.plane_off[0] = 0; j.fg.plane_off[1] = off1; j.fg.plane_off[2] = off2;
     j.fg.stride[0] = st0; j.fg.stride[1] = j.fg.stride[2] = st1;
     j.fg.w = in->p.w; j.fg.h = in->p.h; j.fg.ss_hor = ss_hor; j.fg.ss_ver = ss_ver;
@@ -1188,7 +1204,8 @@ static void bitfn(fg_whole_picture)(Dav1dPicture *const out, const Dav1dPicture 
                            (size_t)prow * j.fg.stride[p] * sizeof(pixel), hf->stream);
     }
     if (!r) r = be->frame_submit_host(&j, NULL, 0, NULL, 0, hf->stream);
-    for (int p = 0; p < npl && !r; p++) {
+    if (!r && dst && dst->event) r = be->event_record(dst->event, hf->stream);
+    for (int p = 0; p < npl && !r && !dst; p++) {
         const int prow = p ? (in->p.h + ss_ver) >> ss_ver : in->p.h, pw = p ? (in->p.w + ss_hor) >> ss_hor : in->p.w;
         const uint8_t *const d = (const uint8_t *)hf->pic[0].dev + (size_t)j.fg.plane_off[p] * sizeof(pixel);
         if (same_pitch) r = be->copy_async(out->data[p], d, (size_t)prow * j.fg.stride[p] * sizeof(pixel), hf->stream);
@@ -1201,22 +1218,42 @@ static void bitfn(fg_whole_picture)(Dav1dPicture *const out, const Dav1dPicture 
     b200hook_job_leave();
     pthread_mutex_unlock(&hf->lock);
     if (r || r2) { fprintf(stderr, "b200hook: film grain job failed: %s\n", be->last_error()); abort(); }
+    if (dst) b200hook_refpic_set_ready(dst, 1);
 }
 
 void bitfn(b200hook_apply_grain)(const Dav1dFilmGrainDSPContext *const dsp, Dav1dPicture *const out, const Dav1dPicture *const in)
 {
-    (void)dsp;
-    bitfn(fg_whole_picture)(out, in);
+    bitfn(fg_whole_picture)(dsp, out, in);
 }
 void bitfn(b200hook_prep_grain)(const Dav1dFilmGrainDSPContext *const dsp, Dav1dPicture *const out, const Dav1dPicture *const in,
                                 uint8_t scaling[3][SCALING_SIZE], entry grain_lut[3][GRAIN_HEIGHT + 1][GRAIN_WIDTH])
 {
-    (void)dsp; (void)scaling; (void)grain_lut;
-    bitfn(fg_whole_picture)(out, in);
+    (void)scaling; (void)grain_lut;
+    bitfn(fg_whole_picture)(dsp, out, in);
 }
 void bitfn(b200hook_apply_grain_row)(const Dav1dFilmGrainDSPContext *const dsp, Dav1dPicture *const out, const Dav1dPicture *const in,
                                      const uint8_t scaling[3][SCALING_SIZE], const entry grain_lut[3][GRAIN_HEIGHT + 1][GRAIN_WIDTH],
                                      const int row)
 {
     (void)dsp; (void)out; (void)in; (void)scaling; (void)grain_lut; (void)row;      /* done by the job prep started */
+}
+
+/* ---- export of an output picture from its device copy (b200hook_export_picture in b200_hooks.c) ------------------------
+ * Ungrained pictures are the frame job's output entry (OUT_KEY: with super-resolution the upscaled picture), grained ones the
+ * entry film grain made for them; either is keyed by the picture's data[0] and laid out as geom_of() says. */
+int bitfn(b200hook_export_picture)(const Dav1dPicture *const p, const B200ExportJob *const tmpl, void *const stream)
+{
+    PicGeom g;
+    bitfn(geom_of)(p, &g);
+    HookRefPic *const r = b200hook_refpic(p->data[0], 0, 0);
+    if (!r || !r->dev || r->bytes < g.bytes) { fprintf(stderr, "b200hook: export: the picture has no device copy\n"); return -1; }
+    b200hook_refpic_wait(r);
+    const int mono = p->p.layout == DAV1D_PIXEL_LAYOUT_I400;
+    B200ExportJob j = *tmpl;
+    j.src = r->dev;
+    for (int k = 0; k < 3; k++) { j.plane_off[k] = g.off[k]; j.stride[k] = g.stride[k]; }
+    j.w = p->p.w; j.h = p->p.h; j.mono = mono;
+    j.ss_hor = p->p.layout != DAV1D_PIXEL_LAYOUT_I444; j.ss_ver = mono || p->p.layout == DAV1D_PIXEL_LAYOUT_I420;
+    j.bitdepth_max = (1 << p->p.bpc) - 1;
+    return b200hook_export_submit(r, &j, stream);
 }

@@ -106,6 +106,84 @@ done:
     return res;
 }
 
+/* ---- the loop of refdrv_decode_stream split into calls, for callers that take each picture as it comes out:
+ *   h = refdrv_stream_open(...); for each temporal unit: refdrv_stream_send(h, tu) until it returns 0, taking the pictures
+ *   refdrv_stream_get(h, info, 0) offers after each call; then refdrv_stream_get(h, info, 1) until it returns EAGAIN (drain).
+ * A picture from refdrv_stream_get is held (refdrv_stream_picture) until refdrv_stream_release or the next get. */
+typedef struct RefdrvStream { Dav1dContext *c; Dav1dData d; Dav1dPicture pic; int held; } RefdrvStream;
+
+API void *refdrv_stream_open(int n_threads, int max_frame_delay, int apply_grain)
+{
+    Dav1dSettings s;
+    dav1d_default_settings(&s);
+    s.n_threads = n_threads;
+    s.max_frame_delay = max_frame_delay;
+    s.apply_grain = apply_grain;
+    RefdrvStream *const h = calloc(1, sizeof(*h));
+    if (!h) return NULL;
+    if (dav1d_open(&h->c, &s) < 0) { free(h); return NULL; }
+    return h;
+}
+
+/* the Dav1dContext * behind a stream (what per-context settings of a library are keyed by) */
+API const void *refdrv_stream_context(void *const hv) { return ((RefdrvStream *)hv)->c; }
+
+/* data = NULL: go on with the temporal unit that is still pending. Returns 0 when it has been consumed entirely, 1 when
+ * dav1d wants pictures taken out first (call again with NULL after refdrv_stream_get), < 0 on a dav1d error. */
+API int refdrv_stream_send(void *const hv, const uint8_t *const data, const uint64_t sz)
+{
+    RefdrvStream *const h = hv;
+    if (data) {
+        if (h->d.sz) return DAV1D_ERR(EINVAL);
+        uint8_t *const buf = dav1d_data_create(&h->d, (size_t)sz);
+        if (!buf) return DAV1D_ERR(ENOMEM);
+        memcpy(buf, data, (size_t)sz);
+    }
+    if (!h->d.sz) return 0;
+    const int r = dav1d_send_data(h->c, &h->d);
+    if (r < 0 && r != DAV1D_ERR(EAGAIN)) { dav1d_data_unref(&h->d); return r; }
+    return h->d.sz ? 1 : 0;
+}
+
+API void refdrv_stream_release(void *const hv)
+{
+    RefdrvStream *const h = hv;
+    if (h->held) { dav1d_picture_unref(&h->pic); h->held = 0; }
+}
+
+/* the next output picture: 0 and info = w, h, bpc, layout, mtrx, color_range; DAV1D_ERR(EAGAIN) when there is none (yet:
+ * drain = 0; any more: drain = 1), another negative value on a dav1d error */
+API int refdrv_stream_get(void *const hv, int32_t *const info, const int drain)
+{
+    RefdrvStream *const h = hv;
+    refdrv_stream_release(h);
+    for (int again = 0;;) {
+        memset(&h->pic, 0, sizeof(h->pic));
+        const int r = dav1d_get_picture(h->c, &h->pic);
+        /* draining: the first EAGAIN only arms dav1d's drain mode (src/lib.c, c->drain) */
+        if (r == DAV1D_ERR(EAGAIN) && drain && ++again < 2) continue;
+        if (r < 0) return r;
+        break;
+    }
+    h->held = 1;
+    const Dav1dPicture *const p = &h->pic;
+    info[0] = p->p.w; info[1] = p->p.h; info[2] = p->p.bpc; info[3] = (int32_t)p->p.layout;
+    info[4] = (int32_t)p->seq_hdr->mtrx; info[5] = p->seq_hdr->color_range;
+    return 0;
+}
+
+API const void *refdrv_stream_picture(void *const hv) { RefdrvStream *const h = hv; return h->held ? &h->pic : NULL; }
+
+API void refdrv_stream_close(void *const hv)
+{
+    RefdrvStream *const h = hv;
+    if (!h) return;
+    refdrv_stream_release(h);
+    dav1d_data_unref(&h->d);
+    dav1d_close(&h->c);
+    free(h);
+}
+
 /* Sends the first n_tu temporal units and closes the decoder at once, without draining: whatever frames are still
  * being decoded are flushed by dav1d_close (reference src/lib.c, dav1d_flush / close_internal). Test hook for the
  * back end's handling of abandoned frames. Returns the number of pictures that happened to come out. */
