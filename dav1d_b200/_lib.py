@@ -300,6 +300,7 @@ _SIGS = {
     "b200_event_sync": (C.c_int, [C.c_void_p]),
     # ---- export of a decoded picture
     "b200_export_picture": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "b200_export_tensor": (C.c_int, [C.c_void_p, C.c_void_p]),
     # ---- ipred
     "b200_ipred_batch": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "b200_ipred": (C.c_int, [C.c_int, C.c_void_p, C.c_ssize_t, C.c_void_p] + [C.c_int] * 6),
@@ -374,6 +375,18 @@ class ExportJob(C.Structure):
                 ("gv", C.c_int32), ("bu", C.c_int32), ("dst", C.c_void_p * 3), ("dst_pitch", C.c_int32 * 3), ("pad2", C.c_int32)]
 
 
+class TensorJob(C.Structure):
+    """B200TensorJob: export of a decoded picture as a resized, normalised float tensor (dtype 0 fp32, 1 fp16, 2 bf16;
+    layout 0 CHW, 1 HWC) into caller memory"""
+    _fields_ = [("src", C.c_void_p), ("plane_off", C.c_uint32 * 3), ("stride", C.c_int32 * 3), ("w", C.c_int32), ("h", C.c_int32),
+                ("ss_hor", C.c_int32), ("ss_ver", C.c_int32), ("mono", C.c_int32), ("bitdepth_max", C.c_int32),
+                ("out_w", C.c_int32), ("out_h", C.c_int32), ("dtype", C.c_int32), ("layout", C.c_int32),
+                ("full_range", C.c_int32), ("identity", C.c_int32), ("siting_x", C.c_int32), ("siting_y", C.c_int32),
+                ("cy", C.c_int32), ("rv", C.c_int32), ("gu", C.c_int32), ("gv", C.c_int32), ("bu", C.c_int32),
+                ("scale", C.c_float * 3), ("bias", C.c_float * 3), ("pad", C.c_int32),
+                ("dst", C.c_void_p), ("pitch_c", C.c_int64), ("pitch_y", C.c_int64)]
+
+
 ABI_STRUCTS = [McFrame, McBlock, CompBlock, BlendBlock, WarpBlock, ItxBlock, LfFrame, CdefFrame, LrFrame, FrameJob,
                Av1Filter, Av1Restoration, FgFrame, FilmGrainData, IntraTx, IntraFrame, McScaledBlock, CoefBlock, IntraSb, CompFusedBlock, FrameBand, ResizeFrame,
-               ExportJob]
+               ExportJob, TensorJob]

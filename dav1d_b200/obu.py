@@ -71,7 +71,9 @@ def _profile(bpc, layout):
 
 
 def sequence_header(w, h, bpc=8, sb128=0, film_grain=0, filter_intra=1, intra_edge_filter=1, cdef=1, restoration=1,
-                    inter_intra=1, masked_compound=1, warped_motion=1, screen_content=0, layout="420", super_res=0):
+                    inter_intra=1, masked_compound=1, warped_motion=1, screen_content=0, layout="420", super_res=0,
+                    chroma_sample_position=0):
+    """chroma_sample_position (4:2:0 only): enum Dav1dChromaSamplePosition, 0 unknown, 1 vertical, 2 colocated"""
     b = BitWriter()
     profile = _profile(bpc, layout)
     b.f(3, profile)
@@ -109,7 +111,7 @@ def sequence_header(w, h, bpc=8, sb128=0, film_grain=0, filter_intra=1, intra_ed
             if layout != "444":
                 b.f(1, 1 if layout == "420" else 0)
         if layout == "420":
-            b.f(2, 0)                        # chroma_sample_position
+            b.f(2, chroma_sample_position)   # chroma_sample_position
         b.f(1, 0)                            # separate_uv_delta_q
     b.f(1, film_grain)
     b.trailing()
@@ -286,10 +288,11 @@ def temporal_unit(*obus):
 
 
 def intra_stream(seed, w, h, n_frames=1, bpc=8, sb128=0, log2_cols=0, log2_rows=0, film_grain=0, screen_content=0, layout="420",
-                 super_res=0, **kw):
+                 super_res=0, chroma_sample_position=0, **kw):
     """A list of temporal units (bytes), each holding one shown key frame."""
     rng = np.random.default_rng(seed)
-    seq = sequence_header(w, h, bpc=bpc, sb128=sb128, film_grain=film_grain, screen_content=screen_content, layout=layout, super_res=super_res)
+    seq = sequence_header(w, h, bpc=bpc, sb128=sb128, film_grain=film_grain, screen_content=screen_content, layout=layout, super_res=super_res,
+                          chroma_sample_position=chroma_sample_position)
     kw = dict(kw, layout=layout, super_res=super_res)
     if film_grain:
         kw = dict(kw, film_grain_seq=1)
@@ -482,7 +485,7 @@ def show_existing_frame(slot):
 
 
 def inter_stream(seed, w, h, n_frames=3, bpc=8, sb128=0, log2_cols=0, log2_rows=0, motion_modes=0, film_grain=0, screen_content=0, layout="420",
-                 hidden_every=0, intra_only_every=0, sizes=None, super_res=0, **kw):
+                 hidden_every=0, intra_only_every=0, sizes=None, super_res=0, chroma_sample_position=0, **kw):
     """Temporal units: one key frame, then n_frames - 1 inter frames (single and compound references incl. wedge /
     difference-weighted masks and distance weights, switchable interpolation filters, variable transform trees, intra
     blocks; identity global motion). motion_modes=1 additionally enables the per-block motion mode (overlapped block
@@ -490,7 +493,8 @@ def inter_stream(seed, w, h, n_frames=3, bpc=8, sb128=0, log2_cols=0, log2_rows=
     every k-th inter frame a hidden future frame (decoded early, referenced with backward prediction, output later by a
     show_existing_frame header)."""
     rng = np.random.default_rng(seed)
-    seq = sequence_header(w, h, bpc=bpc, sb128=sb128, inter_intra=1 if motion_modes >= 2 else 0, warped_motion=1 if motion_modes else 0, film_grain=film_grain, screen_content=screen_content, layout=layout, super_res=super_res)
+    seq = sequence_header(w, h, bpc=bpc, sb128=sb128, inter_intra=1 if motion_modes >= 2 else 0, warped_motion=1 if motion_modes else 0, film_grain=film_grain, screen_content=screen_content, layout=layout, super_res=super_res,
+                          chroma_sample_position=chroma_sample_position)
     kw = dict(kw, layout=layout)
     if super_res:                            # every frame may then be coded narrower and upscaled; its references keep their upscaled size
         kw = dict(kw, super_res=1)

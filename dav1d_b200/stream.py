@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from ._lib import ExportJob  # noqa: F401  (B200ExportJob, filled by DeviceDecoder)
+from ._lib import ExportJob, TensorJob  # noqa: F401  (B200ExportJob / B200TensorJob, filled by DeviceDecoder)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -178,6 +178,67 @@ def rgb_reference(planes, bpc, layout, matrix, full_range):
     return np.clip(np.stack([(yy + rv * cr) >> 14, (yy - gu * cb - gv * cr) >> 14, (yy + bu * cb) >> 14]), 0, bdmax)
 
 
+TENSOR_DTYPES = {"float32": 0, "float16": 1, "bfloat16": 2}
+TENSOR_LAYOUTS = {"chw": 0, "hwc": 1}
+# chroma siting of the tensor export -> (horizontal, vertical): 1 = the chroma sample lies midway between two luma samples,
+# 0 = on the even one. "left" is the MPEG-2 convention (4:2:0 chroma co-sited with luma horizontally, midway vertically).
+SITINGS = {"left": (0, 1), "topleft": (0, 0), "center": (1, 1)}
+# the sequence header's chroma_sample_position (enum Dav1dChromaSamplePosition: 0 unknown, 1 vertical, 2 colocated) -> siting
+CHR_TO_SITING = {0: "left", 1: "left", 2: "topleft"}
+
+
+def tensor_scale_bias(bpc, mean=None, std=None):
+    """float32 (scale, bias) per channel of the tensor export: out = R * scale + bias with R in 0 .. 4 * bdmax, so that
+    out = (R / (4 * bdmax) - mean) / std; mean 0 and std 1 by default (outputs in [0, 1])"""
+    bdmax = (1 << bpc) - 1
+    mean = [0.0] * 3 if mean is None else [float(v) for v in mean]
+    std = [1.0] * 3 if std is None else [float(v) for v in std]
+    if len(mean) != 3 or len(std) != 3 or not all(v > 0 for v in std):
+        raise ValueError("mean and std need 3 values each, std > 0")
+    scale = np.array([1.0 / (4 * bdmax * s) for s in std], np.float32)
+    bias = np.array([-m / s for m, s in zip(mean, std)], np.float32)
+    return scale, bias
+
+
+def tensor_taps(out, inn, n, s=0, k=0):
+    """(i0, i1, f) of the tensor export's bilinear sampling along one axis (include/b200av1.h B200TensorJob): `out` output
+    samples from a plane of n samples whose luma axis has `inn`, sub-sampled by s, chroma sited by k"""
+    x = np.arange(out, dtype=np.int64)
+    pos = np.maximum(0, (2 * x + 1) * inn - (1 + k) * out) * (1 << (7 - s)) // out
+    i0 = np.minimum(pos >> 8, n - 1)
+    return i0, np.minimum(i0 + 1, n - 1), pos & 255
+
+
+def tensor_reference(planes, bpc, layout, size=None, matrix="bt709", full_range=False, siting="left", mean=None, std=None):
+    """numpy statement of the tensor export (include/b200av1.h B200TensorJob) for one picture's planes (layout = enum
+    Dav1dPixelLayout): float32 [3, OH, OW] of R, G, B; size = (OH, OW), by default the picture's"""
+    h, w = planes[0].shape
+    oh, ow = size or (h, w)
+    ssh, ssv = int(layout in (1, 2)), int(layout == 1)
+    kx, ky = SITINGS[siting]
+    s, bdmax = bpc - 8, (1 << bpc) - 1
+
+    def sample(p, sh, sv, kx, ky):
+        p = p.astype(np.int64)
+        x0, x1, fx = tensor_taps(ow, w, p.shape[1], sh, kx if sh else 0)
+        y0, y1, fy = tensor_taps(oh, h, p.shape[0], sv, ky if sv else 0)
+        a = p[np.ix_(y0, x0)] * (256 - fx) + p[np.ix_(y0, x1)] * fx
+        b = p[np.ix_(y1, x0)] * (256 - fx) + p[np.ix_(y1, x1)] * fx
+        return (a * (256 - fy)[:, None] + b * fy[:, None] + (1 << 13)) >> 14
+
+    y = sample(planes[0], 0, 0, 0, 0)
+    u, v = (None, None) if layout == 0 else (sample(planes[1], ssh, ssv, kx, ky), sample(planes[2], ssh, ssv, kx, ky))
+    if matrix == "identity":
+        rgb = np.stack([v, y, u])
+    else:
+        cy, rv, gu, gv, bu = rgb_coefficients(matrix, full_range)
+        yy = cy * (y - (0 if full_range else 64 << s)) + 8192
+        cb, cr = (0, 0) if u is None else (u - (512 << s), v - (512 << s))
+        rgb = np.clip(np.stack([(yy + rv * cr) >> 14, (yy - gu * cb - gv * cr) >> 14, (yy + bu * cb) >> 14]), 0, 4 * bdmax)
+    scale, bias = tensor_scale_bias(bpc, mean, std)
+    return rgb.astype(np.float32) * scale[:, None, None] + bias[:, None, None]
+
+
 class DeviceDecoder:
     """dav1d front end + B200 back end whose output pictures never leave the device: each one is exported by one kernel from
     its HBM copy into memory the caller allocates, and released at once.
@@ -186,6 +247,7 @@ class DeviceDecoder:
         for y, u, v in dec.pictures(tus):                      # torch.uint8 (8 bit) / torch.int16 (10, 12 bit) CUDA tensors
             ...
         for rgb in dec.pictures(tus, format="rgb"):             # [3, h, w], same dtype rule, stream bit depth
+        for x in dec.tensors(tus, size=(224, 224), dtype="bfloat16", batch=8):   # [n, 3, 224, 224] model input
 
     `backend` = path of the C-ABI library the hooks bind (default: the CUDA library); `serialize` = one device job at a time
     (for back ends that are not re-entrant, like the host emulator)."""
@@ -206,6 +268,8 @@ class DeviceDecoder:
         d.refdrv_stream_close.argtypes = [C.c_void_p]
         d.b200hook_set_device_only.argtypes = [C.c_void_p, C.c_int]
         d.b200hook_export_picture.argtypes = [C.c_void_p, C.POINTER(ExportJob), C.c_void_p]
+        d.b200hook_export_tensor.argtypes = [C.c_void_p, C.POINTER(TensorJob), C.c_void_p]
+        d.refdrv_stream_chroma_position.argtypes = [C.c_void_p]
 
     def stats(self, reset=False):
         return self._hooked.stats(reset)
@@ -226,12 +290,68 @@ class DeviceDecoder:
             raise ValueError("format must be 'planes' or 'rgb'")
         if matrix != "auto" and matrix != "identity" and matrix not in MATRICES:
             raise ValueError("unknown matrix %r" % (matrix,))
-        if alloc is None:
-            import torch
-            alloc = lambda shape, dtype: torch.empty(shape, dtype=getattr(torch, dtype), device="cuda")
-            if stream is None:
-                stream = torch.cuda.current_stream()
-        stream = getattr(stream, "cuda_stream", stream) or 0
+        alloc, stream = _default_alloc(alloc, stream)
+        yield from self._decode(tus, lambda h, info: self._export(h, info, format, matrix, full_range, alloc, stream))
+
+    def tensors(self, tus, size=None, dtype="float32", layout="chw", mean=None, std=None, matrix="auto", full_range=None,
+                chroma_siting="auto", batch=None, alloc=None, stream=None):
+        """Decodes the temporal units `tus` and yields every output picture as a model input: R, G, B resized to
+        size = (height, width) (default: the picture's own) by bilinear sampling at half-sample centres, like
+        torch.nn.functional.interpolate(mode="bilinear", align_corners=False) (chroma upsampling is part of the same
+        sampling), then (x - mean) / std with x in [0, 1], as a [3, OH, OW] (layout="chw") or [OH, OW, 3] ("hwc") tensor of
+        dtype "float32", "float16" or "bfloat16". One kernel per picture (include/b200av1.h, B200TensorJob).
+        batch=N: yields [n, ...] tensors of up to N pictures, each picture exported straight into its slot; a picture of
+        another size (size=None with frame-size changes) closes the batch early.
+        matrix and full_range: as in pictures(). chroma_siting: "auto" (the sequence header's chroma_sample_position:
+        colocated -> "topleft", vertical or unknown -> "left", the MPEG-2 convention), "left", "topleft" or "center".
+        alloc(shape, dtype) receives "float32", "float16" or "bfloat16"; alloc and stream otherwise mean what they mean in
+        pictures()."""
+        if dtype not in TENSOR_DTYPES or layout not in TENSOR_LAYOUTS:
+            raise ValueError("dtype must be one of %s, layout 'chw' or 'hwc'" % ", ".join(TENSOR_DTYPES))
+        if matrix != "auto" and matrix != "identity" and matrix not in MATRICES:
+            raise ValueError("unknown matrix %r" % (matrix,))
+        if chroma_siting != "auto" and chroma_siting not in SITINGS:
+            raise ValueError("unknown chroma siting %r" % (chroma_siting,))
+        if size is not None:
+            size = tuple(int(v) for v in size)
+            if len(size) != 2 or not all(1 <= v <= 65536 for v in size):
+                raise ValueError("size must be (height, width), each 1 .. 65536")
+        if batch is not None and int(batch) < 1:
+            raise ValueError("batch must be >= 1")
+        tensor_scale_bias(8, mean, std)                          # checks mean / std
+        alloc, stream = _default_alloc(alloc, stream)
+        esize = 4 if dtype == "float32" else 2
+        state = {"buf": None, "n": 0, "shape": None}
+
+        def export(h, info):
+            oh, ow = size or (int(info[1]), int(info[0]))
+            shape = (3, oh, ow) if layout == "chw" else (oh, ow, 3)
+            if batch is None:
+                out = alloc(shape, dtype)
+                self._export_tensor(h, info, _data_ptr(out), oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, stream)
+                return [out]
+            done = []
+            if state["buf"] is not None and state["shape"] != shape:       # another size closes the batch
+                done.append(state["buf"][:state["n"]])
+                state["buf"] = None
+            if state["buf"] is None:
+                state.update(buf=alloc((int(batch),) + shape, dtype), n=0, shape=shape)
+            dst = _data_ptr(state["buf"]) + state["n"] * 3 * oh * ow * esize
+            self._export_tensor(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, stream)
+            state["n"] += 1
+            if state["n"] == batch:
+                done.append(state["buf"])
+                state["buf"] = None
+            return done
+
+        for outs in self._decode(tus, export):
+            yield from outs
+        if state["buf"] is not None:
+            yield state["buf"][:state["n"]]
+
+    def _decode(self, tus, export):
+        """the decode loop of pictures() and tensors(): export(h, info) runs for every output picture while the stream
+        holds it (info = w, h, bpc, layout, matrix_coefficients, color_range), and what it returns is yielded"""
         self._hooked._bind()
         d = self.dll
         h = d.refdrv_stream_open(self.n_threads, self.max_frame_delay, self.apply_grain)
@@ -254,7 +374,7 @@ class DeviceDecoder:
                         if r < 0:
                             raise RuntimeError("decoding failed: dav1d error %d" % r)
                         try:
-                            out = self._export(h, info, format, matrix, full_range, alloc, stream)
+                            out = export(h, info)
                         finally:
                             d.refdrv_stream_release(h)
                         yield out
@@ -267,6 +387,35 @@ class DeviceDecoder:
             d.refdrv_stream_close(h)                # frames still in flight are flushed as device-output frames
             d.b200hook_set_device_only(ctx, 0)
 
+    @staticmethod
+    def _matrix(matrix, mtrx, layout):
+        name = MTRX_TO_MATRIX.get(mtrx, "bt709") if matrix == "auto" else matrix
+        if name == "identity" and layout != 3:
+            if matrix == "identity":
+                raise ValueError("the identity matrix needs a 4:4:4 picture")
+            name = "bt709"
+        return name
+
+    def _export_tensor(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, stream):
+        w, hh, bpc, pl, mtrx, color_range = (int(v) for v in info)
+        job = TensorJob()
+        job.out_w, job.out_h, job.dtype, job.layout = ow, oh, TENSOR_DTYPES[dtype], TENSOR_LAYOUTS[layout]
+        name = self._matrix(matrix, mtrx, pl)
+        job.identity = name == "identity"
+        job.full_range = int(bool(color_range if full_range is None else full_range))
+        if not job.identity:
+            job.cy, job.rv, job.gu, job.gv, job.bu = rgb_coefficients(name, job.full_range)
+        if siting == "auto":
+            siting = CHR_TO_SITING.get(self.dll.refdrv_stream_chroma_position(h), "left")
+        job.siting_x, job.siting_y = SITINGS[siting]
+        scale, bias = tensor_scale_bias(bpc, mean, std)
+        for c in range(3):
+            job.scale[c], job.bias[c] = float(scale[c]), float(bias[c])
+        job.dst = dst
+        job.pitch_y, job.pitch_c = (ow, oh * ow) if layout == "chw" else (3 * ow, 1)
+        if self.dll.b200hook_export_tensor(self.dll.refdrv_stream_picture(h), C.byref(job), C.c_void_p(stream)) != 0:
+            raise RuntimeError("exporting a picture failed (see stderr)")
+
     def _export(self, h, info, format, matrix, full_range, alloc, stream):
         w, hh, bpc, layout, mtrx, color_range = (int(v) for v in info)
         dtype = "uint8" if bpc == 8 else "int16"
@@ -278,11 +427,7 @@ class DeviceDecoder:
                 job.dst[k], job.dst_pitch[k] = _data_ptr(o), plane_dims(w, hh, layout)[k][0]
             result = tuple(outs)
         else:
-            name = MTRX_TO_MATRIX.get(mtrx, "bt709") if matrix == "auto" else matrix
-            if name == "identity" and layout != 3:
-                if matrix == "identity":
-                    raise ValueError("the identity matrix needs a 4:4:4 picture")
-                name = "bt709"
+            name = self._matrix(matrix, mtrx, layout)
             job.identity = name == "identity"
             job.full_range = int(bool(color_range if full_range is None else full_range))
             if not job.identity:
@@ -297,6 +442,16 @@ class DeviceDecoder:
 
 
 _EAGAIN = -11
+
+
+def _default_alloc(alloc, stream):
+    """(alloc, cudaStream_t handle) of an export: torch CUDA tensors on the current stream unless the caller brings its own"""
+    if alloc is None:
+        import torch
+        alloc = lambda shape, dtype: torch.empty(shape, dtype=getattr(torch, dtype), device="cuda")
+        if stream is None:
+            stream = torch.cuda.current_stream()
+    return alloc, getattr(stream, "cuda_stream", stream) or 0
 
 
 def _data_ptr(a):

@@ -641,7 +641,7 @@ B200_API int b200_frame_run_batch(const B200FrameJob *const *jobs, int n_jobs, v
 /* sizeof() of the ABI structs as compiled into the library (binding self-check): 0 McFrame, 1 McBlock, 2 CompBlock,
  * 3 BlendBlock, 4 WarpBlock, 5 ItxBlock, 6 LfFrame, 7 CdefFrame, 8 LrFrame, 9 FrameJob, 10 Av1Filter, 11 Av1Restoration,
  * 12 FgFrame, 13 FilmGrainData, 14 IntraTx, 15 IntraFrame, 16 McScaledBlock, 17 CoefBlock, 18 IntraSb, 19 CompFusedBlock,
- * 20 FrameBand, 21 ResizeFrame, 22 ExportJob */
+ * 20 FrameBand, 21 ResizeFrame, 22 ExportJob, 23 TensorJob */
 B200_API int b200_struct_size(int which);
 
 /* ==== band-sliced frame job + cross-GPU reference exchange (SURVEY.md §8e) ===================== */
@@ -780,6 +780,49 @@ typedef struct B200ExportJob {
     int32_t pad2;
 } B200ExportJob;
 B200_API int b200_export_picture(const B200ExportJob *job, void *stream);
+
+/* ==== export of a decoded picture as a model-ready float tensor ============================== */
+/* Reads the device copy of a decoded picture (source fields as in B200ExportJob: the visible picture is w x h, planes of
+ * pw x ph samples, chroma sub-sampled by ss_hor / ss_ver, bdmax = bitdepth_max) and writes R, G, B resized to
+ * out_w x out_h (1 .. 65536 each), normalised, as float32 / float16 / bfloat16. Integer arithmetic up to the last step:
+ *   Taps, per axis and plane: OUT = output length on the axis, IN = luma length (w or h), n = plane length, s = the plane's
+ *     sub-sampling on the axis (luma 0), k = chroma siting on the axis when s = 1, else 0 (siting_x / siting_y: 1 = chroma
+ *     sample centred between two luma samples, 0 = on the even luma sample). For output index x, in int64:
+ *       pos = floor(max(0, (2x + 1) * IN - (1 + k) * OUT) * 2^(7 - s) / OUT)
+ *       i0 = min(pos >> 8, n - 1), i1 = min(i0 + 1, n - 1), f = pos & 255
+ *     bilinear sampling at half-sample centres (torch's interpolate(mode="bilinear", align_corners=False)) with positions
+ *     kept to 1/256 sample; upsampling chroma and resizing are one operation.
+ *   Samples, per plane: V = (S[y0][x0] * (256 - fx) + S[y0][x1] * fx) * (256 - fy) + (S[y1][x0] * (256 - fx) + S[y1][x1] * fx) * fy
+ *     Q = (V + 2^13) >> 14: the sample with 2 fractional bits, 0 .. 4 * bdmax.
+ *   Matrix, with s = bitdepth - 8: Y' = Qy - (full_range ? 0 : 64 << s), C' = Qc - (512 << s) (mono: Cb' = Cr' = 0), and
+ *       R = clip((cy * Y' + rv * Cr' + 8192) >> 14)
+ *       G = clip((cy * Y' - gu * Cb' - gv * Cr' + 8192) >> 14)
+ *       B = clip((cy * Y' + bu * Cb' + 8192) >> 14)
+ *     in int32 with a flooring shift, clip to [0, 4 * bdmax]. identity (4:4:4 only): R = Qcr, G = Qy, B = Qcb.
+ *   Output, per channel c: out = ((float)R_c * scale[c]) + bias[c], a float32 multiply and a float32 add, each rounded to
+ *     nearest (never fused); float16 / bfloat16 are that float32 rounded to nearest even. The Python binding passes
+ *     scale = f32(1 / (4 * bdmax * std)), bias = f32(-mean / std); mean 0 and std 1 give outputs in [0, 1].
+ * Destination (pitches in elements): CHW: dst + c * pitch_c + y * pitch_y + x, pitch_y >= out_w and
+ * pitch_c >= (out_h - 1) * pitch_y + out_w (channels may not overlap); HWC: dst + y * pitch_y + 3 * x + c,
+ * pitch_y >= 3 * out_w, pitch_c unused. dst aligned to the element size. One launch on `stream`; -2 on bad arguments. */
+enum { B200_TENSOR_F32 = 0, B200_TENSOR_F16 = 1, B200_TENSOR_BF16 = 2 };
+enum { B200_TENSOR_CHW = 0, B200_TENSOR_HWC = 1 };
+typedef struct B200TensorJob {
+    const void *src;               /* device picture */
+    uint32_t plane_off[3];         /* samples */
+    int32_t stride[3];             /* samples */
+    int32_t w, h, ss_hor, ss_ver, mono, bitdepth_max;
+    int32_t out_w, out_h;
+    int32_t dtype, layout;         /* B200_TENSOR_F32 / F16 / BF16, B200_TENSOR_CHW / HWC */
+    int32_t full_range, identity;
+    int32_t siting_x, siting_y;    /* 0 or 1, see above */
+    int32_t cy, rv, gu, gv, bu;    /* the matrix, 1.0 = 1 << 14 (as B200ExportJob) */
+    float scale[3], bias[3];       /* per output channel R, G, B */
+    int32_t pad;
+    void *dst;                     /* device */
+    int64_t pitch_c, pitch_y;      /* elements */
+} B200TensorJob;
+B200_API int b200_export_tensor(const B200TensorJob *job, void *stream);
 
 #ifdef __cplusplus
 }

@@ -70,12 +70,12 @@ API int b200hook_set_backend(const char *path)
     SYM(event_create, "b200_event_create"); SYM(event_destroy, "b200_event_destroy");
     SYM(event_record, "b200_event_record"); SYM(stream_wait_event, "b200_stream_wait_event");
     SYM(struct_size, "b200_struct_size");
-    SYM(event_sync, "b200_event_sync"); SYM(export_picture, "b200_export_picture");
+    SYM(event_sync, "b200_event_sync"); SYM(export_picture, "b200_export_picture"); SYM(export_tensor, "b200_export_tensor");
 #undef SYM
     /* binding self-check: the structs this file was compiled with are the ones the library was compiled with */
     if (be.struct_size(9) != (int)sizeof(B200FrameJob) || be.struct_size(14) != (int)sizeof(B200IntraTx) ||
         be.struct_size(10) != (int)sizeof(B200Av1Filter) || be.struct_size(11) != (int)sizeof(B200Av1Restoration) ||
-        be.struct_size(22) != (int)sizeof(B200ExportJob)) {
+        be.struct_size(22) != (int)sizeof(B200ExportJob) || be.struct_size(23) != (int)sizeof(B200TensorJob)) {
         fprintf(stderr, "b200hook: ABI struct size mismatch with %s\n", path);
         dlclose(h);
         return -1;
@@ -316,7 +316,7 @@ void b200hook_refpic_forget(const void *const key)
     pthread_mutex_unlock(&g_lock);
 }
 
-int b200hook_export_submit(HookRefPic *const r, const B200ExportJob *const job, void *const stream)
+int b200hook_export_submit(HookRefPic *const r, const int tensor, const void *const job, void *const stream)
 {
     const B200Backend *const be = b200hook_backend();
     if (!be) return -1;
@@ -326,7 +326,7 @@ int b200hook_export_submit(HookRefPic *const r, const B200ExportJob *const job, 
     pthread_mutex_unlock(&g_lock);
     b200hook_job_enter();
     int rc = r->event ? be->stream_wait_event(stream, r->event) : 0;
-    if (!rc) rc = be->export_picture(job, stream);
+    if (!rc) rc = tensor ? be->export_tensor(job, stream) : be->export_picture(job, stream);
     if (!rc) rc = done ? be->event_record(done, stream) : be->frame_wait(stream);      /* no event: the export completes here */
     b200hook_job_leave();
     if (rc) { fprintf(stderr, "b200hook: export failed (%d): %s\n", rc, be->last_error()); return rc; }
@@ -368,6 +368,15 @@ API int b200hook_export_picture(const Dav1dPicture *const p, const B200ExportJob
 {
     if (!p || !tmpl || !p->data[0]) return -1;
     return p->p.bpc > 8 ? b200hook_export_picture_16bpc(p, tmpl, stream) : b200hook_export_picture_8bpc(p, tmpl, stream);
+}
+int b200hook_export_tensor_8bpc(const Dav1dPicture *p, const B200TensorJob *tmpl, void *stream);
+int b200hook_export_tensor_16bpc(const Dav1dPicture *p, const B200TensorJob *tmpl, void *stream);
+/* The same for the tensor export: `tmpl` carries the output size, dtype, layout, siting, matrix, scale / bias and the
+ * destination; the source geometry is the picture's own. */
+API int b200hook_export_tensor(const Dav1dPicture *const p, const B200TensorJob *const tmpl, void *const stream)
+{
+    if (!p || !tmpl || !p->data[0]) return -1;
+    return p->p.bpc > 8 ? b200hook_export_tensor_16bpc(p, tmpl, stream) : b200hook_export_tensor_8bpc(p, tmpl, stream);
 }
 void b200hook_refpic_set_ready(HookRefPic *r, int ready)
 {

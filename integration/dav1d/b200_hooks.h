@@ -36,6 +36,7 @@ typedef struct B200Backend {
     int (*struct_size)(int);
     int (*event_sync)(void *);
     int (*export_picture)(const B200ExportJob *, void *);
+    int (*export_tensor)(const B200TensorJob *, void *);
 } B200Backend;
 const B200Backend *b200hook_backend(void);   /* NULL (after logging) when no back end is loaded: the decode fails */
 
@@ -136,8 +137,9 @@ static inline void *b200hook_tile_append(HookFrame *const hf, const int tile, co
 typedef struct HookRefPic { const void *key; void *dev; size_t bytes; int ready, submitted; void *event; uint64_t last_use;
                             void *export_event; int exported; } HookRefPic;
 HookRefPic *b200hook_refpic(const void *key, size_t bytes, int create);
-/* enqueues the export of a resident picture on `stream` behind the picture's own job, and records its export-done event */
-int b200hook_export_submit(HookRefPic *r, const B200ExportJob *job, void *stream);
+/* enqueues the export of a resident picture on `stream` behind the picture's own job, and records its export-done event:
+ * `job` is a B200ExportJob (b200_export_picture) or, with `tensor` set, a B200TensorJob (b200_export_tensor) */
+int b200hook_export_submit(HookRefPic *r, int tensor, const void *job, void *stream);
 /* a decoder context (Dav1dContext *) opened for device output: its frame jobs and film grain leave the pictures in device
  * memory and copy nothing back into the host pictures */
 int b200hook_device_only(const void *ctx);

@@ -1238,22 +1238,42 @@ void bitfn(b200hook_apply_grain_row)(const Dav1dFilmGrainDSPContext *const dsp, 
     (void)dsp; (void)out; (void)in; (void)scaling; (void)grain_lut; (void)row;      /* done by the job prep started */
 }
 
-/* ---- export of an output picture from its device copy (b200hook_export_picture in b200_hooks.c) ------------------------
+/* ---- export of an output picture from its device copy (b200hook_export_picture / _tensor in b200_hooks.c) --------------
  * Ungrained pictures are the frame job's output entry (OUT_KEY: with super-resolution the upscaled picture), grained ones the
- * entry film grain made for them; either is keyed by the picture's data[0] and laid out as geom_of() says. */
+ * entry film grain made for them; either is keyed by the picture's data[0] and laid out as geom_of() says. Both jobs take
+ * the same source fields from it. */
+#define EXPORT_SOURCE(j, r, g, p) do { \
+        const int mono_ = (p)->p.layout == DAV1D_PIXEL_LAYOUT_I400; \
+        (j).src = (r)->dev; \
+        for (int k = 0; k < 3; k++) { (j).plane_off[k] = (g).off[k]; (j).stride[k] = (g).stride[k]; } \
+        (j).w = (p)->p.w; (j).h = (p)->p.h; (j).mono = mono_; \
+        (j).ss_hor = (p)->p.layout != DAV1D_PIXEL_LAYOUT_I444; (j).ss_ver = mono_ || (p)->p.layout == DAV1D_PIXEL_LAYOUT_I420; \
+        (j).bitdepth_max = (1 << (p)->p.bpc) - 1; \
+    } while (0)
+static HookRefPic *bitfn(export_source)(const Dav1dPicture *const p, PicGeom *const g)
+{
+    bitfn(geom_of)(p, g);
+    HookRefPic *const r = b200hook_refpic(p->data[0], 0, 0);
+    if (!r || !r->dev || r->bytes < g->bytes) { fprintf(stderr, "b200hook: export: the picture has no device copy\n"); return NULL; }
+    b200hook_refpic_wait(r);
+    return r;
+}
 int bitfn(b200hook_export_picture)(const Dav1dPicture *const p, const B200ExportJob *const tmpl, void *const stream)
 {
     PicGeom g;
-    bitfn(geom_of)(p, &g);
-    HookRefPic *const r = b200hook_refpic(p->data[0], 0, 0);
-    if (!r || !r->dev || r->bytes < g.bytes) { fprintf(stderr, "b200hook: export: the picture has no device copy\n"); return -1; }
-    b200hook_refpic_wait(r);
-    const int mono = p->p.layout == DAV1D_PIXEL_LAYOUT_I400;
+    HookRefPic *const r = bitfn(export_source)(p, &g);
+    if (!r) return -1;
     B200ExportJob j = *tmpl;
-    j.src = r->dev;
-    for (int k = 0; k < 3; k++) { j.plane_off[k] = g.off[k]; j.stride[k] = g.stride[k]; }
-    j.w = p->p.w; j.h = p->p.h; j.mono = mono;
-    j.ss_hor = p->p.layout != DAV1D_PIXEL_LAYOUT_I444; j.ss_ver = mono || p->p.layout == DAV1D_PIXEL_LAYOUT_I420;
-    j.bitdepth_max = (1 << p->p.bpc) - 1;
-    return b200hook_export_submit(r, &j, stream);
+    EXPORT_SOURCE(j, r, g, p);
+    return b200hook_export_submit(r, 0, &j, stream);
 }
+int bitfn(b200hook_export_tensor)(const Dav1dPicture *const p, const B200TensorJob *const tmpl, void *const stream)
+{
+    PicGeom g;
+    HookRefPic *const r = bitfn(export_source)(p, &g);
+    if (!r) return -1;
+    B200TensorJob j = *tmpl;
+    EXPORT_SOURCE(j, r, g, p);
+    return b200hook_export_submit(r, 1, &j, stream);
+}
+#undef EXPORT_SOURCE

@@ -174,6 +174,13 @@ API int refdrv_stream_get(void *const hv, int32_t *const info, const int drain)
 
 API const void *refdrv_stream_picture(void *const hv) { RefdrvStream *const h = hv; return h->held ? &h->pic : NULL; }
 
+/* the chroma sample position of the held picture's sequence header (enum Dav1dChromaSamplePosition), -1 when none is held */
+API int refdrv_stream_chroma_position(void *const hv)
+{
+    RefdrvStream *const h = hv;
+    return h->held ? (int)h->pic.seq_hdr->chr : -1;
+}
+
 API void refdrv_stream_close(void *const hv)
 {
     RefdrvStream *const h = hv;

@@ -1,0 +1,213 @@
+"""The tensor export (b200_export_tensor) against the torch chain it replaces (run on a GPU machine):
+
+    python tools/bench_tensor_export.py [--launches 200] [--rounds 5] [--reps 3] [--out FILE]
+
+Kernel level, one JSON line per configuration, on synthetic device pictures (random planes, 4:2:0):
+  fused        one b200_export_tensor launch
+  torch_chain  b200_export_picture (RGB at the stream's bit depth, nearest chroma), then x.float() / bdmax,
+               interpolate(bilinear, align_corners=False) when resizing, (x - mean) / std, .to(dtype), and for HWC
+               .permute(1, 2, 0).contiguous()
+  Each is timed with CUDA events around --launches back-to-back launches after a warm-up (a sleep kernel holds the stream
+  while they are enqueued, so the events time the GPU, not the host); the two alternate for --rounds
+  rounds in the same run, and the median and min of the rounds' per-launch times are reported. `bytes` are algorithmic
+  (computed from the shapes: every tensor each step reads and writes, once), `share_of_3.35TBps` their rate against the
+  H100 SXM data sheet.
+Decoder level, one JSON line per stream workload of bench.py: pictures per second of
+  DeviceDecoder.tensors(size, dtype="bfloat16", batch=8) against DeviceDecoder.pictures(format="rgb") followed by the
+  torch chain and torch.stack of every 8, the whole stream per run (median, min and max of --reps runs, alternated).
+The GPU's name, power limit and SM clock are read in the same run."""
+import argparse
+import ctypes as C
+import json
+import os
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+import torch.nn.functional as F  # noqa: E402
+
+from dav1d_b200 import _lib, stream  # noqa: E402
+from bench_device_output import HBM_BYTES_PER_S, gpu_info, workload_tus  # noqa: E402
+
+MEAN, STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
+ESIZE = {"float32": 4, "float16": 2, "bfloat16": 2}
+CONFIGS = [  # (name, source w, h, bpc, output (h, w) or None, dtype, layout)
+    ("1080p8 native fp32 chw", 1920, 1080, 8, None, "float32", "chw"),
+    ("1080p8 native bf16 hwc", 1920, 1080, 8, None, "bfloat16", "hwc"),
+    ("4k10 native fp32 chw", 3840, 2160, 10, None, "float32", "chw"),
+    ("4k10 native bf16 hwc", 3840, 2160, 10, None, "bfloat16", "hwc"),
+    ("4k10 -> 1920x1080 bf16 chw", 3840, 2160, 10, (1080, 1920), "bfloat16", "chw"),
+    ("1080p8 -> 640x360 fp16 chw", 1920, 1080, 8, (360, 640), "float16", "chw"),
+]
+
+
+def torch_chain(rgb, bdmax, size, dtype, layout, mean, std):
+    x = rgb.float() / bdmax
+    if size is not None:
+        x = F.interpolate(x[None], size=size, mode="bilinear", align_corners=False)[0]
+    x = ((x - mean) / std).to(getattr(torch, dtype))
+    return x.permute(1, 2, 0).contiguous() if layout == "hwc" else x
+
+
+def chain_bytes(w, h, sb, size, dtype, layout):
+    """algorithmic bytes of the torch chain: each step reads its input and writes its output once"""
+    px, (oh, ow) = w * h, size or (h, w)
+    op = oh * ow
+    b = w * h * 3 // 2 * sb + 3 * px * sb            # export: YUV in, RGB out
+    b += 3 * px * sb + 3 * px * 4 + 2 * 3 * px * 4   # .float(), / bdmax
+    if size is not None:
+        b += 3 * px * 4 + 3 * op * 4                 # interpolate
+    b += 2 * (2 * 3 * op * 4)                        # - mean, / std
+    b += 3 * op * 4 + 3 * op * ESIZE[dtype]          # .to(dtype)
+    if layout == "hwc":
+        b += 2 * 3 * op * ESIZE[dtype]               # .contiguous()
+    return b
+
+
+def kernel_level(args):
+    lib = _lib.get_lib()
+    s = torch.cuda.Stream()
+    lines = []
+    for name, w, h, bpc, size, dtype, layout in CONFIGS:
+        rng = np.random.default_rng(w + bpc)
+        bdmax, sb = (1 << bpc) - 1, 1 if bpc == 8 else 2
+        planes = [rng.integers(0, bdmax + 1, (ph, pw)).astype(np.uint8 if bpc == 8 else np.int16) for pw, ph in stream.plane_dims(w, h, 1)]
+        src = torch.from_numpy(np.concatenate([p.ravel() for p in planes])).cuda()
+        offs = [0, planes[0].size, planes[0].size + planes[1].size]
+        oh, ow = size or (h, w)
+        shape = (3, oh, ow) if layout == "chw" else (oh, ow, 3)
+        out = torch.empty(shape, dtype=getattr(torch, dtype), device="cuda")
+        tj = stream.TensorJob()
+        tj.src = src.data_ptr()
+        for k in range(3):
+            tj.plane_off[k], tj.stride[k] = offs[k], planes[k].shape[1]
+        tj.w, tj.h, tj.ss_hor, tj.ss_ver, tj.bitdepth_max = w, h, 1, 1, bdmax
+        tj.out_w, tj.out_h = ow, oh
+        tj.dtype, tj.layout, tj.siting_x, tj.siting_y = stream.TENSOR_DTYPES[dtype], stream.TENSOR_LAYOUTS[layout], 0, 1
+        tj.cy, tj.rv, tj.gu, tj.gv, tj.bu = stream.rgb_coefficients("bt709", False)
+        scale, bias = stream.tensor_scale_bias(bpc, MEAN, STD)
+        for c in range(3):
+            tj.scale[c], tj.bias[c] = float(scale[c]), float(bias[c])
+        tj.dst, tj.pitch_c, tj.pitch_y = out.data_ptr(), (oh * ow if layout == "chw" else 1), (ow if layout == "chw" else 3 * ow)
+        rgb = torch.empty((3, h, w), dtype=torch.uint8 if bpc == 8 else torch.int16, device="cuda")
+        ej = stream.ExportJob()
+        ej.src, ej.format = src.data_ptr(), 1
+        for k in range(3):
+            ej.plane_off[k], ej.stride[k] = offs[k], planes[k].shape[1]
+            ej.dst[k], ej.dst_pitch[k] = rgb.data_ptr() + k * h * w * sb, w
+        ej.w, ej.h, ej.ss_hor, ej.ss_ver, ej.bitdepth_max = w, h, 1, 1, bdmax
+        ej.cy, ej.rv, ej.gu, ej.gv, ej.bu = tj.cy, tj.rv, tj.gu, tj.gv, tj.bu
+        mean = torch.tensor(MEAN, device="cuda").view(3, 1, 1)
+        std = torch.tensor(STD, device="cuda").view(3, 1, 1)
+        sp = C.c_void_p(s.cuda_stream)
+
+        def fused():
+            lib.check(lib.b200_export_tensor(C.byref(tj), sp), "b200_export_tensor")
+
+        def chain():
+            lib.check(lib.b200_export_picture(C.byref(ej), sp), "b200_export_picture")
+            torch_chain(rgb, bdmax, size, dtype, layout, mean, std)
+
+        times = {"fused": [], "torch_chain": []}
+        with torch.cuda.stream(s):
+            for f in (fused, chain):
+                for _ in range(20):
+                    f()
+            for _ in range(args.rounds):
+                for key, f in (("fused", fused), ("torch_chain", chain)):
+                    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    torch.cuda._sleep(50_000_000)            # holds the stream while the launches are enqueued
+                    a.record(s)
+                    for _ in range(args.launches):
+                        f()
+                    b.record(s)
+                    b.synchronize()
+                    times[key].append(1e3 * a.elapsed_time(b) / args.launches)
+        fused_bytes = w * h * 3 // 2 * sb + 3 * oh * ow * ESIZE[dtype]
+        line = {"config": name, "gpu": gpu_info(), "launches_per_round": args.launches, "rounds": args.rounds, "us": {}, "bytes": {
+            "fused": fused_bytes, "torch_chain": chain_bytes(w, h, sb, size, dtype, layout)}, "GBps": {}, "share_of_3.35TBps": {}}
+        for key, v in times.items():
+            med = float(np.median(v))
+            line["us"][key] = {"median": round(med, 2), "min": round(min(v), 2)}
+            line["GBps"][key] = round(line["bytes"][key] / (med * 1e-6) / 1e9, 1)
+            line["share_of_3.35TBps"][key] = round(line["bytes"][key] / (med * 1e-6) / HBM_BYTES_PER_S, 3)
+        line["speedup_median"] = round(line["us"]["torch_chain"]["median"] / line["us"]["fused"]["median"], 2)
+        print(json.dumps(line), flush=True)
+        lines.append(line)
+    return lines
+
+
+def decoder_level(args):
+    import bench
+    lines = []
+    for name in ("stream1080p8_inter", "stream4k10"):
+        W = bench.STREAM_WORKLOADS[name]
+        tus = workload_tus(name)
+        fg = int(W.get("film_grain", 0))
+        nthr = min(os.cpu_count() or 2, 32)
+        mfd = min(8, W["frames"], nthr)
+        dev = stream.DeviceDecoder(n_threads=nthr, max_frame_delay=mfd, apply_grain=fg)
+        size, bdmax = (W["H"] // 2, W["W"] // 2), (1 << W["bpc"]) - 1
+        mean = torch.tensor(MEAN, device="cuda").view(3, 1, 1)
+        std = torch.tensor(STD, device="cuda").view(3, 1, 1)
+        s = torch.cuda.Stream()
+
+        def fused():
+            n = 0
+            for b in dev.tensors(tus, size=size, dtype="bfloat16", batch=8, mean=MEAN, std=STD, stream=s):
+                n += b.shape[0]
+            return n
+
+        def chain():
+            n, pend = 0, []
+            for rgb in dev.pictures(tus, format="rgb", stream=s):
+                pend.append(torch_chain(rgb, bdmax, size, "bfloat16", "chw", mean, std))
+                if len(pend) == 8:
+                    n += torch.stack(pend).shape[0]
+                    pend = []
+            return n + (torch.stack(pend).shape[0] if pend else 0)
+
+        arms = {"tensors_bf16_batch8": fused, "pictures_rgb_plus_torch_chain": chain}
+        dts = {k: [] for k in arms}
+        with torch.cuda.stream(s):
+            for f in arms.values():
+                f()
+            for _ in range(args.reps):
+                for k, f in arms.items():
+                    torch.cuda.synchronize()
+                    t0 = time.perf_counter()
+                    assert f() == W["frames"], k
+                    torch.cuda.synchronize()
+                    dts[k].append(time.perf_counter() - t0)
+        line = {"workload": name, "gpu": gpu_info(), "frames": W["frames"], "output": "%dx%d bf16 chw, batches of 8" % (size[1], size[0]),
+                "dav1d_threads": nthr, "frames_in_flight": mfd, "reps": args.reps,
+                "fps": {k: round(W["frames"] / float(np.median(v)), 2) for k, v in dts.items()},
+                "fps_min_max": {k: [round(W["frames"] / max(v), 2), round(W["frames"] / min(v), 2)] for k, v in dts.items()}}
+        dev.release()
+        print(json.dumps(line), flush=True)
+        lines.append(line)
+    return lines
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--launches", type=int, default=200)
+    ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--out")
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "needs a CUDA device"
+    lines = kernel_level(args) + decoder_level(args)
+    if args.out:
+        with open(args.out, "w") as fh:
+            for line in lines:
+                fh.write(json.dumps(line) + "\n")
+
+
+if __name__ == "__main__":
+    main()
