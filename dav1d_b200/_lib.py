@@ -301,6 +301,7 @@ _SIGS = {
     # ---- export of a decoded picture
     "b200_export_picture": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_export_tensor": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "b200_export_tensor_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     # ---- ipred
     "b200_ipred_batch": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "b200_ipred": (C.c_int, [C.c_int, C.c_void_p, C.c_ssize_t, C.c_void_p] + [C.c_int] * 6),

@@ -181,15 +181,24 @@ B200_DEV typename TensorElem<DT>::type tensor_value(int v, float scale, float bi
     else return f;
 }
 
-// grid (runs of 4 output columns / 32, output rows / (8 * kTensorRows)), block (32, 8): a thread converts its run of 4
-// columns on kTensorRows rows 8 apart, so the column taps are worked out once for all of them
+// The jobs of one launch travel in the kernel's parameter block (no staging copy): B200_TENSOR_BATCH_MAX of them fit the
+// classic 4 KB limit. A one-job launch takes the N = 1 form: its job's fields are then read at fixed parameter offsets, as
+// operands of the instructions that use them; indexed by blockIdx.z they are separate loads, which made the prologue of a
+// small one-picture export up to a quarter slower.
+template <int N> struct TensorBatch { B200TensorJob job[N]; };
+static_assert(sizeof(TensorBatch<B200_TENSOR_BATCH_MAX>) <= 4096, "the jobs of one launch must fit a 4 KB kernel parameter block");
+
+// grid (runs of 4 output columns / 32, output rows / (8 * kTensorRows), jobs), block (32, 8): x / y cover the largest
+// output of the launch, z selects the job. A thread converts its run of 4 columns on kTensorRows rows 8 apart, so the
+// column taps are worked out once for all of them
 constexpr int kTensorRows = 4;
-template <bool HBD, int DT, bool HWC>
-__global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constant__ B200TensorJob j)
+template <bool HBD, int DT, bool HWC, int N>
+__global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constant__ TensorBatch<N> b)
 {
     B200_PDL_ENTRY();
     typedef typename Bd<HBD>::pixel pixel;
     typedef typename TensorElem<DT>::type E;
+    const B200TensorJob &j = b.job[N == 1 ? 0 : blockIdx.z];
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4, y0 = blockIdx.y * 8 * kTensorRows + threadIdx.y;
     if (x >= j.out_w || y0 >= j.out_h) return;
     const int n = imin(4, j.out_w - x);
@@ -271,23 +280,22 @@ extern "C" int b200_export_picture(const B200ExportJob *job, void *stream)
                       [&](auto hbd) { return std::make_tuple(j.ss_hor ? export_rgb_kernel<hbd, 1> : export_rgb_kernel<hbd, 0>, j); });
 }
 
-extern "C" int b200_export_tensor(const B200TensorJob *job, void *stream)
+// every field of one tensor job, checked as it arrives from outside the library: 0, or -2 with the error set
+static int check_tensor_job(const B200TensorJob &j, const char *who)
 {
-    if (!job) { b200_set_error("b200_export_tensor: no job"); return -2; }
-    const B200TensorJob &j = *job;
-    if (int r = check_bdmax(j.bitdepth_max, "b200_export_tensor")) return r;
+    if (int r = check_bdmax(j.bitdepth_max, who)) return r;
     const auto in_range = [](int v, int lo, int hi) { return v >= lo && v <= hi; };
     if (!j.src || !in_range(j.w, 1, 65536) || !in_range(j.h, 1, 65536) || !in_range(j.out_w, 1, 65536) || !in_range(j.out_h, 1, 65536) ||
         !in_range(j.ss_hor, 0, 1) || !in_range(j.ss_ver, 0, 1) || !in_range(j.siting_x, 0, 1) || !in_range(j.siting_y, 0, 1) ||
         !in_range(j.dtype, B200_TENSOR_F32, B200_TENSOR_BF16) || !in_range(j.layout, B200_TENSOR_CHW, B200_TENSOR_HWC)) {
-        b200_set_error("b200_export_tensor: bad arguments (%d x %d -> %d x %d, dtype %d, layout %d)", j.w, j.h, j.out_w, j.out_h,
+        b200_set_error("%s: bad arguments (%d x %d -> %d x %d, dtype %d, layout %d)", who, j.w, j.h, j.out_w, j.out_h,
                        j.dtype, j.layout);
         return -2;
     }
-    if (j.identity && (j.mono || j.ss_hor || j.ss_ver)) { b200_set_error("b200_export_tensor: identity matrix needs 4:4:4"); return -2; }
+    if (j.identity && (j.mono || j.ss_hor || j.ss_ver)) { b200_set_error("%s: identity matrix needs 4:4:4", who); return -2; }
     for (int p = 0; p < (j.mono ? 1 : 3); p++)
         if (j.stride[p] < (p ? (j.w + j.ss_hor) >> j.ss_hor : j.w)) {
-            b200_set_error("b200_export_tensor: stride of plane %d too small", p);
+            b200_set_error("%s: stride of plane %d too small", who, p);
             return -2;
         }
     // the addresses of the last element of every channel must fit int64 with room to spare
@@ -296,16 +304,68 @@ extern "C" int b200_export_tensor(const B200TensorJob *job, void *stream)
     const bool pitch_ok = j.pitch_y >= row && j.pitch_y <= lim / j.out_h;
     if (!j.dst || ((uintptr_t)j.dst % esize) || !pitch_ok ||
         (j.layout == B200_TENSOR_CHW && (j.pitch_c < (j.out_h - 1) * j.pitch_y + row || j.pitch_c > lim / 3))) {
-        b200_set_error("b200_export_tensor: bad destination (pitches %lld, %lld)", (long long)j.pitch_c, (long long)j.pitch_y);
+        b200_set_error("%s: bad destination (pitches %lld, %lld)", who, (long long)j.pitch_c, (long long)j.pitch_y);
         return -2;
     }
-    const int runs = (j.out_w + 3) / 4;
-    const dim3 grid((runs + 31) / 32, (j.out_h + 8 * kTensorRows - 1) / (8 * kTensorRows));
-    return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, (cudaStream_t)stream, [&](auto hbd) {
+    return 0;
+}
+
+// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype and layout
+template <int N>
+static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, cudaStream_t stream)
+{
+    TensorBatch<N> b{};
+    int out_w = 0, out_h = 0;
+    for (int i = 0; i < n; i++) {
+        b.job[i] = *jobs[i];
+        out_w = imax(out_w, jobs[i]->out_w); out_h = imax(out_h, jobs[i]->out_h);
+    }
+    const B200TensorJob &j = b.job[0];
+    const int runs = (out_w + 3) / 4;
+    const dim3 grid((runs + 31) / 32, (out_h + 8 * kTensorRows - 1) / (8 * kTensorRows), n);
+    return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, stream, [&](auto hbd) {
         constexpr bool H = decltype(hbd)::value;
-        void (*const k[3][2])(B200TensorJob) = {{export_tensor_kernel<H, B200_TENSOR_F32, false>, export_tensor_kernel<H, B200_TENSOR_F32, true>},
-                                                {export_tensor_kernel<H, B200_TENSOR_F16, false>, export_tensor_kernel<H, B200_TENSOR_F16, true>},
-                                                {export_tensor_kernel<H, B200_TENSOR_BF16, false>, export_tensor_kernel<H, B200_TENSOR_BF16, true>}};
-        return std::make_tuple(k[j.dtype][j.layout], j);
+        void (*const k[3][2])(TensorBatch<N>) = {
+            {export_tensor_kernel<H, B200_TENSOR_F32, false, N>, export_tensor_kernel<H, B200_TENSOR_F32, true, N>},
+            {export_tensor_kernel<H, B200_TENSOR_F16, false, N>, export_tensor_kernel<H, B200_TENSOR_F16, true, N>},
+            {export_tensor_kernel<H, B200_TENSOR_BF16, false, N>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N>}};
+        return std::make_tuple(k[j.dtype][j.layout], b);
     });
+}
+static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, cudaStream_t stream)
+{
+    return n == 1 ? launch_tensor_jobs<1>(jobs, n, stream) : launch_tensor_jobs<B200_TENSOR_BATCH_MAX>(jobs, n, stream);
+}
+
+extern "C" int b200_export_tensor(const B200TensorJob *job, void *stream)
+{
+    return b200_export_tensor_batch(job, 1, stream);
+}
+
+extern "C" int b200_export_tensor_batch(const B200TensorJob *jobs, int n, void *stream)
+{
+    if (!jobs || n < 1) { b200_set_error("b200_export_tensor_batch: no jobs (%d)", n); return -2; }
+    for (int i = 0; i < n; i++) {
+        if (int r = check_tensor_job(jobs[i], n == 1 ? "b200_export_tensor" : "b200_export_tensor_batch")) return r;
+        if (jobs[i].dtype != jobs[0].dtype || jobs[i].layout != jobs[0].layout) {
+            b200_set_error("b200_export_tensor_batch: job %d has another dtype or layout than job 0", i);
+            return -2;
+        }
+    }
+    // one launch per bit-depth class present and per B200_TENSOR_BATCH_MAX jobs of it, jobs in their order
+    for (int hbd = 0; hbd < 2; hbd++) {
+        const B200TensorJob *part[B200_TENSOR_BATCH_MAX];
+        int m = 0;
+        for (int i = 0; i < n; i++) {
+            if ((jobs[i].bitdepth_max > 255) != hbd) continue;
+            part[m++] = &jobs[i];
+            if (m == B200_TENSOR_BATCH_MAX) {
+                if (int r = launch_tensor_jobs(part, m, (cudaStream_t)stream)) return r;
+                m = 0;
+            }
+        }
+        if (m)
+            if (int r = launch_tensor_jobs(part, m, (cudaStream_t)stream)) return r;
+    }
+    return 0;
 }

@@ -72,8 +72,10 @@ def _profile(bpc, layout):
 
 def sequence_header(w, h, bpc=8, sb128=0, film_grain=0, filter_intra=1, intra_edge_filter=1, cdef=1, restoration=1,
                     inter_intra=1, masked_compound=1, warped_motion=1, screen_content=0, layout="420", super_res=0,
-                    chroma_sample_position=0):
-    """chroma_sample_position (4:2:0 only): enum Dav1dChromaSamplePosition, 0 unknown, 1 vertical, 2 colocated"""
+                    chroma_sample_position=0, color=None):
+    """chroma_sample_position (4:2:0 only): enum Dav1dChromaSamplePosition, 0 unknown, 1 vertical, 2 colocated;
+    color = (matrix_coefficients, color_range): a colour description with BT.709 primaries and transfer (matrix 0, identity,
+    is not supported here); None writes none and limited range"""
     b = BitWriter()
     profile = _profile(bpc, layout)
     b.f(3, profile)
@@ -103,8 +105,11 @@ def sequence_header(w, h, bpc=8, sb128=0, film_grain=0, filter_intra=1, intra_ed
     mono = layout == "400"
     if profile != 1:
         b.f(1, 1 if mono else 0)             # mono_chrome
-    b.f(1, 0)                                # color_description_present
-    b.f(1, 0)                                # color_range
+    b.f(1, color is not None)                # color_description_present
+    if color is not None:
+        assert color[0] != 0, "identity matrix_coefficients need the sRGB special case"
+        b.f(8, 1); b.f(8, 1); b.f(8, color[0])   # color_primaries, transfer_characteristics (BT.709), matrix_coefficients
+    b.f(1, color[1] if color is not None else 0)  # color_range
     if not mono:
         if profile == 2 and bpc == 12:       # explicit subsampling
             b.f(1, 0 if layout == "444" else 1)
@@ -485,16 +490,16 @@ def show_existing_frame(slot):
 
 
 def inter_stream(seed, w, h, n_frames=3, bpc=8, sb128=0, log2_cols=0, log2_rows=0, motion_modes=0, film_grain=0, screen_content=0, layout="420",
-                 hidden_every=0, intra_only_every=0, sizes=None, super_res=0, chroma_sample_position=0, **kw):
+                 hidden_every=0, intra_only_every=0, sizes=None, super_res=0, chroma_sample_position=0, color=None, **kw):
     """Temporal units: one key frame, then n_frames - 1 inter frames (single and compound references incl. wedge /
     difference-weighted masks and distance weights, switchable interpolation filters, variable transform trees, intra
     blocks; identity global motion). motion_modes=1 additionally enables the per-block motion mode (overlapped block
     motion compensation, locally warped motion), motion_modes=2 inter-intra prediction as well. hidden_every=k makes
     every k-th inter frame a hidden future frame (decoded early, referenced with backward prediction, output later by a
-    show_existing_frame header)."""
+    show_existing_frame header). color: the sequence header's colour description (sequence_header)."""
     rng = np.random.default_rng(seed)
     seq = sequence_header(w, h, bpc=bpc, sb128=sb128, inter_intra=1 if motion_modes >= 2 else 0, warped_motion=1 if motion_modes else 0, film_grain=film_grain, screen_content=screen_content, layout=layout, super_res=super_res,
-                          chroma_sample_position=chroma_sample_position)
+                          chroma_sample_position=chroma_sample_position, color=color)
     kw = dict(kw, layout=layout)
     if super_res:                            # every frame may then be coded narrower and upscaled; its references keep their upscaled size
         kw = dict(kw, super_res=1)

@@ -6,6 +6,8 @@ oracle/_ref/ is used). This module binds its stream driver (dav1d's public API: 
 and points the hooks at dav1d_b200/libb200av1.so. No CPU fallback: without the CUDA library the decode fails."""
 import ctypes as C
 import os
+import queue
+import threading
 
 import numpy as np
 
@@ -45,7 +47,8 @@ class HookStats(C.Structure):
     _fields_ = [("frames", C.c_uint64), ("records", C.c_uint64), ("coefs", C.c_uint64), ("h2d_bytes", C.c_uint64),
                 ("d2h_bytes", C.c_uint64), ("device_ms", C.c_double), ("intra_tx", C.c_uint64), ("pred", C.c_uint64),
                 ("comp", C.c_uint64), ("warp", C.c_uint64), ("blend", C.c_uint64), ("itx", C.c_uint64),
-                ("inter_frames", C.c_uint64), ("host_prep_ms", C.c_double), ("interintra", C.c_uint64), ("palette_bytes", C.c_uint64), ("ibc", C.c_uint64), ("scaled", C.c_uint64)]
+                ("inter_frames", C.c_uint64), ("host_prep_ms", C.c_double), ("interintra", C.c_uint64), ("palette_bytes", C.c_uint64), ("ibc", C.c_uint64), ("scaled", C.c_uint64),
+                ("ref_table", C.c_uint64), ("frame_table", C.c_uint64)]
 
 
 def build_hooked(verbose=False):
@@ -248,6 +251,7 @@ class DeviceDecoder:
             ...
         for rgb in dec.pictures(tus, format="rgb"):             # [3, h, w], same dtype rule, stream bit depth
         for x in dec.tensors(tus, size=(224, 224), dtype="bfloat16", batch=8):   # [n, 3, 224, 224] model input
+        x = dec.clips([tus_0, tus_1, ...], frames=16, step=2, size=(224, 224))  # [N, 16, 3, 224, 224] clip batch
 
     `backend` = path of the C-ABI library the hooks bind (default: the CUDA library); `serialize` = one device job at a time
     (for back ends that are not re-entrant, like the host emulator)."""
@@ -269,6 +273,7 @@ class DeviceDecoder:
         d.b200hook_set_device_only.argtypes = [C.c_void_p, C.c_int]
         d.b200hook_export_picture.argtypes = [C.c_void_p, C.POINTER(ExportJob), C.c_void_p]
         d.b200hook_export_tensor.argtypes = [C.c_void_p, C.POINTER(TensorJob), C.c_void_p]
+        d.b200hook_export_tensor_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         d.refdrv_stream_chroma_position.argtypes = [C.c_void_p]
 
     def stats(self, reset=False):
@@ -349,6 +354,131 @@ class DeviceDecoder:
         if state["buf"] is not None:
             yield state["buf"][:state["n"]]
 
+    def clips(self, streams, frames, step=1, start=0, size=None, dtype="float32", layout="chw", mean=None, std=None,
+              matrix="auto", full_range=None, chroma_siting="auto", workers=None, alloc=None, stream=None):
+        """Decodes N streams (each a list of temporal units) concurrently and returns one clip per stream as a
+        [N, frames, 3, OH, OW] tensor (layout="hwc": [N, frames, OH, OW, 3]): x[i, t] is output picture
+        start_i + t * step of stream i, exported exactly as tensors() exports it. `start` is one int or one per stream.
+        size=None needs every sampled picture to have the same size. The tensor options, alloc and stream mean what they
+        mean in tensors(); "auto" matrix, range and siting are resolved per stream from its own headers.
+        Each stream has a dav1d context of its own (this decoder's n_threads / max_frame_delay) driven by a host thread of
+        its own; at most `workers` streams are open at once (default min(N, CLIP_WORKERS), at most CLIP_MAX_WORKERS).
+        Pictures that are not sampled are released unexported, and a stream is closed once its last sampled picture is
+        exported. The calling thread exports every sampled picture that is waiting with one batched kernel launch
+        (b200_export_tensor_batch) straight into its slot of the result. ValueError when a stream has too few pictures (it
+        names the stream); a dav1d error in any stream stops the others and is raised here; no thread outlives the call."""
+        streams = list(streams)
+        n = len(streams)
+        frames, step = int(frames), int(step)
+        starts = [int(start)] * n if isinstance(start, (int, np.integer)) else [int(v) for v in start]
+        workers = min(n, CLIP_WORKERS) if workers is None else int(workers)
+        if n < 1 or frames < 1 or step < 1 or len(starts) != n or min(starts) < 0:
+            raise ValueError("clips needs >= 1 stream, frames >= 1, step >= 1 and one start >= 0 per stream")
+        if not 1 <= workers <= CLIP_MAX_WORKERS:
+            raise ValueError("workers must be 1 .. %d" % CLIP_MAX_WORKERS)
+        if dtype not in TENSOR_DTYPES or layout not in TENSOR_LAYOUTS:
+            raise ValueError("dtype must be one of %s, layout 'chw' or 'hwc'" % ", ".join(TENSOR_DTYPES))
+        if matrix != "auto" and matrix != "identity" and matrix not in MATRICES:
+            raise ValueError("unknown matrix %r" % (matrix,))
+        if chroma_siting != "auto" and chroma_siting not in SITINGS:
+            raise ValueError("unknown chroma siting %r" % (chroma_siting,))
+        if size is not None:
+            size = tuple(int(v) for v in size)
+            if len(size) != 2 or not all(1 <= v <= 65536 for v in size):
+                raise ValueError("size must be (height, width), each 1 .. 65536")
+        tensor_scale_bias(8, mean, std)                          # checks mean / std
+        alloc, stream = _default_alloc(alloc, stream)
+        self._hooked._bind()
+        esize = 4 if dtype == "float32" else 2
+        todo = queue.Queue()                     # stream indices not started yet
+        for i in range(n):
+            todo.put(i)
+        ready = queue.Queue()                    # (stream, t, handle, info, event) of a held sampled picture, or an error
+        stop = threading.Event()
+        threads = [threading.Thread(target=self._clip_worker, args=(streams, starts, frames, step, todo, ready, stop), daemon=True)
+                   for _ in range(workers)]
+        out, hw, left = None, None, n * frames
+        try:
+            for t in threads:
+                t.start()
+            while left:
+                items = [ready.get()]
+                while True:
+                    try:
+                        items.append(ready.get_nowait())
+                    except queue.Empty:
+                        break
+                try:
+                    errors = [it for it in items if isinstance(it, BaseException)]
+                    if errors:
+                        raise errors[0]
+                    jobs = (TensorJob * len(items))()
+                    pics = (C.c_void_p * len(items))()
+                    for k, (i, t, h, info, _) in enumerate(items):
+                        oh, ow = size or (int(info[1]), int(info[0]))
+                        if out is None:
+                            hw = (oh, ow)
+                            out = alloc((n, frames) + ((3, oh, ow) if layout == "chw" else (oh, ow, 3)), dtype)
+                        elif (oh, ow) != hw:
+                            raise ValueError("stream %d picture %d is %dx%d, not %dx%d like the others: pass size= for "
+                                             "pictures of different sizes" % (i, starts[i] + t * step, ow, oh, hw[1], hw[0]))
+                        dst = _data_ptr(out) + (i * frames + t) * 3 * oh * ow * esize
+                        jobs[k] = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting)
+                        pics[k] = self.dll.refdrv_stream_picture(h)
+                    if self.dll.b200hook_export_tensor_batch(pics, jobs, len(items), C.c_void_p(stream)) != 0:
+                        raise RuntimeError("exporting pictures failed (see stderr)")
+                    left -= len(items)
+                finally:
+                    for it in items:                 # the pictures go back to their workers: enqueued, or abandoned
+                        if not isinstance(it, BaseException):
+                            it[4].set()
+        finally:
+            stop.set()
+            while any(t.is_alive() for t in threads):
+                try:                                 # workers blocked on a handed-over picture are let go
+                    it = ready.get(timeout=0.01)
+                    if not isinstance(it, BaseException):
+                        it[4].set()
+                except queue.Empty:
+                    pass
+            for t in threads:
+                t.join()
+        return out
+
+    def _clip_worker(self, streams, starts, frames, step, todo, ready, stop):
+        """one host thread of clips(): decodes streams taken from `todo` one after the other, hands each sampled picture
+        to the calling thread and waits until its export has been enqueued; errors go to `ready` and stop the others"""
+        try:
+            while not stop.is_set():
+                try:
+                    i = todo.get_nowait()
+                except queue.Empty:
+                    return
+                want = {starts[i] + t * step: t for t in range(frames)}
+                last, k = max(want), 0
+
+                def take(h, info):
+                    nonlocal k
+                    t = want.get(k)
+                    k += 1
+                    if t is not None and not stop.is_set():
+                        done = threading.Event()
+                        ready.put((i, t, h, info.copy(), done))
+                        done.wait()
+                    return k > last or stop.is_set()          # True: the stream's last sampled picture is out
+
+                try:
+                    for finished in self._decode(streams[i], take):
+                        if finished:
+                            break
+                except RuntimeError as e:
+                    raise RuntimeError("stream %d: %s" % (i, e)) from None
+                if k <= last and not stop.is_set():
+                    raise ValueError("stream %d has %d pictures; the clip needs picture %d" % (i, k, last))
+        except BaseException as e:                          # noqa: B036  (handed to the calling thread)
+            stop.set()
+            ready.put(e)
+
     def _decode(self, tus, export):
         """the decode loop of pictures() and tensors(): export(h, info) runs for every output picture while the stream
         holds it (info = w, h, bpc, layout, matrix_coefficients, color_range), and what it returns is yielded"""
@@ -397,6 +527,13 @@ class DeviceDecoder:
         return name
 
     def _export_tensor(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, stream):
+        job = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting)
+        if self.dll.b200hook_export_tensor(self.dll.refdrv_stream_picture(h), C.byref(job), C.c_void_p(stream)) != 0:
+            raise RuntimeError("exporting a picture failed (see stderr)")
+
+    def _tensor_job(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting):
+        """the B200TensorJob of the picture stream h holds (info as _decode gives it): "auto" matrix, range and siting come
+        from that stream's own headers"""
         w, hh, bpc, pl, mtrx, color_range = (int(v) for v in info)
         job = TensorJob()
         job.out_w, job.out_h, job.dtype, job.layout = ow, oh, TENSOR_DTYPES[dtype], TENSOR_LAYOUTS[layout]
@@ -413,8 +550,7 @@ class DeviceDecoder:
             job.scale[c], job.bias[c] = float(scale[c]), float(bias[c])
         job.dst = dst
         job.pitch_y, job.pitch_c = (ow, oh * ow) if layout == "chw" else (3 * ow, 1)
-        if self.dll.b200hook_export_tensor(self.dll.refdrv_stream_picture(h), C.byref(job), C.c_void_p(stream)) != 0:
-            raise RuntimeError("exporting a picture failed (see stderr)")
+        return job
 
     def _export(self, h, info, format, matrix, full_range, alloc, stream):
         w, hh, bpc, layout, mtrx, color_range = (int(v) for v in info)
@@ -442,6 +578,11 @@ class DeviceDecoder:
 
 
 _EAGAIN = -11
+# clips(): streams decoded at once by default and at most. Each open stream is a device-output dav1d context (the hooks
+# register up to 64) holding up to 8 reference pictures + its frames in flight + its output in the hooks' pool of 1024
+# page-locked pictures.
+CLIP_WORKERS = 4
+CLIP_MAX_WORKERS = 32
 
 
 def _default_alloc(alloc, stream):

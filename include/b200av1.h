@@ -823,6 +823,15 @@ typedef struct B200TensorJob {
     int64_t pitch_c, pitch_y;      /* elements */
 } B200TensorJob;
 B200_API int b200_export_tensor(const B200TensorJob *job, void *stream);
+/* n >= 1 tensor jobs at once, e.g. the pictures of a clip batch taken from several streams: each job is exactly what
+ * b200_export_tensor(&jobs[i]) writes, with its own source, geometry, bit depth, matrix, range, siting, scale / bias and
+ * destination, but all jobs must share dtype and layout. The destinations must not overlap each other (jobs run in no
+ * particular order). One launch on `stream` per bit-depth class present (8 bit, above 8 bit) and per
+ * B200_TENSOR_BATCH_MAX jobs of it; the jobs ride in the kernel's parameter block. -2 when jobs is NULL, n < 1, dtype or
+ * layout differ, or any job is bad (checked as b200_export_tensor checks it): then nothing is launched. b200_export_tensor
+ * is the n = 1 case. */
+#define B200_TENSOR_BATCH_MAX 24
+B200_API int b200_export_tensor_batch(const B200TensorJob *jobs, int n, void *stream);
 
 #ifdef __cplusplus
 }

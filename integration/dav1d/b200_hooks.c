@@ -45,9 +45,27 @@ API int dav1d_open(Dav1dContext **const c_out, const Dav1dSettings *const s)
 static B200Backend g_be;
 static int g_be_ok;
 static pthread_mutex_t g_lock = PTHREAD_MUTEX_INITIALIZER;
-static HookFrame g_frames[64];
 static B200HookStats g_stats;
 static uint64_t g_clock;            /* LRU stamps of the frame-context and picture tables */
+
+/* The frame-context and device-picture tables grow in chunks of TABLE_CHUNK entries that never move: hooks keep
+ * HookFrame * / HookRefPic * pointers across calls. Entry i is table_at(chunks, i); n = entries in use (a multiple of
+ * TABLE_CHUNK). Grown under g_lock. */
+#define TABLE_CHUNK 64
+#define TABLE_MAX_CHUNKS 64
+static HookFrame *g_frame_chunks[TABLE_MAX_CHUNKS];
+static HookRefPic *g_ref_chunks[TABLE_MAX_CHUNKS];
+static int g_n_frames, g_n_refs;
+#define FRAME_AT(i) (&g_frame_chunks[(i) / TABLE_CHUNK][(i) % TABLE_CHUNK])
+#define REF_AT(i) (&g_ref_chunks[(i) / TABLE_CHUNK][(i) % TABLE_CHUNK])
+/* one more zeroed chunk: its first entry, NULL when out of memory or at TABLE_MAX_CHUNKS */
+static void *table_grow(void **chunks, int *n, size_t elem)
+{
+    if (*n >= TABLE_CHUNK * TABLE_MAX_CHUNKS) return NULL;
+    void *const c = calloc(TABLE_CHUNK, elem);
+    if (c) { chunks[*n / TABLE_CHUNK] = c; *n += TABLE_CHUNK; }
+    return c;
+}
 
 API int b200hook_set_backend(const char *path)
 {
@@ -70,7 +88,8 @@ API int b200hook_set_backend(const char *path)
     SYM(event_create, "b200_event_create"); SYM(event_destroy, "b200_event_destroy");
     SYM(event_record, "b200_event_record"); SYM(stream_wait_event, "b200_stream_wait_event");
     SYM(struct_size, "b200_struct_size");
-    SYM(event_sync, "b200_event_sync"); SYM(export_picture, "b200_export_picture"); SYM(export_tensor, "b200_export_tensor");
+    SYM(event_sync, "b200_event_sync"); SYM(export_picture, "b200_export_picture");
+    SYM(export_tensor_batch, "b200_export_tensor_batch");
 #undef SYM
     /* binding self-check: the structs this file was compiled with are the ones the library was compiled with */
     if (be.struct_size(9) != (int)sizeof(B200FrameJob) || be.struct_size(14) != (int)sizeof(B200IntraTx) ||
@@ -162,6 +181,16 @@ static void pinned_pic_release(Dav1dPicture *const p, void *const cookie)
     pthread_mutex_lock(&g_pin_lock);
     g_pin_pool[slot].used = 0;
     pthread_mutex_unlock(&g_pin_lock);
+}
+/* whether key is the data[0] of a page-locked picture dav1d still holds: its device copy must not be recycled, because
+ * the picture comes back to b200hook_refpic_forget when dav1d releases it (called under g_lock; g_pin_lock nests inside) */
+static int pinned_pic_live(const void *const key)
+{
+    int live = 0;
+    pthread_mutex_lock(&g_pin_lock);
+    for (int i = 0; i < PIN_POOL && !live; i++) live = g_pin_pool[i].used && g_pin_pool[i].ptr == key;
+    pthread_mutex_unlock(&g_pin_lock);
+    return live;
 }
 static void pinned_pool_trim(void)
 {
@@ -260,7 +289,6 @@ int b200hook_tiles_gather(HookFrame *const hf, const int list, HookBuf *const ds
     return (int)total;
 }
 
-static HookRefPic g_refs[64];
 static pthread_cond_t g_ref_cond = PTHREAD_COND_INITIALIZER;
 HookRefPic *b200hook_refpic(const void *key, size_t bytes, int create)
 {
@@ -268,25 +296,29 @@ HookRefPic *b200hook_refpic(const void *key, size_t bytes, int create)
     HookRefPic *r = NULL;
     if (!be || !key) return NULL;
     pthread_mutex_lock(&g_lock);
-    for (int i = 0; i < 64 && !r; i++)
-        if (g_refs[i].key == key) r = &g_refs[i];
+    for (int i = 0; i < g_n_refs && !r; i++)
+        if (REF_AT(i)->key == key) r = REF_AT(i);
     if (!r && create) {
         /* a free entry: one whose device buffer is already large enough if there is one (the buffer and event of a forgotten
          * picture stay with its entry) */
-        for (int i = 0; i < 64; i++)
-            if (!g_refs[i].key && (!r || (r->bytes < bytes && g_refs[i].bytes >= bytes))) r = &g_refs[i];
-        if (r) { r->key = key; r->ready = 0; r->submitted = 0; }
+        for (int i = 0; i < g_n_refs; i++)
+            if (!REF_AT(i)->key && (!r || (r->bytes < bytes && REF_AT(i)->bytes >= bytes))) r = REF_AT(i);
         if (!r) {
-            /* host pictures of closed decoders never come back: recycle the least recently used entry (the live set —
-             * 8 reference slots + frames in flight + pictures waiting for output — is far smaller than the table) */
-            for (int i = 0; i < 64; i++)
-                if (g_refs[i].ready && (!r || g_refs[i].last_use < r->last_use)) r = &g_refs[i];
+            /* Pictures from a caller's own allocator, or of decoders that were closed, never come back through
+             * b200hook_refpic_forget: recycle the least recently used such entry (with one decoder the live set — 8 reference
+             * slots + frames in flight + pictures waiting for output — is far smaller than a chunk). An entry keyed by a
+             * page-locked picture dav1d still holds (`pool`) is live and never recycled: the table grows instead, so any
+             * number of decoders may run at once. */
+            for (int i = 0; i < g_n_refs; i++)
+                if (!REF_AT(i)->pool && REF_AT(i)->ready && (!r || REF_AT(i)->last_use < r->last_use)) r = REF_AT(i);
             if (!r)                              /* only pictures of abandoned frames (never completed) are left: oldest one */
-                for (int i = 0; i < 64; i++)
-                    if (!r || g_refs[i].last_use < r->last_use) r = &g_refs[i];
-            if (r->exported) be->event_sync(r->export_event);
-            r->key = key; r->ready = 0; r->submitted = 0; r->exported = 0;
+                for (int i = 0; i < g_n_refs; i++)
+                    if (!REF_AT(i)->pool && (!r || REF_AT(i)->last_use < r->last_use)) r = REF_AT(i);
+            if (r && r->exported) be->event_sync(r->export_event);
+            if (!r) r = table_grow((void **)g_ref_chunks, &g_n_refs, sizeof(HookRefPic));
+            if (!r) fprintf(stderr, "b200hook: device-picture table full\n");
         }
+        if (r) { r->key = key; r->ready = 0; r->submitted = 0; r->exported = 0; r->pool = pinned_pic_live(key); }
     }
     if (r && create && !r->event) r->event = be->event_create();      /* NULL = no events: consumers then wait for `ready` on the host */
     if (r) r->last_use = ++g_clock;
@@ -306,32 +338,46 @@ void b200hook_refpic_forget(const void *const key)
      * keeps its key until then, so nobody takes it over */
     void *export_done = NULL;
     pthread_mutex_lock(&g_lock);
-    for (int i = 0; i < 64; i++)
-        if (g_refs[i].key == key && g_refs[i].exported) export_done = g_refs[i].export_event;
+    for (int i = 0; i < g_n_refs; i++)
+        if (REF_AT(i)->key == key && REF_AT(i)->exported) export_done = REF_AT(i)->export_event;
     pthread_mutex_unlock(&g_lock);
     if (export_done) g_be.event_sync(export_done);
     pthread_mutex_lock(&g_lock);
-    for (int i = 0; i < 64; i++)
-        if (g_refs[i].key == key) { g_refs[i].key = NULL; g_refs[i].ready = 0; g_refs[i].submitted = 0; g_refs[i].exported = 0; }
+    for (int i = 0; i < g_n_refs; i++) {
+        HookRefPic *const r = REF_AT(i);
+        if (r->key == key) { r->key = NULL; r->ready = 0; r->submitted = 0; r->exported = 0; r->pool = 0; }
+    }
     pthread_mutex_unlock(&g_lock);
 }
 
-int b200hook_export_submit(HookRefPic *const r, const int tensor, const void *const job, void *const stream)
+int b200hook_export_submit(HookRefPic *const *const r, const int n, const int tensor, const void *const jobs, void *const stream)
 {
     const B200Backend *const be = b200hook_backend();
     if (!be) return -1;
+    int events = 1;
     pthread_mutex_lock(&g_lock);
-    if (!r->export_event) r->export_event = be->event_create();
-    void *const done = r->export_event;
+    for (int i = 0; i < n; i++) {
+        if (!r[i]->export_event) r[i]->export_event = be->event_create();
+        events &= r[i]->export_event != NULL;
+    }
     pthread_mutex_unlock(&g_lock);
     b200hook_job_enter();
-    int rc = r->event ? be->stream_wait_event(stream, r->event) : 0;
-    if (!rc) rc = tensor ? be->export_tensor(job, stream) : be->export_picture(job, stream);
-    if (!rc) rc = done ? be->event_record(done, stream) : be->frame_wait(stream);      /* no event: the export completes here */
+    int rc = 0;
+    for (int i = 0; i < n && !rc; i++) {
+        int seen = 0;                             /* one wait per distinct picture job */
+        for (int k = 0; k < i && !seen; k++) seen = r[k]->event == r[i]->event;
+        if (r[i]->event && !seen) rc = be->stream_wait_event(stream, r[i]->event);
+    }
+    if (!rc) rc = tensor ? be->export_tensor_batch(jobs, n, stream) : be->export_picture(jobs, stream);
+    /* a batch that failed part way may have enqueued launches that still read the pictures: they complete here, because no
+     * export-done event is recorded for them */
+    if (rc) be->frame_wait(stream);
+    for (int i = 0; i < n && !rc && events; i++) rc = be->event_record(r[i]->export_event, stream);
+    if (!rc && !events) rc = be->frame_wait(stream);          /* no events: the export completes here */
     b200hook_job_leave();
     if (rc) { fprintf(stderr, "b200hook: export failed (%d): %s\n", rc, be->last_error()); return rc; }
     pthread_mutex_lock(&g_lock);
-    r->exported = done != NULL;
+    for (int i = 0; i < n; i++) r[i]->exported = events;
     pthread_mutex_unlock(&g_lock);
     return 0;
 }
@@ -369,14 +415,33 @@ API int b200hook_export_picture(const Dav1dPicture *const p, const B200ExportJob
     if (!p || !tmpl || !p->data[0]) return -1;
     return p->p.bpc > 8 ? b200hook_export_picture_16bpc(p, tmpl, stream) : b200hook_export_picture_8bpc(p, tmpl, stream);
 }
-int b200hook_export_tensor_8bpc(const Dav1dPicture *p, const B200TensorJob *tmpl, void *stream);
-int b200hook_export_tensor_16bpc(const Dav1dPicture *p, const B200TensorJob *tmpl, void *stream);
-/* The same for the tensor export: `tmpl` carries the output size, dtype, layout, siting, matrix, scale / bias and the
- * destination; the source geometry is the picture's own. */
+HookRefPic *b200hook_tensor_source_8bpc(const Dav1dPicture *p, B200TensorJob *j);
+HookRefPic *b200hook_tensor_source_16bpc(const Dav1dPicture *p, B200TensorJob *j);
+/* The same for the tensor export, for n pictures at once (one kernel launch per bit-depth class, include/b200av1.h
+ * b200_export_tensor_batch): `tmpls[i]` carries picture i's output size, dtype, layout, siting, matrix, scale / bias and
+ * destination; the source geometry is the picture's own. The stream waits once for each picture's job, and every picture's
+ * export-done event is recorded behind the launch, so each entry keeps its device buffer until its export has completed. */
+API int b200hook_export_tensor_batch(const Dav1dPicture *const *const pics, const B200TensorJob *const tmpls, const int n,
+                                     void *const stream)
+{
+    if (!pics || !tmpls || n < 1) return -1;
+    B200TensorJob *const jobs = malloc((size_t)n * sizeof(*jobs));
+    HookRefPic **const refs = malloc((size_t)n * sizeof(*refs));
+    int rc = jobs && refs ? 0 : -1;
+    for (int i = 0; i < n && !rc; i++) {
+        const Dav1dPicture *const p = pics[i];
+        if (!p || !p->data[0]) { rc = -1; break; }
+        jobs[i] = tmpls[i];
+        refs[i] = p->p.bpc > 8 ? b200hook_tensor_source_16bpc(p, &jobs[i]) : b200hook_tensor_source_8bpc(p, &jobs[i]);
+        if (!refs[i]) rc = -1;
+    }
+    if (!rc) rc = b200hook_export_submit(refs, n, 1, jobs, stream);
+    free(jobs); free(refs);
+    return rc;
+}
 API int b200hook_export_tensor(const Dav1dPicture *const p, const B200TensorJob *const tmpl, void *const stream)
 {
-    if (!p || !tmpl || !p->data[0]) return -1;
-    return p->p.bpc > 8 ? b200hook_export_tensor_16bpc(p, tmpl, stream) : b200hook_export_tensor_8bpc(p, tmpl, stream);
+    return b200hook_export_tensor_batch(&p, tmpl, 1, stream);
 }
 void b200hook_refpic_set_ready(HookRefPic *r, int ready)
 {
@@ -449,36 +514,36 @@ HookFrame *b200hook_frame(const void *key)
         if (tl_epoch == g_epoch && tl_slot->users > 0) tl_slot->users--;
         tl_slot = NULL; tl_key = NULL; pthread_setspecific(g_tls_key, NULL);
     }
-    for (int i = 0; i < 64 && !r; i++)
-        if (g_frames[i].key == key) r = &g_frames[i];
-    for (int i = 0; i < 64 && !r; i++)
-        if (!g_frames[i].key) {
-            r = &g_frames[i];
-            memset(r, 0, sizeof(*r));
-            pthread_mutex_init(&r->lock, NULL);
-            r->key = key;
+    for (int i = 0; i < g_n_frames && !r; i++)
+        if (FRAME_AT(i)->key == key) r = FRAME_AT(i);
+    for (int i = 0; i < g_n_frames && !r; i++)
+        if (!FRAME_AT(i)->key) r = FRAME_AT(i);
+    /* every slot has a key: take over the least recently used idle one (with its buffers). A slot whose lock is held (its
+     * job or its exit handler is running) is skipped. Invariant: a slot that is started, has a pending job or is cached by
+     * a thread belongs to a frame dav1d has not ended yet, and is never handed to another key: dav1d ends every frame it
+     * starts through b200hook_decode_frame_exit (completed, failed, or flushed by dav1d_flush / dav1d_close), which
+     * returns the slot to idle. With no idle slot the table grows instead. */
+    uint64_t floor_use = 0;
+    for (int tries = 0; tries < g_n_frames && !r; tries++) {
+        for (int i = 0; i < g_n_frames; i++) {
+            HookFrame *const h = FRAME_AT(i);
+            if (h->pinned || h->users || h->pending || h->started || h->tile_sbrows_done || h->last_use <= floor_use) continue;
+            if (!lru || h->last_use < lru->last_use) lru = h;
         }
-    /* table full: take over the least recently used slot — idle ones first (pass 0), then leftovers of decoders that were
-     * closed in the middle of a frame (pass 1: live contexts are looked up all the time, so an old busy-looking slot is dead).
-     * A slot whose lock is held (its job or its exit handler is running) is skipped. */
-    for (int pass = 0; pass < 2 && !r; pass++) {
-        uint64_t floor_use = 0;
-        for (int tries = 0; tries < 64 && !r; tries++) {
-            for (int i = 0; i < 64; i++) {
-                HookFrame *const h = &g_frames[i];
-                if (h->pinned || h->users || h->pending || h->last_use <= floor_use) continue;      /* pending: its job still uses the buffers */
-                if (!pass && (h->started || h->tile_sbrows_done)) continue;
-                if (!lru || h->last_use < lru->last_use) lru = h;
-            }
-            if (!lru) break;
-            if (pthread_mutex_trylock(&lru->lock) == 0) {
-                lru->started = 0; lru->tile_sbrows_done = 0; lru->cur_pic = NULL;
-                lru->key = key; lru->unsupported = 0; r = lru;
-                pthread_mutex_unlock(&lru->lock);
-            } else {
-                floor_use = lru->last_use; lru = NULL;          /* busy right now: next oldest */
-            }
+        if (!lru) break;
+        if (pthread_mutex_trylock(&lru->lock) == 0) {
+            lru->started = 0; lru->tile_sbrows_done = 0; lru->cur_pic = NULL;
+            lru->key = key; lru->unsupported = 0; r = lru;
+            pthread_mutex_unlock(&lru->lock);
+        } else {
+            floor_use = lru->last_use; lru = NULL;          /* busy right now: next oldest */
         }
+    }
+    if (!r) r = table_grow((void **)g_frame_chunks, &g_n_frames, sizeof(HookFrame));
+    if (r && !r->key) {
+        memset(r, 0, sizeof(*r));
+        pthread_mutex_init(&r->lock, NULL);
+        r->key = key;
     }
     if (!r) fprintf(stderr, "b200hook: no frame-context slot available\n");
     if (r) { r->last_use = ++g_clock; r->users++; r->epoch = g_epoch; pthread_setspecific(g_tls_key, r); }
@@ -588,8 +653,8 @@ void b200hook_decode_frame_exit(struct Dav1dFrameContext *const f, int retval)
 {
     HookFrame *h = NULL;
     pthread_mutex_lock(&g_lock);
-    for (int i = 0; i < 64 && !h; i++)
-        if (g_frames[i].key == (const void *)f) h = &g_frames[i];
+    for (int i = 0; i < g_n_frames && !h; i++)
+        if (FRAME_AT(i)->key == (const void *)f) h = FRAME_AT(i);
     pthread_mutex_unlock(&g_lock);
     if (h) {
         pthread_mutex_lock(&h->lock);
@@ -622,6 +687,7 @@ API void b200hook_get_stats(B200HookStats *out, int reset)
 {
     pthread_mutex_lock(&g_lock);
     *out = g_stats;
+    out->ref_table = (uint64_t)g_n_refs; out->frame_table = (uint64_t)g_n_frames;
     if (reset) memset(&g_stats, 0, sizeof(g_stats));
     pthread_mutex_unlock(&g_lock);
 }
@@ -631,8 +697,10 @@ API void b200hook_release(void)
 {
     pthread_mutex_lock(&g_lock);
     __atomic_add_fetch(&g_epoch, 1, __ATOMIC_RELEASE);
-    for (int i = 0; i < 64; i++) {
-        HookFrame *h = &g_frames[i];
+    /* the frame-context chunks stay allocated: threads' cached slot pointers (released by their exit handlers) point into
+     * them; every slot's buffers are freed and the slot returns to unused */
+    for (int i = 0; i < g_n_frames; i++) {
+        HookFrame *h = FRAME_AT(i);
         if (!h->key) continue;
         if (h->pending && h->stream && g_be_ok) g_be.frame_wait(h->stream);       /* nothing may still read the buffers below */
         b200hook_buf_free(&h->tx); b200hook_buf_free(&h->tx_sorted); b200hook_buf_free(&h->coef); b200hook_buf_free(&h->mask);
@@ -652,13 +720,15 @@ API void b200hook_release(void)
         pthread_mutex_destroy(&h->lock);
         memset(h, 0, sizeof(*h));
     }
-    for (int i = 0; i < 64; i++) {
-        if (g_refs[i].exported && g_be_ok) g_be.event_sync(g_refs[i].export_event);
-        if (g_refs[i].dev && g_be_ok) g_be.dev_free(g_refs[i].dev);
-        if (g_refs[i].event && g_be_ok) g_be.event_destroy(g_refs[i].event);
-        if (g_refs[i].export_event && g_be_ok) g_be.event_destroy(g_refs[i].export_event);
-        memset(&g_refs[i], 0, sizeof(g_refs[i]));
+    for (int i = 0; i < g_n_refs; i++) {
+        HookRefPic *const r = REF_AT(i);
+        if (r->exported && g_be_ok) g_be.event_sync(r->export_event);
+        if (r->dev && g_be_ok) g_be.dev_free(r->dev);
+        if (r->event && g_be_ok) g_be.event_destroy(r->event);
+        if (r->export_event && g_be_ok) g_be.event_destroy(r->export_event);
     }
+    for (int c = 0; c < g_n_refs / TABLE_CHUNK; c++) { free(g_ref_chunks[c]); g_ref_chunks[c] = NULL; }
+    g_n_refs = 0;
     pthread_mutex_unlock(&g_lock);
     pinned_pool_trim();
 }

@@ -36,7 +36,7 @@ typedef struct B200Backend {
     int (*struct_size)(int);
     int (*event_sync)(void *);
     int (*export_picture)(const B200ExportJob *, void *);
-    int (*export_tensor)(const B200TensorJob *, void *);
+    int (*export_tensor_batch)(const B200TensorJob *, int, void *);
 } B200Backend;
 const B200Backend *b200hook_backend(void);   /* NULL (after logging) when no back end is loaded: the decode fails */
 
@@ -134,12 +134,15 @@ static inline void *b200hook_tile_append(HookFrame *const hf, const int tile, co
  * and the copy into the host picture are complete */
 /* exported: an export into caller memory was enqueued and `export_event` marks its end — the entry's device buffer is not
  * handed to another picture before that event has completed */
+/* pool: the key is a page-locked picture of the hooks' pool (b200_hooks.c) that dav1d held when the entry was made: the
+ * entry is freed by b200hook_refpic_forget when dav1d releases the picture and is never recycled before */
 typedef struct HookRefPic { const void *key; void *dev; size_t bytes; int ready, submitted; void *event; uint64_t last_use;
-                            void *export_event; int exported; } HookRefPic;
+                            void *export_event; int exported, pool; } HookRefPic;
 HookRefPic *b200hook_refpic(const void *key, size_t bytes, int create);
-/* enqueues the export of a resident picture on `stream` behind the picture's own job, and records its export-done event:
- * `job` is a B200ExportJob (b200_export_picture) or, with `tensor` set, a B200TensorJob (b200_export_tensor) */
-int b200hook_export_submit(HookRefPic *r, int tensor, const void *job, void *stream);
+/* enqueues the export of n resident pictures r[0..n) on `stream` behind their own jobs (one wait per distinct job), and
+ * records each entry's export-done event behind it: `jobs` is one B200ExportJob (b200_export_picture, n = 1) or, with
+ * `tensor` set, n B200TensorJobs (one b200_export_tensor_batch call) */
+int b200hook_export_submit(HookRefPic *const *r, int n, int tensor, const void *jobs, void *stream);
 /* a decoder context (Dav1dContext *) opened for device output: its frame jobs and film grain leave the pictures in device
  * memory and copy nothing back into the host pictures */
 int b200hook_device_only(const void *ctx);
@@ -160,6 +163,8 @@ typedef struct B200HookStats {
     uint64_t palette_bytes;         /* palettes + index maps shipped for palette blocks */
     uint64_t ibc;                   /* intra block copy records (a subset of intra_tx) */
     uint64_t scaled;                /* predictions from references of another size */
+    uint64_t ref_table, frame_table; /* entries the device-picture / frame-context tables hold now (chunks of 64; not reset,
+                                        the device-picture table returns to 0 in b200hook_release) */
 } B200HookStats;
 void b200hook_account(uint64_t records, uint64_t coefs, uint64_t h2d, uint64_t d2h, double ms, const uint64_t kinds[11], double prep_ms);
 

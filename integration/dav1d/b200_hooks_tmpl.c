@@ -1238,7 +1238,7 @@ void bitfn(b200hook_apply_grain_row)(const Dav1dFilmGrainDSPContext *const dsp, 
     (void)dsp; (void)out; (void)in; (void)scaling; (void)grain_lut; (void)row;      /* done by the job prep started */
 }
 
-/* ---- export of an output picture from its device copy (b200hook_export_picture / _tensor in b200_hooks.c) --------------
+/* ---- export of an output picture from its device copy (b200hook_export_picture / _tensor_batch in b200_hooks.c) --------------
  * Ungrained pictures are the frame job's output entry (OUT_KEY: with super-resolution the upscaled picture), grained ones the
  * entry film grain made for them; either is keyed by the picture's data[0] and laid out as geom_of() says. Both jobs take
  * the same source fields from it. */
@@ -1261,19 +1261,18 @@ static HookRefPic *bitfn(export_source)(const Dav1dPicture *const p, PicGeom *co
 int bitfn(b200hook_export_picture)(const Dav1dPicture *const p, const B200ExportJob *const tmpl, void *const stream)
 {
     PicGeom g;
-    HookRefPic *const r = bitfn(export_source)(p, &g);
+    HookRefPic *r = bitfn(export_source)(p, &g);
     if (!r) return -1;
     B200ExportJob j = *tmpl;
     EXPORT_SOURCE(j, r, g, p);
-    return b200hook_export_submit(r, 0, &j, stream);
+    return b200hook_export_submit(&r, 1, 0, &j, stream);
 }
-int bitfn(b200hook_export_tensor)(const Dav1dPicture *const p, const B200TensorJob *const tmpl, void *const stream)
+/* fills the source fields of tensor job *j from the picture's device copy: that entry, NULL when it has none */
+HookRefPic *bitfn(b200hook_tensor_source)(const Dav1dPicture *const p, B200TensorJob *const j)
 {
     PicGeom g;
     HookRefPic *const r = bitfn(export_source)(p, &g);
-    if (!r) return -1;
-    B200TensorJob j = *tmpl;
-    EXPORT_SOURCE(j, r, g, p);
-    return b200hook_export_submit(r, 1, &j, stream);
+    if (r) EXPORT_SOURCE(*j, r, g, p);
+    return r;
 }
 #undef EXPORT_SOURCE

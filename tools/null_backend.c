@@ -27,3 +27,4 @@ int b200_struct_size(int w) { switch (w) { case 9: return sizeof(B200FrameJob); 
 int b200_event_sync(void *e) { (void)e; return 0; }
 int b200_export_picture(const B200ExportJob *j, void *s) { (void)j; (void)s; return 0; }
 int b200_export_tensor(const B200TensorJob *j, void *s) { (void)j; (void)s; return 0; }
+int b200_export_tensor_batch(const B200TensorJob *j, int n, void *s) { (void)j; (void)n; (void)s; return 0; }
