@@ -384,7 +384,7 @@ class TensorJob(C.Structure):
                 ("out_w", C.c_int32), ("out_h", C.c_int32), ("dtype", C.c_int32), ("layout", C.c_int32),
                 ("full_range", C.c_int32), ("identity", C.c_int32), ("siting_x", C.c_int32), ("siting_y", C.c_int32),
                 ("cy", C.c_int32), ("rv", C.c_int32), ("gu", C.c_int32), ("gv", C.c_int32), ("bu", C.c_int32),
-                ("scale", C.c_float * 3), ("bias", C.c_float * 3), ("pad", C.c_int32),
+                ("scale", C.c_float * 3), ("bias", C.c_float * 3), ("antialias", C.c_int32),
                 ("dst", C.c_void_p), ("pitch_c", C.c_int64), ("pitch_y", C.c_int64)]
 
 

@@ -4,6 +4,8 @@
 //   export_rgb_kernel     planar R / G / B at the stream's bit depth (nearest chroma sample, integer matrix)
 //   export_tensor_kernel  R / G / B resized (bilinear, chroma upsampling included), normalised, as fp32 / fp16 / bf16 in
 //                         CHW or HWC order: what a model takes, in one pass
+//   export_tensor_aa_kernel  the same with antialiasing (triangle filter) on reduced axes: a separable pass over shared-
+//                         memory tiles, sharing export_tensor_kernel's epilogue
 // Memory bound: a thread owns a run of horizontally adjacent output samples (8 bytes: 8 samples at 8 bit, 4 above), read
 // and written with one 8-byte access where the run is complete and the rows are aligned; the RGB kernel of a vertically
 // sub-sampled picture takes two rows per thread, so that each chroma sample is read once for its 2 x 2 luma quad. The
@@ -181,6 +183,42 @@ B200_DEV typename TensorElem<DT>::type tensor_value(int v, float scale, float bi
     else return f;
 }
 
+// The epilogue of both tensor kernels: Q of a run of n (<= 4) output pixels at (x, y), per plane, through the matrix, the
+// clip, scale / bias and rounding into the destination (yoff, coff, qmax as include/b200av1.h defines them for the job)
+template <int DT, bool HWC>
+B200_DEV void tensor_store(const B200TensorJob &j, int x, int y, int n, const int (&qy)[4], const int (&qu)[4], const int (&qv)[4],
+                           int yoff, int coff, int qmax)
+{
+    typedef typename TensorElem<DT>::type E;
+    E o[3][4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        int rgb[3];
+        if (j.identity) {
+            rgb[0] = qv[i]; rgb[1] = qy[i]; rgb[2] = qu[i];
+        } else {
+            const int yy = j.cy * (qy[i] - yoff) + 8192, cb = j.mono ? 0 : qu[i] - coff, cr = j.mono ? 0 : qv[i] - coff;
+            rgb[0] = iclip((yy + j.rv * cr) >> 14, 0, qmax);
+            rgb[1] = iclip((yy - j.gu * cb - j.gv * cr) >> 14, 0, qmax);
+            rgb[2] = iclip((yy + j.bu * cb) >> 14, 0, qmax);
+        }
+#pragma unroll
+        for (int c = 0; c < 3; c++) o[c][i] = tensor_value<DT>(rgb[c], j.scale[c], j.bias[c]);
+    }
+    E *const row = (E *)j.dst + y * j.pitch_y;
+    if constexpr (HWC) {
+        // the run is 12 contiguous values: R G B of pixel 0, then of pixel 1, ...
+        E v[3][4];
+#pragma unroll
+        for (int e = 0; e < 12; e++) v[e >> 2][e & 3] = o[e % 3][e / 3];
+#pragma unroll
+        for (int r = 0; r < 3; r++) store_run(row + 3 * x + 4 * r, imin(4, 3 * n - 4 * r), v[r]);
+    } else {
+#pragma unroll
+        for (int c = 0; c < 3; c++) store_run(row + c * j.pitch_c + x, n, o[c]);
+    }
+}
+
 // The jobs of one launch travel in the kernel's parameter block (no staging copy): B200_TENSOR_BATCH_MAX of them fit the
 // classic 4 KB limit. A one-job launch takes the N = 1 form: its job's fields are then read at fixed parameter offsets, as
 // operands of the instructions that use them; indexed by blockIdx.z they are separate loads, which made the prologue of a
@@ -197,7 +235,6 @@ __global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constan
 {
     B200_PDL_ENTRY();
     typedef typename Bd<HBD>::pixel pixel;
-    typedef typename TensorElem<DT>::type E;
     const B200TensorJob &j = b.job[N == 1 ? 0 : blockIdx.z];
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4, y0 = blockIdx.y * 8 * kTensorRows + threadIdx.y;
     if (x >= j.out_w || y0 >= j.out_h) return;
@@ -220,33 +257,164 @@ __global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constan
             run_samples(qu, src + j.plane_off[1], j.stride[1], crow, ch, ct);
             run_samples(qv, src + j.plane_off[2], j.stride[2], crow, ch, ct);
         }
-        E o[3][4];
+        tensor_store<DT, HWC>(j, x, y, n, qy, qu, qv, yoff, coff, qmax);
+    }
+}
+
+// ---- antialiased reduction (B200TensorJob.antialias = 1, include/b200av1.h) ----
+// floor(num / den) for den > 0 and a quotient below 2^26, without the int64 division routine (a call, whose call sites
+// spill): two float estimates, then the remainder brought into [0, den). Exact whatever the float rounding.
+B200_DEV int64_t floor_div(int64_t num, int64_t den)
+{
+    const float rd = 1.0f / (float)den;
+    int64_t q = (int64_t)((float)num * rd);
+    q += (int64_t)((float)(num - q * den) * rd);
+    int64_t r = num - q * den;
+    while (r < 0) { q--; r += den; }
+    while (r >= den) { q++; r -= den; }
+    return q;
+}
+
+// One output sample on one axis of one plane: its taps [jlo, jhi] and their weights (1/2^14). A reduced axis (sigma > 256)
+// takes the triangle's taps with cumulative rounding, any other the bilinear taps i0 = jlo, i1 = jhi as weights.
+struct AaAxis {
+    int64_t P, T;
+    int sigma, jlo, jhi, f;
+    B200_DEV AaAxis(int x, int in, int out, int n, int s, int k)
+    {
+        P = floor_div(((int64_t)(2 * x + 1) * in - (int64_t)(1 + k) * out) * (128 >> s), out);
+        sigma = (int)floor_div((int64_t)in << (8 - s), out);
+        if (sigma <= 256) {
+            const int pos = (int)(P > 0 ? P : 0);
+            jlo = imin(pos >> 8, n - 1); jhi = imin(jlo + 1, n - 1); f = pos & 255; T = 0;
+        } else {
+            // t_j > 0 <=> P - sigma < 256 j < P + sigma (arithmetic shifts floor)
+            jlo = (int)(((P - sigma) >> 8) + 1); jhi = (int)((P + sigma - 1) >> 8);
+            jlo = imax(jlo, 0); jhi = imin(jhi, n - 1); f = 0;
+            T = cum(jhi);
+        }
+    }
+    // C_j: the sum of t_i over jlo <= i <= j, an arithmetic series on each side of P
+    B200_DEV int64_t cum(int j) const
+    {
+        const int64_t m = P >> 8;                // t_i = sigma - P + 256 i for i <= m, sigma + P - 256 i above
+        int64_t c = 0, a = jlo, e = j < m ? j : m;
+        if (e >= a) c += (e - a + 1) * (sigma - P) + 128 * (e - a + 1) * (a + e);
+        a = jlo > m + 1 ? jlo : m + 1;
+        if (j >= a) c += (j - a + 1) * (sigma + P) - 128 * (j - a + 1) * (a + j);
+        return c;
+    }
+    B200_DEV int64_t rounded(int j) const { return floor_div(cum(j) * 32768 + T, 2 * T); }
+    B200_DEV int weight(int j) const
+    {
+        if (j < jlo || j > jhi) return 0;
+        if (sigma <= 256) return (j == jlo ? (256 - f) * 64 : 0) + (j == jhi ? f * 64 : 0);
+        return (int)(rounded(j) - (j > jlo ? rounded(j - 1) : 0));
+    }
+};
+
+// A CTA owns kAaCols output columns x th output rows of one job (th = 1 .. kAaRowsMax, chosen per launch so that a single
+// picture still fills the GPU). Per plane it walks the tile's source rows in chunks of kAaChunk: the horizontal sums H' of
+// the chunk (a warp per row, a lane per column; the column weights sit in shared memory, kAaTaps at a time) go to shared
+// memory, then each thread adds wy * H' into the vertical sums of its output pixels. Shared memory does not depend on the
+// reduction factor; source samples are read straight from global memory, each source row once per tile.
+constexpr int kAaCols = 32, kAaRowsMax = 32, kAaChunk = 32, kAaTaps = 64;
+template <bool HBD, int DT, bool HWC, int N>
+__global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_constant__ TensorBatch<N> b, int th)
+{
+    B200_PDL_ENTRY();
+    typedef typename Bd<HBD>::pixel pixel;
+    __shared__ int wx[kAaCols][kAaTaps + 1];         // column weights of the current tap window
+    __shared__ int hs[kAaChunk][kAaCols + 1];        // H' of the current row chunk
+    __shared__ int wy[kAaRowsMax][kAaChunk];         // row weights of the current row chunk
+    __shared__ int qs[3][kAaRowsMax][kAaCols];       // Q of the tile
+    __shared__ int cjlo[kAaCols], cnt[kAaCols];
+    const B200TensorJob &j = b.job[N == 1 ? 0 : blockIdx.z];
+    const int x0 = blockIdx.x * kAaCols, y0 = blockIdx.y * th;
+    if (x0 >= j.out_w || y0 >= j.out_h) return;
+    const int lane = threadIdx.x, warp = threadIdx.y, tid = warp * 32 + lane;
+    const int rows = imin(th, j.out_h - y0);
+    for (int p = 0; p < (j.mono ? 1 : 3); p++) {
+        const int sh = p ? j.ss_hor : 0, sv = p ? j.ss_ver : 0;
+        const int kx = sh ? j.siting_x : 0, ky = sv ? j.siting_y : 0;
+        const int pw = (j.w + sh) >> sh, ph = (j.h + sv) >> sv;
+        const pixel *const plane = (const pixel *)j.src + j.plane_off[p];
+        const int stride = j.stride[p];
+        // this lane's column, and the tile's source rows [r_lo, r_hi]
+        const bool col_in = x0 + lane < j.out_w;
+        const AaAxis cx(col_in ? x0 + lane : x0, j.w, j.out_w, pw, sh, kx);
+        const int ntaps = col_in ? cx.jhi - cx.jlo + 1 : 0;
+        int windows = ntaps;                          // tap windows of the widest column
+        for (int o = 16; o; o >>= 1) windows = imax(windows, __shfl_xor_sync(0xffffffffu, windows, o));
+        windows = (windows + kAaTaps - 1) / kAaTaps;
+        const int r_lo = AaAxis(y0, j.h, j.out_h, ph, sv, ky).jlo, r_hi = AaAxis(y0 + rows - 1, j.h, j.out_h, ph, sv, ky).jhi;
+        __syncthreads();                              // the previous plane is done with the shared arrays
+        if (warp == 0) { cjlo[lane] = cx.jlo; cnt[lane] = ntaps; }
+        const auto fill_wx = [&](int w0) {            // the weights of taps w0 .. w0 + kAaTaps - 1 of every column
+            for (int e = tid; e < kAaCols * kAaTaps; e += 256) {
+                const int c = e / kAaTaps, i = e % kAaTaps;
+                const bool in = x0 + c < j.out_w && w0 + i < cnt[c];
+                wx[c][i] = in ? AaAxis(x0 + c, j.w, j.out_w, pw, sh, kx).weight(cjlo[c] + w0 + i) : 0;
+            }
+        };
+        __syncthreads();
+        if (windows == 1) fill_wx(0);
+        int acc[kAaRowsMax / 8] = {};                 // V of output rows warp + 8 k, column lane
+        for (int r0 = r_lo; r0 <= r_hi; r0 += kAaChunk) {
+            const int nr = imin(kAaChunk, r_hi - r0 + 1);
+            int h[kAaChunk / 8] = {};
+            for (int w0 = 0; w0 < windows * kAaTaps; w0 += kAaTaps) {
+                if (windows > 1) { __syncthreads(); fill_wx(w0); }
+                __syncthreads();
+                const int m = imin(kAaTaps, ntaps - w0);
+                const pixel *const src = plane + cx.jlo + w0;
 #pragma unroll
-        for (int i = 0; i < 4; i++) {
-            int rgb[3];
-            if (j.identity) {
-                rgb[0] = qv[i]; rgb[1] = qy[i]; rgb[2] = qu[i];
-            } else {
-                const int yy = j.cy * (qy[i] - yoff) + 8192, cb = j.mono ? 0 : qu[i] - coff, cr = j.mono ? 0 : qv[i] - coff;
-                rgb[0] = iclip((yy + j.rv * cr) >> 14, 0, qmax);
-                rgb[1] = iclip((yy - j.gu * cb - j.gv * cr) >> 14, 0, qmax);
-                rgb[2] = iclip((yy + j.bu * cb) >> 14, 0, qmax);
+                for (int k = 0; k < kAaChunk / 8; k++) {
+                    const int r = warp + 8 * k;
+                    if (r < nr) {
+                        const pixel *const row = src + (ptrdiff_t)(r0 + r) * stride;
+                        int sum = 0;
+                        for (int i = 0; i < m; i++) sum += wx[lane][i] * (int)__ldg(row + i);
+                        h[k] += sum;
+                    }
+                }
             }
 #pragma unroll
-            for (int c = 0; c < 3; c++) o[c][i] = tensor_value<DT>(rgb[c], j.scale[c], j.bias[c]);
+            for (int k = 0; k < kAaChunk / 8; k++) hs[warp + 8 * k][lane] = (h[k] + (1 << 8)) >> 9;
+            for (int e = tid; e < rows * kAaChunk; e += 256) {
+                const int t = e / kAaChunk, r = e % kAaChunk;
+                wy[t][r] = r < nr ? AaAxis(y0 + t, j.h, j.out_h, ph, sv, ky).weight(r0 + r) : 0;
+            }
+            __syncthreads();
+#pragma unroll
+            for (int k = 0; k < kAaRowsMax / 8; k++) {
+                const int t = warp + 8 * k;
+                if (t < rows) {
+                    int v = 0;
+                    for (int r = 0; r < nr; r++) v += wy[t][r] * hs[r][lane];
+                    acc[k] += v;
+                }
+            }
+            __syncthreads();                          // hs and wy are rewritten by the next chunk
         }
-        E *const row = (E *)j.dst + y * j.pitch_y;
-        if constexpr (HWC) {
-            // the run is 12 contiguous values: R G B of pixel 0, then of pixel 1, ...
-            E v[3][4];
 #pragma unroll
-            for (int e = 0; e < 12; e++) v[e >> 2][e & 3] = o[e % 3][e / 3];
+        for (int k = 0; k < kAaRowsMax / 8; k++)
+            if (warp + 8 * k < rows) qs[p][warp + 8 * k][lane] = (acc[k] + (1 << 16)) >> 17;
+    }
+    __syncthreads();
+    const int bdmax = j.bitdepth_max, s = bdmax == 4095 ? 4 : bdmax == 1023 ? 2 : 0;
+    const int yoff = j.full_range ? 0 : 64 << s, coff = 512 << s;
+    // the epilogue: a thread per run of 4 columns of one row
+    for (int e = tid; e < rows * (kAaCols / 4); e += 256) {
+        const int t = e / (kAaCols / 4), c = 4 * (e % (kAaCols / 4)), x = x0 + c;
+        if (x >= j.out_w) continue;
+        int qy[4], qu[4] = {}, qv[4] = {};
 #pragma unroll
-            for (int r = 0; r < 3; r++) store_run(row + 3 * x + 4 * r, imin(4, 3 * n - 4 * r), v[r]);
-        } else {
-#pragma unroll
-            for (int c = 0; c < 3; c++) store_run(row + c * j.pitch_c + x, n, o[c]);
+        for (int i = 0; i < 4; i++) {
+            qy[i] = qs[0][t][c + i];
+            if (!j.mono) { qu[i] = qs[1][t][c + i]; qv[i] = qs[2][t][c + i]; }
         }
+        tensor_store<DT, HWC>(j, x, y0 + t, imin(4, j.out_w - x), qy, qu, qv, yoff, coff, 4 * bdmax);
     }
 }
 
@@ -287,9 +455,10 @@ static int check_tensor_job(const B200TensorJob &j, const char *who)
     const auto in_range = [](int v, int lo, int hi) { return v >= lo && v <= hi; };
     if (!j.src || !in_range(j.w, 1, 65536) || !in_range(j.h, 1, 65536) || !in_range(j.out_w, 1, 65536) || !in_range(j.out_h, 1, 65536) ||
         !in_range(j.ss_hor, 0, 1) || !in_range(j.ss_ver, 0, 1) || !in_range(j.siting_x, 0, 1) || !in_range(j.siting_y, 0, 1) ||
-        !in_range(j.dtype, B200_TENSOR_F32, B200_TENSOR_BF16) || !in_range(j.layout, B200_TENSOR_CHW, B200_TENSOR_HWC)) {
-        b200_set_error("%s: bad arguments (%d x %d -> %d x %d, dtype %d, layout %d)", who, j.w, j.h, j.out_w, j.out_h,
-                       j.dtype, j.layout);
+        !in_range(j.dtype, B200_TENSOR_F32, B200_TENSOR_BF16) || !in_range(j.layout, B200_TENSOR_CHW, B200_TENSOR_HWC) ||
+        !in_range(j.antialias, 0, 1)) {
+        b200_set_error("%s: bad arguments (%d x %d -> %d x %d, dtype %d, layout %d, antialias %d)", who, j.w, j.h, j.out_w,
+                       j.out_h, j.dtype, j.layout, j.antialias);
         return -2;
     }
     if (j.identity && (j.mono || j.ss_hor || j.ss_ver)) { b200_set_error("%s: identity matrix needs 4:4:4", who); return -2; }
@@ -310,9 +479,36 @@ static int check_tensor_job(const B200TensorJob &j, const char *who)
     return 0;
 }
 
-// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype and layout
+// whether a job takes the antialiased kernel: antialias = 1 and a luma axis reduced (sigma > 256, include/b200av1.h)
+static bool tensor_job_aa(const B200TensorJob &j)
+{
+    return j.antialias && ((int64_t)j.w * 256 / j.out_w > 256 || (int64_t)j.h * 256 / j.out_h > 256);
+}
+
+// the antialiased kernel's launch: the tallest tile (th output rows) whose grid still has kAaMinCtas CTAs, the SM count of
+// an H100 SXM, so that a single picture reduced to a small output still spreads over the whole GPU
+constexpr int kAaMinCtas = 132;
 template <int N>
-static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, cudaStream_t stream)
+static int launch_tensor_aa_jobs(const TensorBatch<N> &b, int n, int out_w, int out_h, cudaStream_t stream)
+{
+    const B200TensorJob &j = b.job[0];
+    const int xt = (out_w + kAaCols - 1) / kAaCols;
+    int th = kAaRowsMax;
+    while (th > 1 && (int64_t)xt * ((out_h + th - 1) / th) * n < kAaMinCtas) th >>= 1;
+    const dim3 grid(xt, (out_h + th - 1) / th, n);
+    return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, stream, [&](auto hbd) {
+        constexpr bool H = decltype(hbd)::value;
+        void (*const k[3][2])(TensorBatch<N>, int) = {
+            {export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N>},
+            {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N>},
+            {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N>}};
+        return std::make_tuple(k[j.dtype][j.layout], b, th);
+    });
+}
+
+// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype, layout and kernel (aa)
+template <int N>
+static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, bool aa, cudaStream_t stream)
 {
     TensorBatch<N> b{};
     int out_w = 0, out_h = 0;
@@ -320,6 +516,7 @@ static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, cudaStrea
         b.job[i] = *jobs[i];
         out_w = imax(out_w, jobs[i]->out_w); out_h = imax(out_h, jobs[i]->out_h);
     }
+    if (aa) return launch_tensor_aa_jobs(b, n, out_w, out_h, stream);
     const B200TensorJob &j = b.job[0];
     const int runs = (out_w + 3) / 4;
     const dim3 grid((runs + 31) / 32, (out_h + 8 * kTensorRows - 1) / (8 * kTensorRows), n);
@@ -332,9 +529,9 @@ static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, cudaStrea
         return std::make_tuple(k[j.dtype][j.layout], b);
     });
 }
-static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, cudaStream_t stream)
+static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, bool aa, cudaStream_t stream)
 {
-    return n == 1 ? launch_tensor_jobs<1>(jobs, n, stream) : launch_tensor_jobs<B200_TENSOR_BATCH_MAX>(jobs, n, stream);
+    return n == 1 ? launch_tensor_jobs<1>(jobs, n, aa, stream) : launch_tensor_jobs<B200_TENSOR_BATCH_MAX>(jobs, n, aa, stream);
 }
 
 extern "C" int b200_export_tensor(const B200TensorJob *job, void *stream)
@@ -352,20 +549,23 @@ extern "C" int b200_export_tensor_batch(const B200TensorJob *jobs, int n, void *
             return -2;
         }
     }
-    // one launch per bit-depth class present and per B200_TENSOR_BATCH_MAX jobs of it, jobs in their order
-    for (int hbd = 0; hbd < 2; hbd++) {
+    // one launch per bit-depth class and kernel (bilinear, antialiased) present and per B200_TENSOR_BATCH_MAX jobs of it,
+    // jobs in their order
+    for (int group = 0; group < 4; group++) {
+        const int hbd = group & 1;
+        const bool aa = group >> 1;
         const B200TensorJob *part[B200_TENSOR_BATCH_MAX];
         int m = 0;
         for (int i = 0; i < n; i++) {
-            if ((jobs[i].bitdepth_max > 255) != hbd) continue;
+            if ((jobs[i].bitdepth_max > 255) != hbd || tensor_job_aa(jobs[i]) != aa) continue;
             part[m++] = &jobs[i];
             if (m == B200_TENSOR_BATCH_MAX) {
-                if (int r = launch_tensor_jobs(part, m, (cudaStream_t)stream)) return r;
+                if (int r = launch_tensor_jobs(part, m, aa, (cudaStream_t)stream)) return r;
                 m = 0;
             }
         }
         if (m)
-            if (int r = launch_tensor_jobs(part, m, (cudaStream_t)stream)) return r;
+            if (int r = launch_tensor_jobs(part, m, aa, (cudaStream_t)stream)) return r;
     }
     return 0;
 }

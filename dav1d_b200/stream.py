@@ -212,17 +212,53 @@ def tensor_taps(out, inn, n, s=0, k=0):
     return i0, np.minimum(i0 + 1, n - 1), pos & 255
 
 
-def tensor_reference(planes, bpc, layout, size=None, matrix="bt709", full_range=False, siting="left", mean=None, std=None):
+def tensor_weights(out, inn, n, s=0, k=0):
+    """[out, n] int64 weights (1/2^14, each row summing to 2^14) of the antialiased tensor export along one axis
+    (include/b200av1.h B200TensorJob, antialias = 1); arguments as in tensor_taps. An axis that this plane does not reduce
+    (sigma <= 256) gets its bilinear taps as weights; a reduced one the triangle of half-width sigma, clipped at the edges,
+    with cumulative rounding."""
+    x = np.arange(out, dtype=np.int64)
+    P = ((2 * x + 1) * inn - (1 + k) * out) * (1 << (7 - s)) // out
+    sigma = inn * (1 << (8 - s)) // out
+    W = np.zeros((out, n), np.int64)
+    if sigma <= 256:
+        i0, i1, f = tensor_taps(out, inn, n, s, k)
+        np.add.at(W, (x, i0), (256 - f) * 64)
+        np.add.at(W, (x, i1), f * 64)
+        return W
+    t = np.maximum(sigma - np.abs(256 * np.arange(n, dtype=np.int64)[None, :] - P[:, None]), 0)
+    T = t.sum(1, keepdims=True)
+    R = (np.cumsum(t, axis=1) * (1 << 15) + T) // (2 * T)
+    return np.diff(R, axis=1, prepend=0)
+
+
+def tensor_antialiased(w, h, size, antialias):
+    """whether an export of a w x h picture to size = (OH, OW) takes the antialiased definition: antialias and a luma axis
+    reduced (sigma > 256)"""
+    oh, ow = size
+    return bool(antialias) and (w * 256 // ow > 256 or h * 256 // oh > 256)
+
+
+def tensor_reference(planes, bpc, layout, size=None, matrix="bt709", full_range=False, siting="left", mean=None, std=None,
+                     antialias=False):
     """numpy statement of the tensor export (include/b200av1.h B200TensorJob) for one picture's planes (layout = enum
-    Dav1dPixelLayout): float32 [3, OH, OW] of R, G, B; size = (OH, OW), by default the picture's"""
+    Dav1dPixelLayout): float32 [3, OH, OW] of R, G, B; size = (OH, OW), by default the picture's. antialias=True: the
+    antialiased definition (triangle filter on reduced axes), which leaves exports without a reduced luma axis unchanged."""
     h, w = planes[0].shape
     oh, ow = size or (h, w)
     ssh, ssv = int(layout in (1, 2)), int(layout == 1)
     kx, ky = SITINGS[siting]
     s, bdmax = bpc - 8, (1 << bpc) - 1
+    aa = tensor_antialiased(w, h, (oh, ow), antialias)
 
     def sample(p, sh, sv, kx, ky):
         p = p.astype(np.int64)
+        if aa:
+            wx = tensor_weights(ow, w, p.shape[1], sh, kx if sh else 0)
+            wy = tensor_weights(oh, h, p.shape[0], sv, ky if sv else 0)
+            # float64 products are exact here (every partial sum is an integer below 2^31) and take the BLAS path
+            hq = (np.rint(p.astype(np.float64) @ wx.T.astype(np.float64)).astype(np.int64) + (1 << 8)) >> 9
+            return (np.rint(wy.astype(np.float64) @ hq.astype(np.float64)).astype(np.int64) + (1 << 16)) >> 17
         x0, x1, fx = tensor_taps(ow, w, p.shape[1], sh, kx if sh else 0)
         y0, y1, fy = tensor_taps(oh, h, p.shape[0], sv, ky if sv else 0)
         a = p[np.ix_(y0, x0)] * (256 - fx) + p[np.ix_(y0, x1)] * fx
@@ -299,12 +335,15 @@ class DeviceDecoder:
         yield from self._decode(tus, lambda h, info: self._export(h, info, format, matrix, full_range, alloc, stream))
 
     def tensors(self, tus, size=None, dtype="float32", layout="chw", mean=None, std=None, matrix="auto", full_range=None,
-                chroma_siting="auto", batch=None, alloc=None, stream=None):
+                chroma_siting="auto", batch=None, alloc=None, stream=None, antialias=False):
         """Decodes the temporal units `tus` and yields every output picture as a model input: R, G, B resized to
         size = (height, width) (default: the picture's own) by bilinear sampling at half-sample centres, like
         torch.nn.functional.interpolate(mode="bilinear", align_corners=False) (chroma upsampling is part of the same
         sampling), then (x - mean) / std with x in [0, 1], as a [3, OH, OW] (layout="chw") or [OH, OW, 3] ("hwc") tensor of
         dtype "float32", "float16" or "bfloat16". One kernel per picture (include/b200av1.h, B200TensorJob).
+        antialias=True filters reduced axes with a triangle as wide as the reduction, like interpolate(mode="bilinear",
+        antialias=True) and torchvision's Resize: what vision models are trained on. It changes nothing when no luma axis
+        is reduced.
         batch=N: yields [n, ...] tensors of up to N pictures, each picture exported straight into its slot; a picture of
         another size (size=None with frame-size changes) closes the batch early.
         matrix and full_range: as in pictures(). chroma_siting: "auto" (the sequence header's chroma_sample_position:
@@ -333,7 +372,8 @@ class DeviceDecoder:
             shape = (3, oh, ow) if layout == "chw" else (oh, ow, 3)
             if batch is None:
                 out = alloc(shape, dtype)
-                self._export_tensor(h, info, _data_ptr(out), oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, stream)
+                self._export_tensor(h, info, _data_ptr(out), oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
+                                    antialias, stream)
                 return [out]
             done = []
             if state["buf"] is not None and state["shape"] != shape:       # another size closes the batch
@@ -342,7 +382,7 @@ class DeviceDecoder:
             if state["buf"] is None:
                 state.update(buf=alloc((int(batch),) + shape, dtype), n=0, shape=shape)
             dst = _data_ptr(state["buf"]) + state["n"] * 3 * oh * ow * esize
-            self._export_tensor(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, stream)
+            self._export_tensor(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, antialias, stream)
             state["n"] += 1
             if state["n"] == batch:
                 done.append(state["buf"])
@@ -355,12 +395,12 @@ class DeviceDecoder:
             yield state["buf"][:state["n"]]
 
     def clips(self, streams, frames, step=1, start=0, size=None, dtype="float32", layout="chw", mean=None, std=None,
-              matrix="auto", full_range=None, chroma_siting="auto", workers=None, alloc=None, stream=None):
+              matrix="auto", full_range=None, chroma_siting="auto", workers=None, alloc=None, stream=None, antialias=False):
         """Decodes N streams (each a list of temporal units) concurrently and returns one clip per stream as a
         [N, frames, 3, OH, OW] tensor (layout="hwc": [N, frames, OH, OW, 3]): x[i, t] is output picture
         start_i + t * step of stream i, exported exactly as tensors() exports it. `start` is one int or one per stream.
-        size=None needs every sampled picture to have the same size. The tensor options, alloc and stream mean what they
-        mean in tensors(); "auto" matrix, range and siting are resolved per stream from its own headers.
+        size=None needs every sampled picture to have the same size. The tensor options (antialias included), alloc and
+        stream mean what they mean in tensors(); "auto" matrix, range and siting are resolved per stream from its own headers.
         Each stream has a dav1d context of its own (this decoder's n_threads / max_frame_delay) driven by a host thread of
         its own; at most `workers` streams are open at once (default min(N, CLIP_WORKERS), at most CLIP_MAX_WORKERS).
         Pictures that are not sampled are released unexported, and a stream is closed once its last sampled picture is
@@ -423,7 +463,8 @@ class DeviceDecoder:
                             raise ValueError("stream %d picture %d is %dx%d, not %dx%d like the others: pass size= for "
                                              "pictures of different sizes" % (i, starts[i] + t * step, ow, oh, hw[1], hw[0]))
                         dst = _data_ptr(out) + (i * frames + t) * 3 * oh * ow * esize
-                        jobs[k] = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting)
+                        jobs[k] = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
+                                                   antialias)
                         pics[k] = self.dll.refdrv_stream_picture(h)
                     if self.dll.b200hook_export_tensor_batch(pics, jobs, len(items), C.c_void_p(stream)) != 0:
                         raise RuntimeError("exporting pictures failed (see stderr)")
@@ -526,12 +567,12 @@ class DeviceDecoder:
             name = "bt709"
         return name
 
-    def _export_tensor(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, stream):
-        job = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting)
+    def _export_tensor(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, stream):
+        job = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias)
         if self.dll.b200hook_export_tensor(self.dll.refdrv_stream_picture(h), C.byref(job), C.c_void_p(stream)) != 0:
             raise RuntimeError("exporting a picture failed (see stderr)")
 
-    def _tensor_job(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting):
+    def _tensor_job(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias=False):
         """the B200TensorJob of the picture stream h holds (info as _decode gives it): "auto" matrix, range and siting come
         from that stream's own headers"""
         w, hh, bpc, pl, mtrx, color_range = (int(v) for v in info)
@@ -548,6 +589,7 @@ class DeviceDecoder:
         scale, bias = tensor_scale_bias(bpc, mean, std)
         for c in range(3):
             job.scale[c], job.bias[c] = float(scale[c]), float(bias[c])
+        job.antialias = int(bool(antialias))
         job.dst = dst
         job.pitch_y, job.pitch_c = (ow, oh * ow) if layout == "chw" else (3 * ow, 1)
         return job

@@ -794,6 +794,19 @@ B200_API int b200_export_picture(const B200ExportJob *job, void *stream);
  *     kept to 1/256 sample; upsampling chroma and resizing are one operation.
  *   Samples, per plane: V = (S[y0][x0] * (256 - fx) + S[y0][x1] * fx) * (256 - fy) + (S[y1][x0] * (256 - fx) + S[y1][x1] * fx) * fy
  *     Q = (V + 2^13) >> 14: the sample with 2 fractional bits, 0 .. 4 * bdmax.
+ *   antialias = 1 with a reduced luma axis (luma sigma below > 256 on either axis; a job with neither is exported exactly
+ *     as with antialias = 0, so enlarging and same-size exports never change): a triangle filter whose half-width is the reduction factor (torch's
+ *     interpolate(mode="bilinear", antialias=True, align_corners=False), PIL's and torchvision's antialiased resize), with
+ *     taps clipped at the picture edge and the weights renormalised over the taps that remain. Per axis and plane:
+ *       P = floor(((2x + 1) * IN - (1 + k) * OUT) * 2^(7 - s) / OUT)   the output's centre in 1/256 sample (pos unclamped)
+ *       sigma = floor(IN * 2^(8 - s) / OUT)                             half-width in 1/256 sample
+ *       sigma <= 256 (axis not reduced on this plane): taps i0, i1 above with weights (256 - f) * 64 and f * 64
+ *       sigma > 256: taps j in [0, n - 1] with t_j = sigma - |256 j - P| > 0, T = sum of t_j, C_j = sum of t_i for i <= j,
+ *         R_j = floor((C_j * 2^15 + T) / (2T)), weight w_j = R_j - R_(j-1): each within 2^-14 of t_j / T, summing to 2^14
+ *       H  = sum over j of wx_j * S[row][j]       per source row, int32 (<= 4095 * 2^14)
+ *       H' = (H + 2^8) >> 9                       5 fractional bits (<= 131040)
+ *       V  = sum over rows r of wy_r * H'[r]      int32 (<= 131040 * 2^14)
+ *       Q  = (V + 2^16) >> 17                     2 fractional bits, 0 .. 4 * bdmax; the matrix and output below follow
  *   Matrix, with s = bitdepth - 8: Y' = Qy - (full_range ? 0 : 64 << s), C' = Qc - (512 << s) (mono: Cb' = Cr' = 0), and
  *       R = clip((cy * Y' + rv * Cr' + 8192) >> 14)
  *       G = clip((cy * Y' - gu * Cb' - gv * Cr' + 8192) >> 14)
@@ -818,7 +831,7 @@ typedef struct B200TensorJob {
     int32_t siting_x, siting_y;    /* 0 or 1, see above */
     int32_t cy, rv, gu, gv, bu;    /* the matrix, 1.0 = 1 << 14 (as B200ExportJob) */
     float scale[3], bias[3];       /* per output channel R, G, B */
-    int32_t pad;
+    int32_t antialias;             /* 0: bilinear; 1: triangle filter on reduced axes (see above) */
     void *dst;                     /* device */
     int64_t pitch_c, pitch_y;      /* elements */
 } B200TensorJob;

@@ -1,6 +1,6 @@
 """The tensor export (b200_export_tensor) against the torch chain it replaces (run on a GPU machine):
 
-    python tools/bench_tensor_export.py [--launches 200] [--rounds 5] [--reps 3] [--out FILE]
+    python tools/bench_tensor_export.py [--launches 200] [--rounds 5] [--reps 3] [--antialias] [--kernel-only] [--out FILE]
 
 Kernel level, one JSON line per configuration, on synthetic device pictures (random planes, 4:2:0):
   fused        one b200_export_tensor launch
@@ -15,6 +15,9 @@ Kernel level, one JSON line per configuration, on synthetic device pictures (ran
 Decoder level, one JSON line per stream workload of bench.py: pictures per second of
   DeviceDecoder.tensors(size, dtype="bfloat16", batch=8) against DeviceDecoder.pictures(format="rgb") followed by the
   torch chain and torch.stack of every 8, the whole stream per run (median, min and max of --reps runs, alternated).
+--antialias: the kernel level only, on AA_CONFIGS, with B200TensorJob.antialias = 1 against the chain with
+  interpolate(..., antialias=True); a config with a batch runs that many pictures as one b200_export_tensor_batch call
+  (the chain then loops over them). --kernel-only skips the decoder level.
 The GPU's name, power limit and SM clock are read in the same run."""
 import argparse
 import ctypes as C
@@ -46,10 +49,19 @@ CONFIGS = [  # (name, source w, h, bpc, output (h, w) or None, dtype, layout)
 ]
 
 
-def torch_chain(rgb, bdmax, size, dtype, layout, mean, std):
+AA_CONFIGS = [  # (name, source w, h, bpc, output (h, w), dtype, layout, pictures per call)
+    ("aa 1080p8 -> 224x224 bf16 chw", 1920, 1080, 8, (224, 224), "bfloat16", "chw", 1),
+    ("aa 4k10 -> 398x224 bf16 chw", 3840, 2160, 10, (224, 398), "bfloat16", "chw", 1),
+    ("aa 4k8 -> 1920x1080 fp16 chw", 3840, 2160, 8, (1080, 1920), "float16", "chw", 1),
+    ("aa 1080p8 -> 640x360 fp32 hwc", 1920, 1080, 8, (360, 640), "float32", "hwc", 1),
+    ("aa 64 x 1080p8 -> 224x224 bf16 chw, one batch call", 1920, 1080, 8, (224, 224), "bfloat16", "chw", 64),
+]
+
+
+def torch_chain(rgb, bdmax, size, dtype, layout, mean, std, antialias=False):
     x = rgb.float() / bdmax
     if size is not None:
-        x = F.interpolate(x[None], size=size, mode="bilinear", align_corners=False)[0]
+        x = F.interpolate(x[None], size=size, mode="bilinear", align_corners=False, antialias=antialias)[0]
     x = ((x - mean) / std).to(getattr(torch, dtype))
     return x.permute(1, 2, 0).contiguous() if layout == "hwc" else x
 
@@ -73,7 +85,8 @@ def kernel_level(args):
     lib = _lib.get_lib()
     s = torch.cuda.Stream()
     lines = []
-    for name, w, h, bpc, size, dtype, layout in CONFIGS:
+    configs = AA_CONFIGS if args.antialias else [c + (1,) for c in CONFIGS]
+    for name, w, h, bpc, size, dtype, layout, pics in configs:
         rng = np.random.default_rng(w + bpc)
         bdmax, sb = (1 << bpc) - 1, 1 if bpc == 8 else 2
         planes = [rng.integers(0, bdmax + 1, (ph, pw)).astype(np.uint8 if bpc == 8 else np.int16) for pw, ph in stream.plane_dims(w, h, 1)]
@@ -94,6 +107,13 @@ def kernel_level(args):
         for c in range(3):
             tj.scale[c], tj.bias[c] = float(scale[c]), float(bias[c])
         tj.dst, tj.pitch_c, tj.pitch_y = out.data_ptr(), (oh * ow if layout == "chw" else 1), (ow if layout == "chw" else 3 * ow)
+        tj.antialias = int(args.antialias)
+        if pics > 1:                             # the same picture into pics slots, one call
+            out = torch.empty((pics,) + shape, dtype=getattr(torch, dtype), device="cuda")
+            tjs = (stream.TensorJob * pics)()
+            for k in range(pics):
+                tjs[k] = stream.TensorJob.from_buffer_copy(tj)
+                tjs[k].dst = out[k].data_ptr()
         rgb = torch.empty((3, h, w), dtype=torch.uint8 if bpc == 8 else torch.int16, device="cuda")
         ej = stream.ExportJob()
         ej.src, ej.format = src.data_ptr(), 1
@@ -107,11 +127,15 @@ def kernel_level(args):
         sp = C.c_void_p(s.cuda_stream)
 
         def fused():
-            lib.check(lib.b200_export_tensor(C.byref(tj), sp), "b200_export_tensor")
+            if pics > 1:
+                lib.check(lib.b200_export_tensor_batch(tjs, pics, sp), "b200_export_tensor_batch")
+            else:
+                lib.check(lib.b200_export_tensor(C.byref(tj), sp), "b200_export_tensor")
 
         def chain():
-            lib.check(lib.b200_export_picture(C.byref(ej), sp), "b200_export_picture")
-            torch_chain(rgb, bdmax, size, dtype, layout, mean, std)
+            for _ in range(pics):
+                lib.check(lib.b200_export_picture(C.byref(ej), sp), "b200_export_picture")
+                torch_chain(rgb, bdmax, size, dtype, layout, mean, std, args.antialias)
 
         times = {"fused": [], "torch_chain": []}
         with torch.cuda.stream(s):
@@ -128,9 +152,11 @@ def kernel_level(args):
                     b.record(s)
                     b.synchronize()
                     times[key].append(1e3 * a.elapsed_time(b) / args.launches)
-        fused_bytes = w * h * 3 // 2 * sb + 3 * oh * ow * ESIZE[dtype]
+        fused_bytes = pics * (w * h * 3 // 2 * sb + 3 * oh * ow * ESIZE[dtype])
         line = {"config": name, "gpu": gpu_info(), "launches_per_round": args.launches, "rounds": args.rounds, "us": {}, "bytes": {
-            "fused": fused_bytes, "torch_chain": chain_bytes(w, h, sb, size, dtype, layout)}, "GBps": {}, "share_of_3.35TBps": {}}
+            "fused": fused_bytes, "torch_chain": pics * chain_bytes(w, h, sb, size, dtype, layout)}, "GBps": {}, "share_of_3.35TBps": {}}
+        if args.antialias:
+            line["antialias"] = True
         for key, v in times.items():
             med = float(np.median(v))
             line["us"][key] = {"median": round(med, 2), "min": round(min(v), 2)}
@@ -199,10 +225,12 @@ def main():
     ap.add_argument("--launches", type=int, default=200)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--antialias", action="store_true")
+    ap.add_argument("--kernel-only", action="store_true")
     ap.add_argument("--out")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
-    lines = kernel_level(args) + decoder_level(args)
+    lines = kernel_level(args) + ([] if args.antialias or args.kernel_only else decoder_level(args))
     if args.out:
         with open(args.out, "w") as fh:
             for line in lines:
