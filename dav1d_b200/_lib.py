@@ -164,7 +164,8 @@ class FrameJob(C.Structure):
                 ("coef_bytes", C.c_uint64),
                 ("run_fg", C.c_int32), ("pad5", C.c_int32), ("fg", FgFrame),
                 ("d_blend2", C.c_void_p), ("n_blend2", C.c_int32), ("pad9", C.c_int32),
-                ("run_resize", C.c_int32), ("pad10", C.c_int32), ("resize", ResizeFrame * 2)]
+                ("run_resize", C.c_int32), ("pad10", C.c_int32), ("resize", ResizeFrame * 2),
+                ("d_itx_coff", C.c_void_p * 19)]
 
 
 class FrameBand(C.Structure):

@@ -13,8 +13,6 @@
 #include <utility>
 
 namespace b200 {   // itx.cu
-int launch_itx_grouped(const void *const *blocks, const int32_t *n, void *coefs, void *pic, const int32_t *st,
-                       int bdmax, int zero, cudaStream_t stream);
 int launch_itx(int tx, const B200ItxBlock *blocks, int n, void *coefs, void *pic, const int32_t *st, int bdmax, int zero,
                cudaStream_t stream);
 }

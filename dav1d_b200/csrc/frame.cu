@@ -19,15 +19,26 @@ static B200FrameBand whole_band(const B200FrameJob *j)
     return b;
 }
 
-// The stages before intra reconstruction, over the band's records. The first band zeroes the dense coefficients that
-// the coefficient expansion of every band fills.
+// The inverse transforms read the compact coefficient stream directly (B200FrameJob.d_itx_coff): the job has the stream
+// and an offset array for every size with blocks, and no intra records (the intra kernels read the dense plane).
+static bool itx_reads_compact(const B200FrameJob *j)
+{
+    if (!j->d_ccoef || j->n_intra > 0) return false;
+    for (int t = 0; t < B200_N_RECT_TX_SIZES; t++)
+        if (j->d_itx[t] && j->n_itx[t] > 0 && !j->d_itx_coff[t]) return false;
+    return true;
+}
+
+// The stages before intra reconstruction, over the band's records. Dense coefficient input: the first band zeroes the
+// dense coefficients that the coefficient expansion of every band fills. Compact input: neither runs.
 static int band_recon(const B200FrameJob *j, const B200FrameBand *b, void *stream)
 {
     int r;
     const int bd = j->bitdepth_max;
-    if (b->y0 == 0 && j->n_expand > 0) B200_CUDA_OK(cudaMemsetAsync(j->d_coef, 0, j->coef_bytes, (cudaStream_t)stream));
+    const bool compact = itx_reads_compact(j);
+    if (!compact && b->y0 == 0 && j->n_expand > 0) B200_CUDA_OK(cudaMemsetAsync(j->d_coef, 0, j->coef_bytes, (cudaStream_t)stream));
 #define SUB(ptr, rng) ((ptr) ? (ptr) + (rng)[0] : (ptr)), ((ptr) ? (rng)[1] : 0)
-    if (j->n_expand > 0 && (r = b200_coef_expand(bd, SUB(j->d_expand, b->expand), j->d_ccoef, j->d_coef, stream))) return r;
+    if (!compact && j->n_expand > 0 && (r = b200_coef_expand(bd, SUB(j->d_expand, b->expand), j->d_ccoef, j->d_coef, stream))) return r;
     if ((r = b200_mc_batch(bd, &j->mc, SUB(j->d_pred, b->pred), stream))) return r;
     if ((r = b200_mc_scaled_batch(bd, &j->mc, SUB(j->d_scaled, b->scaled), stream))) return r;
     if ((r = b200_mc_warp_batch(bd, &j->mc, SUB(j->d_warp, b->warp), stream))) return r;
@@ -39,10 +50,17 @@ static int band_recon(const B200FrameJob *j, const B200FrameBand *b, void *strea
     if ((r = b200_mc_blend_batch(bd, &j->mc, SUB(j->d_blend2, b->blend2), stream))) return r;
 #undef SUB
     const void *itx_p[B200_N_RECT_TX_SIZES];
+    const uint32_t *itx_c[B200_N_RECT_TX_SIZES];
     int32_t itx_n[B200_N_RECT_TX_SIZES];
     for (int t = 0; t < B200_N_RECT_TX_SIZES; t++) {
+        // (a band's b->itx[t] range indexes the records and their offsets alike)
         itx_p[t] = j->d_itx[t] ? j->d_itx[t] + b->itx[t][0] : nullptr;
+        itx_c[t] = j->d_itx[t] && j->d_itx_coff[t] ? j->d_itx_coff[t] + b->itx[t][0] : nullptr;
         itx_n[t] = j->d_itx[t] ? b->itx[t][1] : 0;
+    }
+    if (compact) {
+        if (int e = b200::check_bdmax(bd, "b200_frame_run")) return e;
+        return b200::launch_itx_grouped(itx_p, itx_n, (void *)j->d_ccoef, j->mc.dst, j->itx_stride, bd, 0, (cudaStream_t)stream, itx_c);
     }
     return b200_itx_add_frame(bd, itx_p, itx_n, j->d_coef, j->mc.dst, j->itx_stride, j->zero_coefs, stream);
 }

@@ -52,6 +52,10 @@ int lr_frame_rows(int bdmax, const B200LrFrame *f, int r0, int r1, cudaStream_t 
 // y1 into `edge` at the end of a band's reconstruction
 int intra_band(int bdmax, const B200IntraFrame *f, const B200IntraTx *d_tx, int n, int y0, const void *edge, cudaStream_t stream);
 int intra_edge_save(int bdmax, const B200IntraFrame *f, int y1, void *edge, cudaStream_t stream);
+// all transform sizes of a frame (itx.cu, b200_itx_add_frame). coffs != nullptr: the compact form, `coefs` is the compact
+// coefficient stream and coffs[tx][i] the offset of block i's coefficients in it (B200FrameJob.d_itx_coff)
+int launch_itx_grouped(const void *const *blocks, const int32_t *n, void *coefs, void *pic, const int32_t *st,
+                       int bdmax, int zero, cudaStream_t stream, const uint32_t *const *coffs = nullptr);
 
 [[noreturn]] inline void die(const char *what) {
     fprintf(stderr, "b200av1: %s failed: %s\n", what, b200_last_error());

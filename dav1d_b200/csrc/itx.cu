@@ -14,6 +14,8 @@
 #include "itx_body.cuh"
 #include "host_util.h"
 #include "launch_count.h"
+#define B200_SCAN_TBL __device__
+#include "scan_gen.h"
 
 namespace b200 {
 
@@ -33,6 +35,7 @@ itx_add_kernel(const B200ItxBlock *__restrict__ blocks, int n_blocks,
 // ---- all transform sizes of a frame in two launches (one per register class), CTAs dealt largest size first ---
 struct ItxGroups {
     const B200ItxBlock *blocks[B200_N_RECT_TX_SIZES];
+    const uint32_t *coffs[B200_N_RECT_TX_SIZES];          // compact form: per block the offset of its coefficients
     int n[B200_N_RECT_TX_SIZES];
     int cta_begin[B200_N_RECT_TX_SIZES], cta_end[B200_N_RECT_TX_SIZES];
 };
@@ -48,7 +51,8 @@ template <bool BIG> struct ItxClass {
                                                        : ItxGeom<32, 32>::NB * ItxGeom<32, 32>::SLOT);
 };
 
-template <bool HBD, bool BIG>
+// COMPACT: `coefs` is the compact coefficient stream, g.coffs[tx] the blocks' offsets into it (itx_add_body)
+template <bool HBD, bool BIG, bool COMPACT>
 __global__ void __launch_bounds__(kItxWarps * 32, ItxClass<BIG>::kMinCtas)
 itx_add_grouped_kernel(const __grid_constant__ ItxGroups g, typename Bd<HBD>::coef *__restrict__ coefs, typename Bd<HBD>::pixel *__restrict__ pic,
                        int stride0, int stride1, int stride2, int bitdepth_max, int zero_coefs)
@@ -59,8 +63,9 @@ itx_add_grouped_kernel(const __grid_constant__ ItxGroups g, typename Bd<HBD>::co
 #define X(TX, W, H, SH) \
     if constexpr ((W == 64 || H == 64) == BIG) { \
         if (c < g.cta_end[TX]) { \
-            itx_add_body<W, H, TX, SH, HBD>(c - g.cta_begin[TX], tile, g.blocks[TX], g.n[TX], coefs, pic, stride0, stride1, \
-                                            stride2, bitdepth_max, zero_coefs); \
+            itx_add_body<W, H, TX, SH, HBD, false, COMPACT>(c - g.cta_begin[TX], tile, g.blocks[TX], g.n[TX], coefs, pic, stride0, \
+                                                            stride1, stride2, bitdepth_max, zero_coefs, g.coffs[TX], \
+                                                            b200_scan + b200_scan_off[TX]); \
             return; \
         } \
     }
@@ -69,7 +74,7 @@ itx_add_grouped_kernel(const __grid_constant__ ItxGroups g, typename Bd<HBD>::co
 }
 
 int launch_itx_grouped(const void *const *blocks, const int32_t *n, void *coefs, void *pic, const int32_t *st,
-                       int bdmax, int zero, cudaStream_t stream)
+                       int bdmax, int zero, cudaStream_t stream, const uint32_t *const *coffs)
 {
     for (int big = 1; big >= 0; big--) {
         ItxGroups g;
@@ -79,14 +84,16 @@ int launch_itx_grouped(const void *const *blocks, const int32_t *n, void *coefs,
             const int mine = ((W == 64 || H == 64) ? 1 : 0) == big; \
             const int ctas = (mine && n[TX] > 0) ? (n[TX] + per_cta - 1) / per_cta : 0; \
             g.blocks[TX] = (const B200ItxBlock *)blocks[TX]; g.n[TX] = n[TX] > 0 ? n[TX] : 0; \
+            g.coffs[TX] = coffs ? coffs[TX] : nullptr; \
             g.cta_begin[TX] = total; total += ctas; g.cta_end[TX] = total; }
         B200_ITX_SIZES(X)
 #undef X
         if (!total) continue;
         if (int r = launch_hbd(bdmax, Launch::pdl, dim3(total), dim3(kItxWarps * 32), 0, stream, [&](auto hbd) {
                 typedef Bd<hbd> B;
-                return std::make_tuple(big ? itx_add_grouped_kernel<hbd, true> : itx_add_grouped_kernel<hbd, false>, g,
-                                       (typename B::coef *)coefs, (typename B::pixel *)pic, st[0], st[1], st[2], bdmax, zero);
+                auto kern = coffs ? (big ? itx_add_grouped_kernel<hbd, true, true> : itx_add_grouped_kernel<hbd, false, true>)
+                                  : (big ? itx_add_grouped_kernel<hbd, true, false> : itx_add_grouped_kernel<hbd, false, false>);
+                return std::make_tuple(kern, g, (typename B::coef *)coefs, (typename B::pixel *)pic, st[0], st[1], st[2], bdmax, zero);
             }))
             return r;
     }

@@ -14,6 +14,8 @@ namespace b200 {
 // Slot X_Y = X vertical, Y horizontal (reference src/levels.h:81-83, src/itx_tmpl.c:232-262).
 static __constant__ uint8_t c_tx_first[16]  = { 0, 0, 1, 1, 0, 2, 2, 2, 1, 3, 3, 0, 3, 1, 3, 2 };
 static __constant__ uint8_t c_tx_second[16] = { 0, 1, 0, 1, 2, 0, 2, 1, 2, 3, 0, 3, 1, 3, 2, 3 };
+// per TxfmType slot: dav1d_tx_type_class (reference src/tables.c): 0 2-D (scan of the size), 1 H_*, 2 V_*; WHT_WHT is 2-D
+static __constant__ uint8_t c_tx_class[16] = { 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 2, 1, 2, 1, 2, 1 };
 
 constexpr int kItxWarps = 4;
 
@@ -25,6 +27,8 @@ template <int W, int H> struct ItxGeom {
     static constexpr int P = W + 1;                       // tile pitch (words)
     static constexpr int SLOT = SH * P;                   // words per block tile
     static constexpr int LW = W == 4 ? 0 : W == 8 ? 1 : W == 16 ? 2 : W == 32 ? 3 : 4;
+    static constexpr int LSW = SW == 4 ? 2 : SW == 8 ? 3 : SW == 16 ? 4 : 5;    // log2 of the coded region's size
+    static constexpr int LSH = SH == 4 ? 2 : SH == 8 ? 3 : SH == 16 ? 4 : 5;
     static constexpr bool RECT2 = (W * 2 == H) || (H * 2 == W);
     // 64-wide blocks are shared by a pair of warps: one warp runs the row pass (32 coefficient rows), then each warp
     // takes 32 of the 64 picture columns of the column pass
@@ -86,11 +90,16 @@ __device__ __noinline__ void itx_col_pass_shared(const int *tcol, int pitch, typ
 }
 
 // the work of one CTA (`cta` = its index among the CTAs of this transform size); smem: kItxWarps * NB * SLOT words
-template <int W, int H, int TX, int SHIFT, bool HBD, bool SHARED = false>
+// COMPACT: `coefs` is the compact coefficient stream (per block the coefficients 0 .. eob in the scan order of its class,
+// include/b200av1.h B200CoefBlock) and block bi's first value is coefs[coffs[bi]]; blk.coef_off is not read. `scan` =
+// dav1d_scans[TX]. The block's coefficients are scattered into its own tile before pass 1, which then reads them from there.
+template <int W, int H, int TX, int SHIFT, bool HBD, bool SHARED = false, bool COMPACT = false>
 B200_DEV void itx_add_body(const int cta, int *const smem, const B200ItxBlock *__restrict__ blocks, int n_blocks,
                            typename Bd<HBD>::coef *__restrict__ coefs, typename Bd<HBD>::pixel *__restrict__ pic,
-                           int stride0, int stride1, int stride2, int bitdepth_max, int zero_coefs)
+                           int stride0, int stride1, int stride2, int bitdepth_max, int zero_coefs,
+                           const uint32_t *__restrict__ coffs = nullptr, const uint16_t *__restrict__ scan = nullptr)
 {
+    static_assert(!(SHARED && COMPACT), "the intra kernels read the dense coefficient plane");
     typedef ItxGeom<W, H> G;
     typedef typename Bd<HBD>::pixel pixel;
     typedef typename Bd<HBD>::coef coef;
@@ -108,7 +117,9 @@ B200_DEV void itx_add_body(const int cta, int *const smem, const B200ItxBlock *_
     if (valid) blk = blocks[bi];
     const int txtp = blk.txtp;
     const int eob = blk.eob;
-    coef *const cf = coefs + blk.coef_off;
+    uint32_t coff = blk.coef_off;
+    if constexpr (COMPACT) coff = valid ? coffs[bi] : 0;
+    coef *const cf = coefs + coff;
     const int stride = blk.plane == 0 ? stride0 : blk.plane == 1 ? stride1 : stride2;
     pixel *const dst = pic + blk.dst_off;
 
@@ -128,6 +139,44 @@ B200_DEV void itx_add_body(const int cta, int *const smem, const B200ItxBlock *_
     const int t_first = is_wht ? 0 : c_tx_first[txtp & 15];
     const int t_second = is_wht ? 0 : c_tx_second[txtp & 15];
 
+    // rows past this bound are zero by definition (reference src/itx_tmpl.c:86-105)
+    const auto last_row = [&]() {
+        if (t_second == TX1D_IDENTITY && t_first != TX1D_IDENTITY) return imin(G::SH - 1, eob);
+        if (t_first == TX1D_IDENTITY && t_second != TX1D_IDENTITY) return eob >> (G::LW + 2);
+        return (int)b200_lnz_col[b200_lnz_col_off[TX] + eob];
+    };
+
+    int dc = 0;
+    if constexpr (COMPACT) {
+        if (valid && dc_only) dc = (int)cf[0];
+        // Stage the coded region in the tile, coefficient (y, x) at t[y * P + x]: lane y of pass 1 then reads its row from
+        // where it writes it back (no lane reads another's row), and the odd pitch keeps those reads conflict-free. The rows
+        // pass 1 reads are cleared, then the block's group scatters cf[0 .. eob] through the scan of its class, the mapping
+        // of coef_expand_kernel (coef.cu). A dc-only block reads cf[0] (scan position 0 is coefficient 0) and stages nothing.
+        const bool stage = valid && !dc_only && half == 0;
+        if (stage && li < G::SH && li <= (is_wht ? G::SH - 1 : last_row())) {
+#pragma unroll
+            for (int x = 0; x < G::SW; x++) t[li * G::P + x] = 0;
+        }
+        __syncwarp();
+        if (stage) {
+            const int cls = is_wht ? 0 : c_tx_class[txtp & 15];
+            for (int k = li; k <= eob; k += G::L) {
+                int y, x;
+                if (cls == 0) {
+                    const int d = scan[k];
+                    y = d & (G::SH - 1); x = d >> G::LSH;
+                } else if (cls == 1) {
+                    y = k & (G::SH - 1); x = k >> G::LSH;
+                } else {
+                    y = k >> G::LSW; x = k & (G::SW - 1);
+                }
+                t[y * G::P + x] = (int)cf[k];
+            }
+        }
+        __syncwarp();
+    }
+
     // ---------------- pass 1: one lane per coefficient row ----------------
     if (valid && !dc_only && li < G::SH && half == 0) {
         const int y = li;
@@ -135,24 +184,20 @@ B200_DEV void itx_add_body(const int cta, int *const smem, const B200ItxBlock *_
         if (is_wht) {
             if constexpr (W == 4 && H == 4) {
 #pragma unroll
-                for (int x = 0; x < 4; x++) c[x] = (int)cf[y + x * 4] >> 2;
+                for (int x = 0; x < 4; x++) c[x] = (COMPACT ? t[y * G::P + x] : (int)cf[y + x * 4]) >> 2;
                 iwht4(c);
 #pragma unroll
                 for (int x = 0; x < 4; x++) t[y * G::P + x] = c[x];
             }
         } else {
-            // rows past this bound are zero by definition (reference src/itx_tmpl.c:86-105)
-            int last;
-            if (t_second == TX1D_IDENTITY && t_first != TX1D_IDENTITY) last = imin(G::SH - 1, eob);
-            else if (t_first == TX1D_IDENTITY && t_second != TX1D_IDENTITY) last = eob >> (G::LW + 2);
-            else last = b200_lnz_col[b200_lnz_col_off[TX] + eob];
+            const int last = last_row();
             if (SHARED && y <= last) {
                 itx_row_pass_shared<W, HBD>(cf + y, G::SH, t + y * G::P, G::RECT2, SHIFT, t_first, row_lo, row_hi, col_lo, col_hi);
             } else if (y <= last) {
 #pragma unroll
                 for (int x = 0; x < W; x++) {
                     if (x < G::SW) {
-                        const int v = (int)cf[y + x * G::SH];
+                        const int v = COMPACT ? t[y * G::P + x] : (int)cf[y + x * G::SH];
                         c[x] = G::RECT2 ? (int)((unsigned)v * 181u + 128u) >> 8 : v;
                     } else {
                         c[x] = 0;
@@ -167,15 +212,14 @@ B200_DEV void itx_add_body(const int cta, int *const smem, const B200ItxBlock *_
                 for (int x = 0; x < W; x++) t[y * G::P + x] = 0;
             }
         }
-        if (zero_coefs) {
+        if (!COMPACT && zero_coefs) {          // (the compact stream is read-only)
 #pragma unroll
             for (int x = 0; x < G::SW; x++) cf[y + x * G::SH] = 0;
         }
     }
-    int dc = 0;
-    if (valid && dc_only) dc = (int)cf[0];
+    if (!COMPACT && valid && dc_only) dc = (int)cf[0];
     if (G::PAIR) __syncthreads(); else __syncwarp();               // (every thread of the CTA runs this function)
-    if (valid && dc_only && zero_coefs && li == 0 && half == 0) cf[0] = 0;
+    if (!COMPACT && valid && dc_only && zero_coefs && li == 0 && half == 0) cf[0] = 0;
 
     // ---------------- pass 2: one lane per picture column ----------------
     if (valid) {

@@ -78,7 +78,7 @@ def band_plan(S, band_rows, compact=False, fused=False):
     order is kept inside a band), bands = list of dicts {y0, y1, last, <record list>: (first, count)} and need[k][ref] =
     (luma rows, chroma rows) of reference `ref` that band k's predictions read — the `lowest_pixel` of dav1d's
     check_tile (reference src/thread_task.c:415, src/decode.c lowest_pixel bookkeeping); expand = the compact coefficient
-    stream and its band-sorted B200CoefBlock records when `compact`. Intra records (S["intra_tx"]) are sorted by band too
+    stream, its band-sorted B200CoefBlock records and the per-size block offsets into it (itx_compact_offsets) when `compact`. Intra records (S["intra_tx"]) are sorted by band too
     (bands[k]["intra"]); see check_intra_bands for what they may read."""
     assert band_rows % 64 == 0 and band_rows > 0
     H, off, stride = S["H"], S["off"], S["stride"]
@@ -165,7 +165,7 @@ def band_plan(S, band_rows, compact=False, fused=False):
         assert len(eb) == len(ex)
         order = np.argsort(eb, kind="stable")
         cnt = np.bincount(eb, minlength=nb)
-        expand = (cc, ex[order])
+        expand = (cc, ex[order], itx_compact_offsets(S2, ex))
         ranges["expand"] = (np.concatenate([[0], np.cumsum(cnt)[:-1]]), cnt)
     bands = []
     for k in range(nb):
@@ -185,6 +185,22 @@ def band_plan(S, band_rows, compact=False, fused=False):
     ph = [H, (H + ssv[1]) >> ssv[1]]
     need[:, :, 0] = np.minimum(need[:, :, 0], ph[0]); need[:, :, 1] = np.minimum(need[:, :, 1], ph[1])
     return S2, bands, need, expand
+
+
+def itx_compact_offsets(S, ex):
+    """B200FrameJob.d_itx_coff: per transform size, where the coefficients of each block of S["itx"][tx] start in the compact
+    stream. synth.compact_coefs emits its B200CoefBlock records `ex` size after size, each in the order of S["itx"][tx]
+    (the coded intra records follow); that order is checked and kept, so a band's range of S["itx"][tx] indexes the
+    offsets too."""
+    out, pos = {}, 0
+    for tx in range(19):
+        a = S["itx"][tx]
+        if len(a):
+            r = ex[pos:pos + len(a)]
+            assert len(r) == len(a) and (r["tx"] == tx).all() and (r["dense_off"] == a["coef_off"]).all()
+            out[tx] = r["compact_off"].astype("<u4")
+            pos += len(a)
+    return out
 
 
 def check_intra_bands(S, tx, band, band_rows, nb):
@@ -325,13 +341,27 @@ class FrameBuffers:
                 j.d_itx[tx] = up("itx%d" % tx, a); j.n_itx[tx] = len(a)
                 self.uploads.append(("itx%d" % tx, a))
         if compact:
-            # the emitter ships coefficients 0 .. eob in scan order; the job zeroes + rebuilds the dense buffer
+            # the emitter ships coefficients 0 .. eob in scan order. Without intra records the inverse transforms read them
+            # in place through per-block offsets (B200FrameJob.d_itx_coff); with intra records, whose kernels read the dense
+            # buffer, the job zeroes + rebuilds it from the B200CoefBlock records. The dense buffer stays allocated either way
+            # (b200_itx_add_frame takes it).
             from . import synth
-            cc, ex = expand if expand is not None else synth.compact_coefs(S)
+            if expand is not None:
+                cc, ex, coffs = expand
+            else:
+                cc, ex = synth.compact_coefs(S)
+                coffs = itx_compact_offsets(S, ex)
             j.d_coef = zeros("coef", S["coefs"].nbytes)
             j.coef_bytes = S["coefs"].nbytes
             j.d_ccoef = up("ccoef", cc); self.uploads.append(("ccoef", cc))
-            if len(ex):
+            if (S.get("intra_tx") is None or not len(S["intra_tx"])) and coffs:
+                allo = np.concatenate([coffs[tx] for tx in sorted(coffs)])       # one upload, one pointer per size into it
+                base, pos = up("itx_coff", allo), 0
+                self.uploads.append(("itx_coff", allo))
+                for tx in sorted(coffs):
+                    j.d_itx_coff[tx] = base + 4 * pos
+                    pos += len(coffs[tx])
+            elif len(ex):
                 j.d_expand = up("expand", ex); j.n_expand = len(ex); self.uploads.append(("expand", ex))
         else:
             j.d_coef = up("coef", S["coefs"]); self.uploads.append(("coef", S["coefs"]))

@@ -633,6 +633,12 @@ typedef struct B200FrameJob {
      * stripe-boundary rows from (n_planes = 0: not needed). */
     int32_t run_resize, pad10;
     B200ResizeFrame resize[2];
+    /* compact transform input (optional): d_itx_coff[tx][i] = index in d_ccoef of the first coefficient of block d_itx[tx][i]
+     * (its coefficients 0 .. eob in the scan order of its class, as for B200CoefBlock). When d_ccoef is set, every size with
+     * blocks has offsets and the job has no intra records, the inverse transforms read d_ccoef directly: d_coef is neither
+     * zeroed nor expanded into (nor read, nor cleared by zero_coefs), and d_expand may be empty. Otherwise the offsets are
+     * ignored. */
+    const uint32_t *d_itx_coff[B200_N_RECT_TX_SIZES];
 } B200FrameJob;
 B200_API int b200_frame_run(const B200FrameJob *job, void *stream);
 /* n independent jobs of the same bit depth on one stream: reconstruction of every job, then ONE batched intra launch
