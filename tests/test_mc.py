@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 import refs
+from test_scaled_prediction import resize_params
 
 PAD = 8
 
@@ -238,11 +239,7 @@ def run_mc_checks(new, chk, bpc, seed, light=False, scaled=False, sections=None)
             src_w = 16 + int(rng.integers(0, 512 - 16 + 1))
             w_den = 9 + int(rng.integers(0, 8))
             dst_w = w_den * src_w >> 3
-            dx = ((src_w << 14) + (dst_w >> 1)) // dst_w
-            err = dst_w * dx - (src_w << 14)
-            num = -((dst_w - src_w) << 13) + (dst_w >> 1)
-            x0 = int(num / dst_w) + 128 - (err >> 1)   # C division truncates toward zero
-            mx0 = x0 & 0x3fff
+            dx, mx0 = resize_params(src_w, dst_w)
             hh = 8 if light else 64
             src = rng.integers(0, bd + 1, (hh, 512)).astype(dt)
             c1 = padded(hh, dst_w, dt, rng, bd); c2 = c1.copy()
