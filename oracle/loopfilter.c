@@ -17,9 +17,22 @@ static inline void SPX(void *p, int hbd, ptrdiff_t i, int v) {
     if (hbd) ((uint16_t *)p)[i] = (uint16_t)v; else ((uint8_t *)p)[i] = (uint8_t)v;
 }
 
+/* Branch counters for the tests (oracle_lf_branch_counts): per plane class (0 luma, 1 chroma) and direction
+ * (0 column edges, 1 row edges), the number of edge lines that took each branch of lf_segment. They only observe. */
+enum { LF_FM_FAIL, LF_NARROW_HEV, LF_NARROW, LF_FLAT6, LF_FLAT8, LF_FLAT8_OF16, LF_FLAT16, LF_NARROW_CLIP, LF_N_BRANCHES };
+static long lf_counts[2][2][LF_N_BRANCHES];
+
+/* copies the counters to out[2][2][LF_N_BRANCHES] (plane class, direction, branch) and resets them; returns the branch count */
+ORACLE_API int oracle_lf_branch_counts(long *out)
+{
+    if (out) memcpy(out, lf_counts, sizeof(lf_counts));
+    memset(lf_counts, 0, sizeof(lf_counts));
+    return LF_N_BRANCHES;
+}
+
 /* dst: pixel index base; sa = step between the 4 lines, sb = step across the edge (pixels) */
 static void lf_segment(void *pic, ptrdiff_t base, int E, int I, int H, ptrdiff_t sa, ptrdiff_t sb,
-                       int wd, int bdmax)
+                       int wd, int bdmax, long *cnt)
 {
     const int hbd = bdmax > 255;
     const int b8 = (o_ulog2((unsigned)bdmax) + 1) - 8;
@@ -37,7 +50,7 @@ static void lf_segment(void *pic, ptrdiff_t base, int E, int I, int H, ptrdiff_t
                  o_abs(p[0] - q[0]) * 2 + (o_abs(p[1] - q[1]) >> 1) <= E;
         if (wd > 4) fm &= o_abs(p[2] - p[1]) <= I && o_abs(q[2] - q[1]) <= I;
         if (wd > 6) fm &= o_abs(p[3] - p[2]) <= I && o_abs(q[3] - q[2]) <= I;
-        if (!fm) continue;
+        if (!fm) { cnt[LF_FM_FAIL]++; continue; }
 
         int flat8out = 0, flat8in = 0;
         if (wd >= 16)
@@ -50,6 +63,7 @@ static void lf_segment(void *pic, ptrdiff_t base, int E, int I, int H, ptrdiff_t
             flat8in &= o_abs(p[3] - p[0]) <= F && o_abs(q[3] - q[0]) <= F;
 
         if (wd >= 16 && (flat8out & flat8in)) {
+            cnt[LF_FLAT16]++;
             /* 13-tap smoothing: out(k) = (sum of a 13-wide window with replicated ends + 8) >> 4 */
             int s[14];   /* s[0..6] = p6..p0, s[7..13] = q0..q6 */
             for (int k = 0; k < 7; k++) { s[k] = p[6 - k]; s[7 + k] = q[k]; }
@@ -68,6 +82,7 @@ static void lf_segment(void *pic, ptrdiff_t base, int E, int I, int H, ptrdiff_t
                 SPX(pic, hbd, pos, sum >> 4);
             }
         } else if (wd >= 8 && flat8in) {
+            cnt[wd == 8 ? LF_FLAT8 : LF_FLAT8_OF16]++;
             const int p3 = p[3], p2 = p[2], p1 = p[1], p0 = p[0], q0 = q[0], q1 = q[1], q2 = q[2], q3 = q[3];
             SPX(pic, hbd, base - 3 * sb, (p3 + p3 + p3 + 2 * p2 + p1 + p0 + q0 + 4) >> 3);
             SPX(pic, hbd, base - 2 * sb, (p3 + p3 + p2 + 2 * p1 + p0 + q0 + q1 + 4) >> 3);
@@ -76,6 +91,7 @@ static void lf_segment(void *pic, ptrdiff_t base, int E, int I, int H, ptrdiff_t
             SPX(pic, hbd, base + 1 * sb, (p1 + p0 + q0 + 2 * q1 + q2 + q3 + q3 + 4) >> 3);
             SPX(pic, hbd, base + 2 * sb, (p0 + q0 + q1 + 2 * q2 + q3 + q3 + q3 + 4) >> 3);
         } else if (wd == 6 && flat8in) {
+            cnt[LF_FLAT6]++;
             const int p2 = p[2], p1 = p[1], p0 = p[0], q0 = q[0], q1 = q[1], q2 = q[2];
             SPX(pic, hbd, base - 2 * sb, (p2 + 2 * p2 + 2 * p1 + 2 * p0 + q0 + 4) >> 3);
             SPX(pic, hbd, base - 1 * sb, (p2 + 2 * p1 + 2 * p0 + 2 * q0 + q1 + 4) >> 3);
@@ -89,11 +105,15 @@ static void lf_segment(void *pic, ptrdiff_t base, int E, int I, int H, ptrdiff_t
             const int f1 = o_min(f + 4, hi) >> 3, f2 = o_min(f + 3, hi) >> 3;
             SPX(pic, hbd, base - sb, o_clip(p[0] + f2, 0, bdmax));
             SPX(pic, hbd, base, o_clip(q[0] - f1, 0, bdmax));
+            int clipped = p[0] + f2 < 0 || p[0] + f2 > bdmax || q[0] - f1 < 0 || q[0] - f1 > bdmax;
             if (!hev) {
                 const int g = (f1 + 1) >> 1;
                 SPX(pic, hbd, base - 2 * sb, o_clip(p[1] + g, 0, bdmax));
                 SPX(pic, hbd, base + sb, o_clip(q[1] - g, 0, bdmax));
+                clipped |= p[1] + g < 0 || p[1] + g > bdmax || q[1] - g < 0 || q[1] - g > bdmax;
             }
+            cnt[hev ? LF_NARROW_HEV : LF_NARROW]++;
+            cnt[LF_NARROW_CLIP] += clipped;
         }
     }
 }
@@ -117,8 +137,9 @@ ORACLE_API void oracle_loop_filter_sb(int plane_class, int dir, void *dst, ptrdi
         int wd;
         if (plane_class) wd = 4 + 2 * !!(mask[1] & bit);
         else wd = 4 << ((mask[2] & bit) ? 2 : !!(mask[1] & bit));
-        if (dir) lf_segment(dst, base, lut->e[L], lut->i[L], L >> 4, 1, ps, wd, bdmax);
-        else     lf_segment(dst, base, lut->e[L], lut->i[L], L >> 4, ps, 1, wd, bdmax);
+        long *const cnt = lf_counts[!!plane_class][!!dir];
+        if (dir) lf_segment(dst, base, lut->e[L], lut->i[L], L >> 4, 1, ps, wd, bdmax, cnt);
+        else     lf_segment(dst, base, lut->e[L], lut->i[L], L >> 4, ps, 1, wd, bdmax, cnt);
     }
 }
 
