@@ -24,6 +24,20 @@ static const int8_t cdef_dir_off[8][2][2] = {
     { { 1, 1 }, { 2, 2 } },   { { 1, 0 }, { 2, 1 } },  { { 1, 0 }, { 2, 0 } }, { { 1, 0 }, { 2, -1 } },
 };
 
+/* Branch counters for the tests (oracle_cdef_counts): per plane class (0 luma, 1 chroma), 8x8 blocks (4x4 / 4x8 in
+ * subsampled chroma) of oracle_cdef_frame by the way they were filtered, plus pixels and taps. They only observe. */
+enum { CD_SKIP_IDX, CD_SKIP_NOSKIP, CD_SKIP_ZERO, CD_PRI_SEC, CD_PRI, CD_SEC, CD_ADJ_ZERO, CD_ADJ_FULL, CD_SHIFT_CLAMP,
+       CD_DIR0, CD_EDGE_L = CD_DIR0 + 8, CD_EDGE_R, CD_EDGE_T, CD_EDGE_B, CD_CLAMP_PX, CD_TAP_DROPPED, CD_N };
+static long cd_counts[2][CD_N];
+
+/* copies the counters to out[2][CD_N] (plane class, counter) and resets them; returns CD_N */
+ORACLE_API int oracle_cdef_counts(long *out)
+{
+    if (out) memcpy(out, cd_counts, sizeof(cd_counts));
+    memset(cd_counts, 0, sizeof(cd_counts));
+    return CD_N;
+}
+
 static inline int constrain(int diff, int threshold, int shift) {
     const int adiff = o_abs(diff);
     const int v = o_min(adiff, o_max(0, threshold - (adiff >> shift)));
@@ -78,8 +92,10 @@ ORACLE_API int oracle_cdef_dir(const void *img, ptrdiff_t stride_bytes, unsigned
 typedef int (*sample_fn)(const void *ctx, int x, int y, int *v);
 
 static void cdef_block(void *dst, ptrdiff_t ps, int hbd, sample_fn get, const void *ctx, int pri, int sec,
-                       int dir, int damping, int w, int h, int bdmax)
+                       int dir, int damping, int w, int h, int bdmax, long *cnt)
 {
+    static long unused[CD_N];
+    if (!cnt) cnt = unused;
     const int b8 = (o_ulog2((unsigned)bdmax) + 1) - 8;
     const int pri_tap0 = 4 - ((pri >> b8) & 1);
     const int pri_shift = pri ? o_max(0, damping - o_ulog2((unsigned)pri)) : 0;
@@ -94,7 +110,9 @@ static void cdef_block(void *dst, ptrdiff_t ps, int hbd, sample_fn get, const vo
                     for (int s = -1; s <= 1; s += 2) {
                         int p;
                         if (!get(ctx, x + s * cdef_dir_off[dir][k][1], y + s * cdef_dir_off[dir][k][0], &p)) continue;
-                        sum += tap * constrain(p - px, pri, pri_shift);
+                        const int c = constrain(p - px, pri, pri_shift);
+                        cnt[CD_TAP_DROPPED] += p != px && !c;
+                        sum += tap * c;
                         mn = o_min(mn, p); mx = o_max(mx, p);
                     }
                 }
@@ -105,14 +123,19 @@ static void cdef_block(void *dst, ptrdiff_t ps, int hbd, sample_fn get, const vo
                         for (int s = -1; s <= 1; s += 2) {
                             int p;
                             if (!get(ctx, x + s * cdef_dir_off[d2][k][1], y + s * cdef_dir_off[d2][k][0], &p)) continue;
-                            sum += tap * constrain(p - px, sec, sec_shift);
+                            const int c = constrain(p - px, sec, sec_shift);
+                            cnt[CD_TAP_DROPPED] += p != px && !c;
+                            sum += tap * c;
                             mn = o_min(mn, p); mx = o_max(mx, p);
                         }
                     }
                 }
             }
             int v = px + ((sum - (sum < 0) + 8) >> 4);
-            if (pri && sec) v = o_clip(v, mn, mx);     /* only the combined filter clamps (:165) */
+            if (pri && sec) {                          /* only the combined filter clamps (:165) */
+                cnt[CD_CLAMP_PX] += v < mn || v > mx;
+                v = o_clip(v, mn, mx);
+            }
             SPX(dst, hbd, y * ps + x, v);
         }
 }
@@ -139,7 +162,7 @@ ORACLE_API void oracle_cdef_fb(void *dst, ptrdiff_t stride_bytes, const void *le
     c.dst = dst; c.left = left; c.top = top; c.bottom = bottom; c.w = w; c.h = h; c.edges = edges;
     for (int y = 0; y < h; y++)
         for (int x = 0; x < w; x++) SPX(c.copy, c.hbd, y * w + x, PX(dst, c.hbd, y * c.ps + x));
-    cdef_block(dst, c.ps, c.hbd, l1_get, &c, pri, sec, dir, damping, w, h, bdmax);
+    cdef_block(dst, c.ps, c.hbd, l1_get, &c, pri, sec, dir, damping, w, h, bdmax, NULL);
 }
 
 /* ---- whole frame, out of place ---- */
@@ -190,10 +213,11 @@ ORACLE_API void oracle_cdef_frame(int bdmax, const OracleCdefFrame *f)
             }
             const OracleAv1Filter *m = &f->mask[(by >> 5) * f->sb128w + (bx >> 5)];
             const int cdef_idx = m->cdef_idx[((by & 16) >> 3) + ((bx & 16) >> 4)];
-            if (cdef_idx == -1 || (!f->y_strength[cdef_idx] && !f->uv_strength[cdef_idx])) continue;
             const uint16_t *nr = m->noskip_mask[(by & 30) >> 1];
             const unsigned noskip = (unsigned)nr[1] << 16 | nr[0];
-            if (!(noskip & (3U << (bx & 30)))) continue;
+            const int skip = cdef_idx == -1 ? CD_SKIP_IDX : !f->y_strength[cdef_idx] && !f->uv_strength[cdef_idx] ? CD_SKIP_ZERO :
+                             !(noskip & (3U << (bx & 30))) ? CD_SKIP_NOSKIP : -1;
+            if (skip >= 0) { cd_counts[0][skip]++; cd_counts[1][skip] += 2; continue; }
             const int y_lvl = f->y_strength[cdef_idx], uv_lvl = f->uv_strength[cdef_idx];
             const int y_pri = (y_lvl >> 2) << b8;
             int y_sec = y_lvl & 3; y_sec += y_sec == 3; y_sec <<= b8;
@@ -209,8 +233,14 @@ ORACLE_API void oracle_cdef_frame(int bdmax, const OracleCdefFrame *f)
                 const int sh = pl ? ss_hor : 0, sv = pl ? ss_ver : 0;
                 const int w = 8 >> sh, h = 8 >> sv;
                 int pri, sec, d, damp;
+                long *const cnt = cd_counts[!!pl];
                 if (!pl) {
-                    if (y_pri) { pri = adjust_strength(y_pri, var); sec = y_sec; d = dir; if (!pri && !sec) continue; }
+                    if (y_pri) {
+                        pri = adjust_strength(y_pri, var); sec = y_sec; d = dir;
+                        cnt[CD_ADJ_ZERO] += !pri;
+                        cnt[CD_ADJ_FULL] += pri == y_pri;
+                        if (!pri && !sec) continue;
+                    }
                     else if (y_sec) { pri = 0; sec = y_sec; d = 0; }
                     else continue;
                     damp = damping;
@@ -218,13 +248,16 @@ ORACLE_API void oracle_cdef_frame(int bdmax, const OracleCdefFrame *f)
                     if (!uv_lvl) continue;
                     pri = uv_pri; sec = uv_sec; d = uv_pri ? uv_dir[dir] : 0; damp = damping - 1;
                 }
+                cnt[pri && sec ? CD_PRI_SEC : pri ? CD_PRI : CD_SEC]++;
+                if (pri) { cnt[CD_DIR0 + d]++; cnt[CD_SHIFT_CLAMP] += damp < o_ulog2((unsigned)pri); }
+                cnt[CD_EDGE_L] += !have_l; cnt[CD_EDGE_R] += !have_r; cnt[CD_EDGE_T] += !have_t; cnt[CD_EDGE_B] += !have_b;
                 FrCtx c;
                 c.base = (const uint8_t *)f->src + (size_t)f->plane_off[pl] * px; c.ps = f->stride[pl]; c.hbd = hbd;
                 c.x0 = bx * 4 >> sh; c.y0 = by * 4 >> sv;
                 c.xmin = c.x0 - 2 * have_l; c.xmax = c.x0 + w + 2 * have_r;
                 c.ymin = c.y0 - 2 * have_t; c.ymax = c.y0 + h + 2 * have_b;
                 uint8_t *d8 = (uint8_t *)f->dst + ((size_t)f->plane_off[pl] + (size_t)c.y0 * f->stride[pl] + c.x0) * px;
-                cdef_block(d8, f->stride[pl], hbd, fr_get, &c, pri, sec, d, damp, w, h, bdmax);
+                cdef_block(d8, f->stride[pl], hbd, fr_get, &c, pri, sec, d, damp, w, h, bdmax, cnt);
             }
         }
 }

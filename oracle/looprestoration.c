@@ -17,6 +17,23 @@
 #include "tables_gen.h"
 #include <stdlib.h>
 
+/* Branch counters for the tests (oracle_lr_counts): per plane class (0 luma, 1 chroma), the restoration units of
+ * oracle_lr_frame by filter (one per unit and stripe), the stripes by their edges and unit row, and the samples that took
+ * a clip or clamp. The filters count into the class of the plane oracle_lr_frame is restoring (luma for direct calls).
+ * They only observe. */
+enum { LR_NONE, LR_WIENER, LR_SGR5, LR_SGR3, LR_SGR_MIX, LR_EXT_H, LR_PULLED_UP, LR_HOR_CLIP_LO, LR_HOR_CLIP_HI,
+       LR_OUT_CLIP_LO, LR_OUT_CLIP_HI, LR_Z0, LR_Z255, LR_SGR_BIG, LR_TOP, LR_NO_TOP, LR_BOT, LR_NO_BOT, LR_BOT_CLAMP, LR_N };
+static long lr_counts[2][LR_N];
+static int lr_cls;
+
+/* copies the counters to out[2][LR_N] (plane class, counter) and resets them; returns LR_N */
+ORACLE_API int oracle_lr_counts(long *out)
+{
+    if (out) memcpy(out, lr_counts, sizeof(lr_counts));
+    memset(lr_counts, 0, sizeof(lr_counts));
+    return LR_N;
+}
+
 typedef struct {
     const void *p, *left, *lpf;
     ptrdiff_t ps;
@@ -68,13 +85,19 @@ ORACLE_API void oracle_wiener(void *p, ptrdiff_t stride_bytes, const void *left,
             int sum = 1 << (bitdepth + 6);
             if (!hbd) sum += lr_S(&s, x, y) * 128;
             for (int i = 0; i < 7; i++) sum += lr_S(&s, x + i - 3, y) * filter[0][i];
-            hor[(size_t)(y + 3) * w + x] = (uint16_t)o_clip((sum + (1 << (rbh - 1))) >> rbh, 0, clip_limit - 1);
+            const int v = (sum + (1 << (rbh - 1))) >> rbh;
+            lr_counts[lr_cls][LR_HOR_CLIP_LO] += v < 0;
+            lr_counts[lr_cls][LR_HOR_CLIP_HI] += v > clip_limit - 1;
+            hor[(size_t)(y + 3) * w + x] = (uint16_t)o_clip(v, 0, clip_limit - 1);
         }
     for (int y = 0; y < h; y++)
         for (int x = 0; x < w; x++) {
             int sum = -round_offset;
             for (int k = 0; k < 7; k++) sum += hor[(size_t)(y + k) * w + x] * filter[1][k];
-            st_px(p, hbd, y * s.ps + x, o_clip((sum + (1 << (rbv - 1))) >> rbv, 0, bdmax));
+            const int v = (sum + (1 << (rbv - 1))) >> rbv;
+            lr_counts[lr_cls][LR_OUT_CLIP_LO] += v < 0;
+            lr_counts[lr_cls][LR_OUT_CLIP_HI] += v > bdmax;
+            st_px(p, hbd, y * s.ps + x, o_clip(v, 0, bdmax));
         }
     free(hor);
 }
@@ -98,6 +121,9 @@ static void sgr_ab(const LrSrc *s, int r, unsigned strength, int bdmax, int32_t 
             const unsigned p = (unsigned)o_max(a * n - b * b, 0);
             const unsigned z = (p * strength + (1 << 19)) >> 20;
             const unsigned xx = b200_sgr_x_by_x[z < 255 ? z : 255];
+            lr_counts[lr_cls][LR_Z0] += z == 0;
+            lr_counts[lr_cls][LR_Z255] += z >= 255;
+            lr_counts[lr_cls][LR_SGR_BIG] += xx * (unsigned)sum * (unsigned)one_by_x >= 0x80000000u;   /* past the int32 range */
             A[(y + 1) * (w + 2) + x + 1] = (int32_t)((xx * (unsigned)sum * (unsigned)one_by_x + (1 << 11)) >> 12);
             B[(y + 1) * (w + 2) + x + 1] = (int32_t)xx;
         }
@@ -141,7 +167,10 @@ ORACLE_API void oracle_sgr(int mode, void *p, ptrdiff_t stride_bytes, const void
                 t3 = (b - a * src + (1 << 8)) >> 9;
             }
             const int v = mode == 0 ? w0 * t5 : mode == 1 ? w1 * t3 : w0 * t5 + w1 * t3;
-            st_px(out, hbd, (ptrdiff_t)y * w + x, o_clip(src + ((v + (1 << 10)) >> 11), 0, bdmax));
+            const int o = src + ((v + (1 << 10)) >> 11);
+            lr_counts[lr_cls][LR_OUT_CLIP_LO] += o < 0;
+            lr_counts[lr_cls][LR_OUT_CLIP_HI] += o > bdmax;
+            st_px(out, hbd, (ptrdiff_t)y * w + x, o_clip(o, 0, bdmax));
         }
     for (int y = 0; y < h; y++)
         memcpy((uint8_t *)p + (ptrdiff_t)y * stride_bytes, out + (size_t)y * w * (hbd ? 2 : 1), (size_t)w * (hbd ? 2 : 1));
@@ -180,6 +209,7 @@ ORACLE_API void oracle_lr_frame(int bdmax, const OracleLrFrame *f)
         if (!(f->restore_planes & (1 << pl))) continue;
         const int us_log2 = f->unit_size_log2[!!pl], unit = 1 << us_log2, half = unit >> 1, max_unit = unit + half;
         const int shift_hor = 7 - ssh;
+        long *const cnt = lr_counts[lr_cls = !!pl];
         uint8_t *lpf = malloc((size_t)8 * sb), *left = malloc(64 * 4 * px), *work = malloc((size_t)64 * sb);
         for (int y0 = 0, k = 0; y0 < h; k++) {
             const int y1 = o_min(h, ((64 * (k + 1) - 8) >> ssv));
@@ -188,10 +218,13 @@ ORACLE_API void oracle_lr_frame(int bdmax, const OracleLrFrame *f)
             const int sby = ((y0 << ssv) + (y0 ? 8 : 0)) >> (6 + f->sb128);
             const int row_y = (sby << (6 + f->sb128)) >> ssv;
             int aligned = row_y & ~(unit - 1);
-            if (aligned && aligned + half > h) aligned -= unit;
+            if (aligned && aligned + half > h) { aligned -= unit; cnt[LR_PULLED_UP]++; }
             aligned <<= ssv;
             const int sb_idx = (aligned >> 7) * f->sr_sb128w, unit_idx = ((aligned >> 6) & 1) << 1;
             int edges = (y0 > 0 ? 4 : 0) | (y1 < h ? 8 : 0);
+            cnt[y0 > 0 ? LR_TOP : LR_NO_TOP]++;
+            cnt[y1 < h ? LR_BOT : LR_NO_BOT]++;
+            cnt[LR_BOT_CLAMP] += y1 < h && y1 + 1 > h - 1;
             /* rows above / below the stripe from the deblocked picture (8-row lpf layout: 0,1 above, 6,7 below) */
             for (int i = 0; i < 2; i++) {
                 memcpy(lpf + i * sb, D + (ptrdiff_t)o_max(y0 - 2 + i, 0) * sb, (size_t)sb);
@@ -201,6 +234,9 @@ ORACLE_API void oracle_lr_frame(int bdmax, const OracleLrFrame *f)
                 const int last = !(x + max_unit <= w);
                 const int uw = last ? w - x : unit;
                 const OracleLrUnit *u = &f->lr_mask[sb_idx + (x >> shift_hor)].lr[pl][unit_idx + ((x >> (shift_hor - 1)) & 1)];
+                const int s0 = u->type >= 3 && b200_sgr_params[u->type - 3][0], s1 = u->type >= 3 && b200_sgr_params[u->type - 3][1];
+                cnt[!u->type ? LR_NONE : u->type == 2 ? LR_WIENER : s0 && s1 ? LR_SGR_MIX : s0 ? LR_SGR5 : LR_SGR3]++;
+                cnt[LR_EXT_H] += uw > unit;
                 if (u->type) {
                     const int e = edges | (x > 0 ? 1 : 0) | (last ? 0 : 2);
                     /* working copy of the stripe rows of this unit plus its right neighbourhood, pre-LR */
@@ -234,4 +270,5 @@ ORACLE_API void oracle_lr_frame(int bdmax, const OracleLrFrame *f)
         }
         free(lpf); free(left); free(work);
     }
+    lr_cls = 0;
 }
