@@ -31,6 +31,40 @@ static inline void SPX(void *p, int hbd, ptrdiff_t i, int v) {
 }
 #define PSTRIDE(bytes, hbd) ((hbd) ? (bytes) / 2 : (bytes))
 
+/* Coverage counters for the tests (oracle_mc_counts) over the unscaled put / prep and w_mask: they only observe.
+ * PREP_MAX_* hold the largest |prep| value before the bias is removed, per bit depth (8 / 10 / 12); the tap counts
+ * are per prediction and axis: a 4-tap or 8-tap set (w or h <= 4 selects the 4-tap one), or no phase on the axis. */
+enum { MC_PUT_CLIP_LO, MC_PUT_CLIP_HI, MC_PREP_MAX_8, MC_PREP_MAX_10, MC_PREP_MAX_12, MC_WMASK_38, MC_WMASK_64,
+       MC_H_4TAP, MC_H_8TAP, MC_V_4TAP, MC_V_8TAP, MC_H_IDENTITY, MC_V_IDENTITY, MC_N_COUNTS };
+static long mc_counts[MC_N_COUNTS];
+
+/* copies the counters to out[MC_N_COUNTS] and resets them; returns MC_N_COUNTS */
+ORACLE_API int oracle_mc_counts(long *out)
+{
+    if (out) memcpy(out, mc_counts, sizeof(mc_counts));
+    memset(mc_counts, 0, sizeof(mc_counts));
+    return MC_N_COUNTS;
+}
+/* a put output: counted when the clip changes it */
+static inline int put_clip(int v, int bdmax)
+{
+    if (v < 0) mc_counts[MC_PUT_CLIP_LO]++;
+    else if (v > bdmax) mc_counts[MC_PUT_CLIP_HI]++;
+    return o_clip(v, 0, bdmax);
+}
+/* a prep output before the bias is removed */
+static inline int prep_out(int v, BdInfo b)
+{
+    long *const m = &mc_counts[MC_PREP_MAX_8 + (b.bdmax > 255) + (b.bdmax > 1023)];
+    if (o_abs(v) > *m) *m = o_abs(v);
+    return v - b.bias;
+}
+static void count_taps(int mx, int my, int w, int h, int bilin)
+{
+    if (!mx) mc_counts[MC_H_IDENTITY]++; else if (!bilin) mc_counts[w > 4 ? MC_H_8TAP : MC_H_4TAP]++;
+    if (!my) mc_counts[MC_V_IDENTITY]++; else if (!bilin) mc_counts[h > 4 ? MC_V_8TAP : MC_V_4TAP]++;
+}
+
 /* enum Filter2d -> (horizontal, vertical) Dav1dFilterMode; reference src/levels.h:184-196,
  * src/mc_tmpl.c:406-414 */
 static const uint8_t f2d_h[9] = { 0, 0, 0, 2, 2, 2, 1, 1, 1 };
@@ -69,6 +103,7 @@ static void mc_8tap(int op, void *out, ptrdiff_t out_stride, const void *src, pt
     const int8_t *fh = h_filter(f2d, mx, w), *fv = v_filter(f2d, my, h);
     int16_t *tmp = (int16_t *)out;
     static __thread int16_t mid[128 * 135];
+    count_taps(mx, my, w, h, 0);
 
     if (fh && fv) {
         for (int y = 0; y < h + 7; y++)
@@ -77,29 +112,29 @@ static void mc_8tap(int op, void *out, ptrdiff_t out_stride, const void *src, pt
         for (int y = 0; y < h; y++)
             for (int x = 0; x < w; x++) {
                 const int s = tap8_mid(mid + (y + 3) * 128, x, fv, 128);
-                if (op) tmp[y * ds + x] = (int16_t)(RND(s, 6) - b.bias);
-                else SPX(out, hbd, y * ds + x, o_clip(RND(s, 6 + ib), 0, bdmax));
+                if (op) tmp[y * ds + x] = (int16_t)prep_out(RND(s, 6), b);
+                else SPX(out, hbd, y * ds + x, put_clip(RND(s, 6 + ib), bdmax));
             }
     } else if (fh) {
         const int irnd = 32 + ((1 << (6 - ib)) >> 1);
         for (int y = 0; y < h; y++)
             for (int x = 0; x < w; x++) {
                 const int s = tap8_px(src, hbd, y * ss + x, fh, 1);
-                if (op) tmp[y * ds + x] = (int16_t)(RND(s, 6 - ib) - b.bias);
-                else SPX(out, hbd, y * ds + x, o_clip((s + irnd) >> 6, 0, bdmax));
+                if (op) tmp[y * ds + x] = (int16_t)prep_out(RND(s, 6 - ib), b);
+                else SPX(out, hbd, y * ds + x, put_clip((s + irnd) >> 6, bdmax));
             }
     } else if (fv) {
         for (int y = 0; y < h; y++)
             for (int x = 0; x < w; x++) {
                 const int s = tap8_px(src, hbd, y * ss + x, fv, ss);
-                if (op) tmp[y * ds + x] = (int16_t)(RND(s, 6 - ib) - b.bias);
-                else SPX(out, hbd, y * ds + x, o_clip(RND(s, 6), 0, bdmax));
+                if (op) tmp[y * ds + x] = (int16_t)prep_out(RND(s, 6 - ib), b);
+                else SPX(out, hbd, y * ds + x, put_clip(RND(s, 6), bdmax));
             }
     } else {
         for (int y = 0; y < h; y++)
             for (int x = 0; x < w; x++) {
                 const int p = PX(src, hbd, y * ss + x);
-                if (op) tmp[y * ds + x] = (int16_t)((p << ib) - b.bias);
+                if (op) tmp[y * ds + x] = (int16_t)prep_out(p << ib, b);
                 else SPX(out, hbd, y * ds + x, p);
             }
     }
@@ -113,6 +148,7 @@ static void mc_bilin(int op, void *out, ptrdiff_t out_stride, const void *src, p
     const ptrdiff_t ss = PSTRIDE(src_stride, hbd), ds = op ? w : PSTRIDE(out_stride, hbd);
     int16_t *tmp = (int16_t *)out;
     static __thread int16_t mid[128 * 129];
+    count_taps(mx, my, w, h, 1);
 #define BIL(a, bb, m) (16 * (a) + (m) * ((bb) - (a)))
     if (mx && my) {
         for (int y = 0; y < h + 1; y++)
@@ -121,29 +157,29 @@ static void mc_bilin(int op, void *out, ptrdiff_t out_stride, const void *src, p
         for (int y = 0; y < h; y++)
             for (int x = 0; x < w; x++) {
                 const int s = BIL(mid[y * 128 + x], mid[(y + 1) * 128 + x], my);
-                if (op) tmp[y * ds + x] = (int16_t)(RND(s, 4) - b.bias);
-                else SPX(out, hbd, y * ds + x, o_clip(RND(s, 4 + ib), 0, bdmax));
+                if (op) tmp[y * ds + x] = (int16_t)prep_out(RND(s, 4), b);
+                else SPX(out, hbd, y * ds + x, put_clip(RND(s, 4 + ib), bdmax));
             }
     } else if (mx) {
         const int irnd = (1 << ib) >> 1;
         for (int y = 0; y < h; y++)
             for (int x = 0; x < w; x++) {
                 const int px = RND(BIL(PX(src, hbd, y * ss + x), PX(src, hbd, y * ss + x + 1), mx), 4 - ib);
-                if (op) tmp[y * ds + x] = (int16_t)(px - b.bias);
-                else SPX(out, hbd, y * ds + x, o_clip((px + irnd) >> ib, 0, bdmax));
+                if (op) tmp[y * ds + x] = (int16_t)prep_out(px, b);
+                else SPX(out, hbd, y * ds + x, put_clip((px + irnd) >> ib, bdmax));
             }
     } else if (my) {
         for (int y = 0; y < h; y++)
             for (int x = 0; x < w; x++) {
                 const int s = BIL(PX(src, hbd, y * ss + x), PX(src, hbd, (y + 1) * ss + x), my);
-                if (op) tmp[y * ds + x] = (int16_t)(RND(s, 4 - ib) - b.bias);
-                else SPX(out, hbd, y * ds + x, o_clip(RND(s, 4), 0, bdmax));
+                if (op) tmp[y * ds + x] = (int16_t)prep_out(RND(s, 4 - ib), b);
+                else SPX(out, hbd, y * ds + x, put_clip(RND(s, 4), bdmax));
             }
     } else {
         for (int y = 0; y < h; y++)
             for (int x = 0; x < w; x++) {
                 const int p = PX(src, hbd, y * ss + x);
-                if (op) tmp[y * ds + x] = (int16_t)((p << ib) - b.bias);
+                if (op) tmp[y * ds + x] = (int16_t)prep_out(p << ib, b);
                 else SPX(out, hbd, y * ds + x, p);
             }
     }
@@ -281,11 +317,13 @@ ORACLE_API void oracle_w_mask(void *dst, ptrdiff_t dst_stride, const int16_t *t1
         for (int x = 0; x < w; x++) {
             const int d = t1[y * w + x] - t2[y * w + x];
             const int m = o_min(38 + ((o_abs(d) + mask_rnd) >> mask_sh), 64);
+            mc_counts[MC_WMASK_38] += m == 38; mc_counts[MC_WMASK_64] += m == 64;
             SPX(dst, b.hbd, y * ds + x, o_clip((d * m + t2[y * w + x] * 64 + rnd) >> sh, 0, bdmax));
             if (!ss_hor) { mrow[x] = (uint8_t)m; continue; }
             x++;
             const int d2 = t1[y * w + x] - t2[y * w + x];
             const int n = o_min(38 + ((o_abs(d2) + mask_rnd) >> mask_sh), 64);
+            mc_counts[MC_WMASK_38] += n == 38; mc_counts[MC_WMASK_64] += n == 64;
             SPX(dst, b.hbd, y * ds + x, o_clip((d2 * n + t2[y * w + x] * 64 + rnd) >> sh, 0, bdmax));
             if (ss_ver && (y & 1)) mrow[x >> 1] = (uint8_t)((m + n + mrow[x >> 1] + 2 - sign) >> 2);
             else if (ss_ver)       mrow[x >> 1] = (uint8_t)(m + n);
