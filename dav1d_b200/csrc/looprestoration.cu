@@ -1,8 +1,9 @@
 // Loop restoration (dav1d Dav1dLoopRestorationDSPContext; reference src/looprestoration_tmpl.c,
 // driver src/lr_apply_tmpl.c, stripe-border rows src/lf_apply_tmpl.c:40-174).
 //
-// Frame-wide and out of place. A CTA restores one tile (<= 64 x 32) that lies inside one 64-row
-// stripe and one restoration unit:
+// Frame-wide and out of place. A CTA of 256 threads restores one tile (<= 64 x 32) that lies inside one 64-row stripe
+// and one restoration unit, or, where a plane's units are 32 wide (4:2:0 / 4:2:2 chroma), the U and the V tile at the
+// same place on 128 threads each:
 //   1. the tile plus a 3-sample halo of the *virtual source* is staged in shared memory: rows inside
 //      the stripe come from the post-CDEF picture, the two rows above / below the stripe from the
 //      post-deblock picture (third row repeated), columns are clamped at the picture edges — the same
@@ -12,42 +13,62 @@
 //      sums -> output (5x5 at half vertical rate, exactly like sgr_finish_filter2).
 // The Level-1 entry points run the same tile code over a host-assembled window.
 #include "host_util.h"
-#define B200_TBL __constant__
+// the tables live in global memory: x_by_x is copied into shared memory per CTA, the sgr parameters are read once per tile
+#define B200_TBL __device__
 #include "tables_gen.h"
 
 namespace b200 {
 
-constexpr int kTW = 64, kTH = 32, kSW = kTW + 6, kSH = kTH + 6;
+constexpr int kTW = 64, kTH = 32, kSH = kTH + 6;
 
 struct LrTileParams {
     int type;             // 0 none, 1 wiener, 2 sgr
     int fh[7], fv[7];     // wiener taps (fh[3] without the 8-bit +128 split: added from the centre sample)
     unsigned s0, s1; int w0, w1;   // sgr
+    ptrdiff_t out; int st;   // lr_frame_kernel: the tile's first output sample (in samples from B200LrFrame::dst), pitch
 };
 
-struct LrShared {
-    uint16_t src[kSH][kSW + 2];
+// the shared layout of one tile at most TW wide; a 32-wide one is half the size of a 64-wide one, so a U / V pair of
+// them overlays one 64-wide tile
+template <int TW> struct LrShared {
+    static constexpr int SW = TW + 6;
+    LrTileParams P;       // lr_frame_kernel: the tile's parameters (at the tile's own base: one address register per half)
+    uint16_t src[kSH][SW + 2];
     union {
-        uint16_t hor[kSH][kTW];
+        uint16_t hor[kSH][TW];
         struct {
-            int A3[kTH + 2][kTW + 2]; uint16_t B3[kTH + 2][kTW + 2];
-            int A5[kTH / 2 + 2][kTW + 2]; uint16_t B5[kTH / 2 + 2][kTW + 2];
+            int A3[kTH + 2][TW + 2]; uint16_t B3[kTH + 2][TW + 2];
+            int A5[kTH / 2 + 2][TW + 2]; uint16_t B5[kTH / 2 + 2][TW + 2];
         } s;
     } u;
 };
+constexpr size_t kLrSmem = sizeof(LrShared<kTW>) > 2 * sizeof(LrShared<32>) ? sizeof(LrShared<kTW>) : 2 * sizeof(LrShared<32>);
 
-// everything after the source tile is staged: tw x th outputs, tile-relative row parity r0 (even)
-template <bool HBD, class Store>
-B200_DEV void lr_tile_compute(LrShared &sm, const LrTileParams &P, int tw, int th, int bdmax, Store store)
+// b200_sgr_x_by_x as 64 words in shared memory: the self-guided passes index it per lane, which a constant-bank load
+// would serialise into one replay per distinct index; a shared byte table costs at most a 2-way bank conflict
+B200_DEV void lr_stage_x_by_x(unsigned *tbl)
 {
-    const int tid = threadIdx.x, nt = blockDim.x;
+    const int i = threadIdx.x;
+    if (i < 64)
+        tbl[i] = (unsigned)b200_sgr_x_by_x[4 * i] | (unsigned)b200_sgr_x_by_x[4 * i + 1] << 8 |
+                 (unsigned)b200_sgr_x_by_x[4 * i + 2] << 16 | (unsigned)b200_sgr_x_by_x[4 * i + 3] << 24;
+}
+
+// The two compute passes of a staged tile on threads tid = 0 .. nt - 1; the caller puts one barrier between them, so
+// both tiles of a pair (and every tile type) run one barrier schedule.
+// pass 1: Wiener rows into u.hor, or the self-guided (a, b) surfaces
+template <bool HBD, int TW>
+B200_DEV void lr_tile_pass1(LrShared<TW> &sm, const LrTileParams &P, const unsigned *tbl, int tw, int th, int bdmax,
+                            int tid, int nt)
+{
     const int bitdepth = HBD ? 32 - __clz(bdmax) : 8;
+    const uint8_t *x_by_x = (const uint8_t *)tbl;
     if (P.type == 1) {
-        const int rbh = 3 + (bitdepth == 12) * 2, rbv = 11 - (bitdepth == 12) * 2;
+        const int rbh = 3 + (bitdepth == 12) * 2;
         const int clip_limit = 1 << (bitdepth + 1 + 7 - rbh);
         // horizontal: 4 consecutive outputs per thread share their 10 source samples
-        for (int i = tid; i < (th + 6) * (kTW / 4); i += nt) {
-            const int y = i / (kTW / 4), x = (i - y * (kTW / 4)) * 4;
+        for (int i = tid; i < (th + 6) * (TW / 4); i += nt) {
+            const int y = i / (TW / 4), x = (i - y * (TW / 4)) * 4;
             if (x >= tw) continue;
             int v[10];
 #pragma unroll
@@ -61,31 +82,13 @@ B200_DEV void lr_tile_compute(LrShared &sm, const LrTileParams &P, int tw, int t
                 sm.u.hor[y][x + j] = (uint16_t)iclip((sum + (1 << (rbh - 1))) >> rbh, 0, clip_limit - 1);
             }
         }
-        __syncthreads();
-        // vertical: 4 consecutive rows per thread share their 10 intermediate samples
-        const int round_offset = 1 << (bitdepth + (rbv - 1));
-        for (int i = tid; i < ((th + 3) / 4) * kTW; i += nt) {
-            const int yq = i / kTW, x = i - yq * kTW, y = yq * 4;
-            if (x >= tw) continue;
-            int v[10];
-#pragma unroll
-            for (int k = 0; k < 10; k++) v[k] = y + k < th + 6 ? (int)sm.u.hor[y + k][x] : 0;
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                if (y + j >= th) break;
-                int sum = -round_offset;
-#pragma unroll
-                for (int k = 0; k < 7; k++) sum += v[j + k] * P.fv[k];
-                store(x, y + j, iclip((sum + (1 << (rbv - 1))) >> rbv, 0, bdmax));
-            }
-        }
         return;
     }
     // ---- self-guided ----
     const int b8 = bitdepth - 8;
+    constexpr int NS = (TW + 2 + 3) / 4;
     if (P.s1) {      // 3x3 surfaces at rows -1 .. th, cols -1 .. tw
         // 4 consecutive surface points per thread: 3 x 6 source samples -> column sums -> sliding 3-wide sums
-        constexpr int NS = (kTW + 2 + 3) / 4;
         for (int i = tid; i < (th + 2) * NS; i += nt) {
             const int yy = i / NS, xx = (i - yy * NS) * 4;           // surface index; source centre (xx + 2, yy + 2)
             if (xx >= tw + 2) continue;
@@ -103,7 +106,7 @@ B200_DEV void lr_tile_compute(LrShared &sm, const LrTileParams &P, int tw, int t
                 const int b = (sum + ((1 << b8) >> 1)) >> b8;
                 const unsigned p = (unsigned)imax(a * 9 - b * b, 0);
                 const unsigned z = (p * P.s1 + (1u << 19)) >> 20;
-                const unsigned x = b200_sgr_x_by_x[z < 255u ? z : 255u];
+                const unsigned x = x_by_x[z < 255u ? z : 255u];
                 sm.u.s.A3[yy][xx + k] = (int)((x * (unsigned)sum * 455u + (1u << 11)) >> 12);
                 sm.u.s.B3[yy][xx + k] = (uint16_t)x;
             }
@@ -111,7 +114,6 @@ B200_DEV void lr_tile_compute(LrShared &sm, const LrTileParams &P, int tw, int t
     }
     if (P.s0) {      // 5x5 surfaces at odd rows -1, 1, 3, ... (index j <-> row 2j - 1)
         const int nrow = (th + 1) / 2 + 1;
-        constexpr int NS = (kTW + 2 + 3) / 4;
         for (int i = tid; i < nrow * NS; i += nt) {
             const int j = i / NS, xx = (i - j * NS) * 4;
             if (xx >= tw + 2) continue;
@@ -133,16 +135,43 @@ B200_DEV void lr_tile_compute(LrShared &sm, const LrTileParams &P, int tw, int t
                 const int b = (sum + ((1 << b8) >> 1)) >> b8;
                 const unsigned p = (unsigned)imax(a * 25 - b * b, 0);
                 const unsigned z = (p * P.s0 + (1u << 19)) >> 20;
-                const unsigned x = b200_sgr_x_by_x[z < 255u ? z : 255u];
+                const unsigned x = x_by_x[z < 255u ? z : 255u];
                 sm.u.s.A5[j][xx + k] = (int)((x * (unsigned)sum * 164u + (1u << 11)) >> 12);
                 sm.u.s.B5[j][xx + k] = (uint16_t)x;
             }
         }
     }
-    __syncthreads();
+}
+
+// pass 2: Wiener columns, or the self-guided output; tw x th outputs
+template <bool HBD, int TW, class Store>
+B200_DEV void lr_tile_pass2(LrShared<TW> &sm, const LrTileParams &P, int tw, int th, int bdmax, int tid, int nt, Store store)
+{
+    const int bitdepth = HBD ? 32 - __clz(bdmax) : 8;
+    if (P.type == 1) {
+        const int rbv = 11 - (bitdepth == 12) * 2;
+        // vertical: 4 consecutive rows per thread share their 10 intermediate samples
+        const int round_offset = 1 << (bitdepth + (rbv - 1));
+        for (int i = tid; i < ((th + 3) / 4) * TW; i += nt) {
+            const int yq = i / TW, x = i - yq * TW, y = yq * 4;
+            if (x >= tw) continue;
+            int v[10];
+#pragma unroll
+            for (int k = 0; k < 10; k++) v[k] = y + k < th + 6 ? (int)sm.u.hor[y + k][x] : 0;
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                if (y + j >= th) break;
+                int sum = -round_offset;
+#pragma unroll
+                for (int k = 0; k < 7; k++) sum += v[j + k] * P.fv[k];
+                store(x, y + j, iclip((sum + (1 << (rbv - 1))) >> rbv, 0, bdmax));
+            }
+        }
+        return;
+    }
     // 4 consecutive pixels of a row per thread: the neighbourhood sums are built from per-column partial sums
-    for (int i = tid; i < th * (kTW / 4); i += nt) {
-        const int y = i / (kTW / 4), x = (i - y * (kTW / 4)) * 4;
+    for (int i = tid; i < th * (TW / 4); i += nt) {
+        const int y = i / (TW / 4), x = (i - y * (TW / 4)) * 4;
         if (x >= tw) continue;
         int t5a[4] = { 0, 0, 0, 0 }, t5b[4] = { 0, 0, 0, 0 }, t3a[4] = { 0, 0, 0, 0 }, t3b[4] = { 0, 0, 0, 0 };
         if (P.s0) {
@@ -187,7 +216,7 @@ B200_DEV void lr_tile_compute(LrShared &sm, const LrTileParams &P, int tw, int t
     }
 }
 
-// where lr_tile_compute writes: sample (x, y) of the tile, or 4 consecutive samples of a row of which the first n are inside
+// where lr_tile_pass2 writes: sample (x, y) of the tile, or 4 consecutive samples of a row of which the first n are inside
 template <class pixel> struct LrStore {
     pixel *o; ptrdiff_t st;   // tile origin and row pitch
     B200_DEV void operator()(int x, int y, int v) const { o[y * st + x] = (pixel)v; }
@@ -221,27 +250,27 @@ B200_DEV void lr_unit_params(const B200RestorationUnit &u, bool hbd, LrTileParam
     }
 }
 
-struct LrGrid { int base[3], nx[3]; unsigned nx_recip[3]; int ty0[3]; };   // flattened tile list: plane p owns CTAs base[p] .. , nx[p] tiles per row;
-                                                               // nx_recip = ceil(2^32 / nx): local / nx == mulhi(local, nx_recip) while local * nx < 2^32
+// flattened tile list: plane p owns CTAs base[p] .. , nx[p] tiles per row; nx_recip = ceil(2^32 / nx):
+// local / nx == mulhi(local, nx_recip) while local * nx < 2^32. pair: the chroma tiles are 32 wide and run as U / V
+// pairs, so plane 1's CTAs restore both chroma planes and plane 2's range is empty.
+struct LrGrid { int base[3], nx[3]; unsigned nx_recip[3]; int ty0[3]; int pair; };
 
-template <bool HBD>
-#ifndef B200_LR_MINB
-#define B200_LR_MINB 6
-#endif
-__global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __grid_constant__ B200LrFrame f, const __grid_constant__ LrGrid lg, int bdmax)
+// One tile of plane pl on threads tid = 0 .. NT - 1 (all 256 of the CTA, or one half of a U / V pair). Both halves of
+// a pair have the same geometry, so they leave together or run the same two barriers whatever their unit types: one
+// after the parameters and the staged source, one between the two compute passes (an unrestored tile is copied out
+// of the staged source in the first pass).
+template <bool HBD, int TW, int NT>
+B200_DEV void lr_frame_tile(const B200LrFrame &f, const LrGrid &lg, int bdmax, int rp, int pl, int local, int tid,
+                            LrShared<TW> &sm, const unsigned *tbl)
 {
-    B200_PDL_ENTRY();
     typedef typename Bd<HBD>::pixel pixel;
-    __shared__ LrShared sm;
-    const int bid = blockIdx.x;
-    const int pl = bid >= lg.base[2] ? 2 : bid >= lg.base[1] ? 1 : 0;
     const int ssh = pl ? f.ss_hor : 0, ssv = pl ? f.ss_ver : 0;
     const int w = (f.w + ssh) >> ssh, h = (f.h + ssv) >> ssv;
     const int us_log2 = f.unit_size_log2[pl ? 1 : 0], unit = 1 << us_log2, half = unit >> 1;
-    const int tw_full = unit < kTW ? unit : kTW;
-    const int local = bid - lg.base[pl], nxp = lg.nx[pl];
-    const int tyl = nxp > 1 ? (int)__umulhi((unsigned)local, lg.nx_recip[pl]) : local, txi = local - tyl * nxp;
-    const int tyi = tyl + lg.ty0[pl];                     // first tile row of this launch (a band, or 0 for the frame)
+    const int tw_full = unit < TW ? unit : TW;
+    const int nxp = lg.nx[rp];
+    const int tyl = nxp > 1 ? (int)__umulhi((unsigned)local, lg.nx_recip[rp]) : local, txi = local - tyl * nxp;
+    const int tyi = tyl + lg.ty0[rp];                     // first tile row of this launch (a band, or 0 for the frame)
     const int x0 = txi * tw_full;
     // a 64-row luma stripe is 2 tiles tall; a vertically subsampled stripe (32 rows) is 1
     const int k = ssv ? tyi : tyi >> 1, ty = ssv ? 0 : tyi & 1;
@@ -252,25 +281,23 @@ __global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __gri
     const int tw = imin(tw_full, w - x0), th = imin(kTH, y1s - ty0);
     const pixel *C = (const pixel *)f.cdef + f.plane_off[pl];
     const pixel *D = (const pixel *)f.dbl + f.plane_off[pl];
-    pixel *O = (pixel *)f.dst + f.plane_off[pl];
     const int st = f.stride[pl];
 
     const bool have_top = y0s > 0, have_bot = y1s < h;
     constexpr int PPW = HBD ? 2 : 4;                                 // samples per 32-bit word
     // interior tiles are staged from aligned words over picture columns x0-4 .. x0+tw+3 (one more column on each
-    // side than needed); the copy of an unrestored interior tile writes the same words
+    // side than needed)
     const bool interior = x0 >= 4 && x0 + tw + 4 <= w && !(tw & 3) && !(x0 & 3) && !(st & (PPW - 1)) &&
-                          !(((uintptr_t)C | (uintptr_t)D | (uintptr_t)O) & 3);
+                          !(((uintptr_t)C | (uintptr_t)D | (uintptr_t)((pixel *)f.dst + f.plane_off[pl])) & 3);
     const int NW = (tw + 8) / PPW;
     const unsigned magic = recip16(NW);                   // exact i / NW for i < 38 * 36
 
-    // The unit lookup and the tap / weight set-up are per-tile work: thread 0 starts them, the loads of the interior
-    // staging are issued by every thread while its lr_mask load is in flight, and the tile reads the parameters from
-    // shared memory after one barrier.
-    __shared__ LrTileParams sP;
+    // The unit lookup and the tap / weight set-up are per-tile work: the tile's thread 0 starts them, the loads of the
+    // interior staging are issued by every thread while its lr_mask load is in flight, and the tile reads the
+    // parameters and the staged source after the first barrier.
     B200RestorationUnit u;
     u.type = 0;
-    if (threadIdx.x == 0 && (f.restore_planes & (1 << pl))) {
+    if (tid == 0 && (f.restore_planes & (1 << pl))) {
         // unit lookup: reference src/lr_apply_tmpl.c:107-148
         int n_full = 0;
         { const int max_unit = unit + half; if (w >= max_unit) n_full = (w - max_unit) / unit + 1; }
@@ -284,12 +311,12 @@ __global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __gri
         const int shift_hor = 7 - ssh;
         u = f.lr_mask[sb_idx + (xu >> shift_hor)].lr[pl][unit_idx + ((xu >> (shift_hor - 1)) & 1)];
     }
-    constexpr int NI = HBD ? 6 : 3;                       // ceil(38 * 72 / PPW / 256) words per thread
+    constexpr int NI = ((kSH * (TW + 8)) / PPW + NT - 1) / NT;    // words per thread: 3 (8-bit) or 6
     unsigned wv[NI];
     if (interior) {
 #pragma unroll
         for (int n = 0; n < NI; n++) {
-            const int i = threadIdx.x + n * 256;
+            const int i = tid + n * NT;
             const int yy = (int)((i * magic) >> 16), g = i - yy * NW;
             if (yy >= th + 6) break;
             int Y = ty0 - 3 + yy;
@@ -302,36 +329,11 @@ __global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __gri
             wv[n] = *(const unsigned *)(base + (ptrdiff_t)Y * st + x0 - 4 + g * PPW);
         }
     }
-    if (threadIdx.x == 0) {
-        LrTileParams P;
-        lr_unit_params(u, HBD, P);
-        sP = P;
-    }
-    __syncthreads();
-    const LrTileParams &P = sP;
-    if (P.type == 0) {
-        if (interior) {
-#pragma unroll
-            for (int n = 0; n < NI; n++) {
-                const int i = threadIdx.x + n * 256;
-                const int yy = (int)((i * magic) >> 16), g = i - yy * NW;
-                if (yy >= th + 6) break;
-                if (yy >= 3 && yy < th + 3 && g * PPW >= 4 && g * PPW < tw + 4)
-                    *(unsigned *)(O + (ptrdiff_t)(ty0 - 3 + yy) * st + x0 - 4 + g * PPW) = wv[n];
-            }
-        } else
-        for (int i = threadIdx.x; i < kTW * th; i += blockDim.x) {
-            const int y = i / kTW, x = i - y * kTW;
-            if (x >= tw) continue;
-            O[(ptrdiff_t)(ty0 + y) * st + x0 + x] = C[(ptrdiff_t)(ty0 + y) * st + x0 + x];
-        }
-        return;
-    }
     // stage the virtual source: rows ty0-3 .. ty0+th+2, cols x0-3 .. x0+tw+2
     if (interior) {
 #pragma unroll
         for (int n = 0; n < NI; n++) {
-            const int i = threadIdx.x + n * 256;
+            const int i = tid + n * NT;
             const int yy = (int)((i * magic) >> 16), g = i - yy * NW;
             if (yy >= th + 6) break;
             const int c0 = g * PPW - 1;                              // tile column of the word's first sample
@@ -342,8 +344,8 @@ __global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __gri
             }
         }
     } else
-    for (int i = threadIdx.x; i < (th + 6) * kSW; i += blockDim.x) {
-        const int yy = i / kSW, xx = i - yy * kSW;
+    for (int i = tid; i < (th + 6) * LrShared<TW>::SW; i += NT) {
+        const int yy = i / LrShared<TW>::SW, xx = i - yy * LrShared<TW>::SW;
         if (xx >= tw + 6) continue;
         int Y = ty0 - 3 + yy;
         const int X = iclip(x0 - 3 + xx, 0, w - 1);
@@ -355,8 +357,49 @@ __global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __gri
         }
         sm.src[yy][xx] = base[(ptrdiff_t)Y * st + X];
     }
+    if (tid == 0) {
+        LrTileParams P;
+        lr_unit_params(u, HBD, P);
+        P.out = f.plane_off[pl] + (ptrdiff_t)ty0 * st + x0; P.st = st;
+        sm.P = P;
+    }
     __syncthreads();
-    lr_tile_compute<HBD>(sm, P, tw, th, bdmax, LrStore<pixel>{ O + (ptrdiff_t)ty0 * st + x0, st });
+    const LrTileParams &P = sm.P;
+    // (the output origin and pitch are read from shared memory where they are used: kept in registers across the
+    // passes, they cost registers the passes need)
+    if (P.type == 0) {
+        // an unrestored tile is the staged tile copied out, 4 samples of a row per thread
+        const LrStore<pixel> store{ (pixel *)f.dst + P.out, P.st };
+        for (int i = tid; i < th * (TW / 4); i += NT) {
+            const int y = i / (TW / 4), x = (i - y * (TW / 4)) * 4;
+            if (x >= tw) continue;
+            const int v[4] = { sm.src[y + 3][x + 3], sm.src[y + 3][x + 4], sm.src[y + 3][x + 5], sm.src[y + 3][x + 6] };
+            store.row4(x, y, v, imin(4, tw - x));
+        }
+    } else
+        lr_tile_pass1<HBD>(sm, P, tbl, tw, th, bdmax, tid, NT);
+    __syncthreads();
+    if (P.type) lr_tile_pass2<HBD>(sm, P, tw, th, bdmax, tid, NT, LrStore<pixel>{ (pixel *)f.dst + P.out, P.st });
+}
+
+template <bool HBD>
+#ifndef B200_LR_MINB
+#define B200_LR_MINB 6
+#endif
+__global__ void __launch_bounds__(256, B200_LR_MINB) lr_frame_kernel(const __grid_constant__ B200LrFrame f, const __grid_constant__ LrGrid lg, int bdmax)
+{
+    B200_PDL_ENTRY();
+    __shared__ __align__(16) unsigned char smem[kLrSmem];
+    __shared__ unsigned tbl[64];
+    lr_stage_x_by_x(tbl);                                 // read after the tile's first barrier
+    const int bid = blockIdx.x;
+    const int pl = bid >= lg.base[2] ? 2 : bid >= lg.base[1] ? 1 : 0;
+    if (pl && lg.pair) {
+        const int hf = threadIdx.x >> 7;                  // threads 0-127: U, 128-255: V
+        lr_frame_tile<HBD, 32, 128>(f, lg, bdmax, 1, 1 + hf, bid - lg.base[1], threadIdx.x & 127,
+                                    ((LrShared<32> *)smem)[hf], tbl);
+    } else
+        lr_frame_tile<HBD, kTW, 256>(f, lg, bdmax, pl, pl, bid - lg.base[pl], threadIdx.x, *(LrShared<kTW> *)smem, tbl);
 }
 
 // Level 1: window = host-assembled (w + 6) x (h + 6) virtual source; out = dense w x h
@@ -364,16 +407,20 @@ template <bool HBD>
 __global__ void __launch_bounds__(256) lr_window_kernel(const typename Bd<HBD>::pixel *win, typename Bd<HBD>::pixel *out,
                                                         int w, int h, LrTileParams P, int bdmax)
 {
-    __shared__ LrShared sm;
+    __shared__ LrShared<kTW> sm;
+    __shared__ unsigned tbl[64];
+    lr_stage_x_by_x(tbl);
     const int x0 = blockIdx.x * kTW, y0 = blockIdx.y * kTH;
     const int tw = imin(kTW, w - x0), th = imin(kTH, h - y0);
-    for (int i = threadIdx.x; i < (th + 6) * kSW; i += blockDim.x) {
-        const int yy = i / kSW, xx = i - yy * kSW;
+    for (int i = threadIdx.x; i < (th + 6) * LrShared<kTW>::SW; i += blockDim.x) {
+        const int yy = i / LrShared<kTW>::SW, xx = i - yy * LrShared<kTW>::SW;
         if (xx >= tw + 6) continue;
         sm.src[yy][xx] = win[(size_t)(y0 + yy) * (w + 6) + x0 + xx];
     }
     __syncthreads();
-    lr_tile_compute<HBD>(sm, P, tw, th, bdmax, LrStore<typename Bd<HBD>::pixel>{ out + (size_t)y0 * w + x0, w });
+    lr_tile_pass1<HBD>(sm, P, tbl, tw, th, bdmax, (int)threadIdx.x, (int)blockDim.x);
+    __syncthreads();
+    lr_tile_pass2<HBD>(sm, P, tw, th, bdmax, (int)threadIdx.x, (int)blockDim.x, LrStore<typename Bd<HBD>::pixel>{ out + (size_t)y0 * w + x0, w });
 }
 
 // tile rows [r0, r1) of the sweep, counted in half stripes: tile row r is rows 32 r - 8 .. 32 r + 23 of the luma plane
@@ -389,6 +436,7 @@ int lr_frame_rows(int bdmax, const B200LrFrame *f, int r0, int r1, cudaStream_t 
     // (A register-only path for Wiener tiles — rolling ring as in mc.cu, dp4a horizontal pass, no staging — was no faster
     // than this staged form, and slower with all rows loaded up front at lower occupancy. Dropped.)
     LrGrid lg;
+    lg.pair = f->unit_size_log2[1] == 5;                  // 32-wide chroma tiles: U / V pairs in plane 1's range
     int total = 0;
     for (int p = 0; p < 3; p++) {
         const int ssh = p ? f->ss_hor : 0, ssv = p ? f->ss_ver : 0;
@@ -399,7 +447,7 @@ int lr_frame_rows(int bdmax, const B200LrFrame *f, int r0, int r1, cudaStream_t 
         lg.base[p] = total;
         const int a = ssv ? r0 >> 1 : r0, b = ssv ? r1 >> 1 : r1;
         lg.ty0[p] = a;
-        total += lg.nx[p] * imax(b - a, 0);
+        if (p < 2 || !lg.pair) total += lg.nx[p] * imax(b - a, 0);
     }
     if (!total) return 0;
     return launch_hbd(bdmax, Launch::pdl, dim3(total), dim3(256), 0, stream,
