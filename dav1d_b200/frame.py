@@ -72,6 +72,82 @@ class NumpyAlloc:
         return None, None
 
 
+# ---- the stage descriptors of a frame: S's geometry and parameters, buffers as plain addresses ----
+def mc_frame(S):
+    """B200McFrame geometry: every reference has S's planes (the callers set the buffer pointers)"""
+    fr = _lib.McFrame()
+    ssh, ssv = [0, S["ss_hor"], S["ss_hor"]], [0, S["ss_ver"], S["ss_ver"]]
+    for p in range(3):
+        fr.ref_plane_off[p] = S["off"][p]; fr.ref_stride[p] = fr.dst_stride[p] = S["stride"][p]
+        fr.ref_w[p] = (S["W"] + ssh[p]) >> ssh[p]; fr.ref_h[p] = (S["H"] + ssv[p]) >> ssv[p]
+    return fr
+
+
+def intra_frame(S, pic, coef):
+    """B200IntraFrame geometry over the picture at `pic` and the dense coefficients at `coef`"""
+    fr = _lib.IntraFrame()
+    fr.pic, fr.d_coef = pic, coef
+    fr.ss_hor, fr.ss_ver = S["ss_hor"], S["ss_ver"]
+    for p in range(3):
+        ssh, ssv = (S["ss_hor"], S["ss_ver"]) if p else (0, 0)
+        fr.stride[p], fr.plane_off[p] = S["stride"][p], S["off"][p]
+        fr.w4[p], fr.h4[p] = S["w4"] >> ssh, S["h4"] >> ssv
+    return fr
+
+
+def lf_frame(S, pic, mask, level):
+    """B200LfFrame: deblocks the picture at `pic` in place. S["sb128"] (default 0) is the superblock walk order and
+    S["filter_uv"] (default 1) whether chroma is filtered; luma always is."""
+    fr = _lib.LfFrame()
+    fr.pic, fr.mask, fr.level = pic, mask, level
+    for p in range(3):
+        fr.plane_off[p] = S["off"][p]; fr.stride[p] = S["stride"][p]
+    fr.w4, fr.h4, fr.sb128w, fr.b4_stride = S["w4"], S["h4"], S["sb128w"], S["b4_stride"]
+    fr.ss_hor, fr.ss_ver, fr.sb128 = S["ss_hor"], S["ss_ver"], S.get("sb128", 0)
+    fr.filter_y, fr.filter_uv = 1, S.get("filter_uv", 1)
+    for k in range(64):
+        fr.lut.e[k], fr.lut.i[k] = int(S["lut_e"][k]), int(S["lut_i"][k])
+    fr.lut.sharp[0], fr.lut.sharp[1] = S["lut_sharp"]
+    return fr
+
+
+def cdef_frame(S, src, dst, mask):
+    """B200CdefFrame: the picture at `src` filtered into `dst`"""
+    fr = _lib.CdefFrame()
+    fr.src, fr.dst, fr.mask = src, dst, mask
+    for p in range(3):
+        fr.plane_off[p] = S["off"][p]; fr.stride[p] = S["stride"][p]
+    fr.bw, fr.bh, fr.sb128w, fr.ss_hor, fr.ss_ver, fr.damping = S["bw"], S["bh"], S["sb128w"], S["ss_hor"], S["ss_ver"], S["damping"]
+    for i in range(8):
+        fr.y_strength[i], fr.uv_strength[i] = S["y_strength"][i], S["uv_strength"][i]
+    return fr
+
+
+def lr_frame(S, cdef, dbl, dst, lr_mask):
+    """B200LrFrame: the CDEF output at `cdef` (and the deblocked picture at `dbl`, for the stripe edges) restored
+    into `dst`"""
+    fr = _lib.LrFrame()
+    fr.cdef, fr.dbl, fr.dst, fr.lr_mask = cdef, dbl, dst, lr_mask
+    for p in range(3):
+        fr.plane_off[p] = S["off"][p]; fr.stride[p] = S["stride"][p]
+    fr.w, fr.h, fr.ss_hor, fr.ss_ver, fr.sb128 = S["W"], S["H"], S["ss_hor"], S["ss_ver"], S["sb128"]
+    fr.sr_sb128w = (S["W"] + 127) >> 7
+    fr.unit_size_log2[0], fr.unit_size_log2[1] = S["us"]
+    fr.restore_planes = S["rp"]
+    return fr
+
+
+def fg_frame(S, src, dst):
+    """B200FgFrame: film grain S["fg"] applied to the picture at `src`, written to `dst` (the caller sets the scratch)"""
+    fr = _lib.FgFrame()
+    fr.in_, fr.out = src, dst
+    for p in range(3):
+        fr.plane_off[p] = S["off"][p]; fr.stride[p] = S["stride"][p]
+    fr.w, fr.h, fr.ss_hor, fr.ss_ver, fr.is_id = S["W"], S["H"], S["ss_hor"], S["ss_ver"], 0
+    fr.data = S["fg"]
+    return fr
+
+
 def band_plan(S, band_rows, compact=False, fused=False):
     """Cut a frame's records into horizontal bands of `band_rows` luma rows (a multiple of 64: blocks never straddle a
     band). Returns (S2, bands, need): S2 = shallow copy of S whose record arrays are stably sorted by band (the by-area
@@ -310,13 +386,11 @@ class FrameBuffers:
         mask = up("mask", S["mask"])
         j = _lib.FrameJob()
         j.bitdepth_max, j.zero_coefs = S["bd"], 0
+        j.mc = mc_frame(S)
         for i, r in enumerate(refs):
             j.mc.ref[i] = r
-        ssh, ssv = [0, S["ss_hor"], S["ss_hor"]], [0, S["ss_ver"], S["ss_ver"]]
         for p in range(3):
-            j.mc.ref_plane_off[p] = S["off"][p]; j.mc.ref_stride[p] = S["stride"][p]
-            j.mc.ref_w[p] = (S["W"] + ssh[p]) >> ssh[p]; j.mc.ref_h[p] = (S["H"] + ssv[p]) >> ssv[p]
-            j.mc.dst_stride[p] = S["stride"][p]; j.itx_stride[p] = S["stride"][p]
+            j.itx_stride[p] = S["stride"][p]
         j.mc.dst, j.mc.tmp, j.mc.mask, j.mc.px_tmp = p0, tmp, mask, (zeros("px_tmp", S["px_tmp_len"] * px) if S.get("px_tmp_len") else None)
         self.uploads = []          # (name, host array) re-sent per frame on the end-to-end path
 
@@ -367,16 +441,11 @@ class FrameBuffers:
             j.d_coef = up("coef", S["coefs"]); self.uploads.append(("coef", S["coefs"]))
         if len(S["mask"]) > 1:
             self.uploads.append(("mask", S["mask"]))
-        n_intra = 0
         if S.get("intra_tx") is not None and len(S["intra_tx"]):
+            j.intra = intra_frame(S, p0, j.d_coef)
             it = j.intra
-            it.pic, it.d_coef, it.zero_coefs, it.grid = p0, j.d_coef, 0, intra_grid
-            it.ss_hor, it.ss_ver = S["ss_hor"], S["ss_ver"]
+            it.grid = intra_grid
             it.mask = mask                            # blend masks of inter-intra (II) records
-            for p in range(3):
-                it.stride[p] = S["stride"][p]
-                it.w4[p] = S["w4"] >> ssh[p]; it.h4[p] = S["h4"] >> ssv[p]
-                it.plane_off[p] = S["off"][p]
             nb = self.lib.b200_intra_scratch_bytes(C.byref(it)) if hasattr(self.lib, "b200_intra_scratch_bytes") else 1 << 22
             it.scratch = zeros("intra_scratch", nb)
             if intra_sb:     # superblock-granular schedule (records grouped by 64x64 superblock)
@@ -391,64 +460,28 @@ class FrameBuffers:
                 if S.get("done_init") is not None:       # a frame that mixes inter and intra blocks: inter cells are final already
                     it.done_init = up("done_init", S["done_init"])
                     self.uploads.append(("done_init", S["done_init"]))
-            n_intra = 1
         # post filters
         j.run_lf, j.run_cdef, j.run_lr = int(run_lf), int(run_cdef), int(run_lr)
         d_masks = up("masks", S["masks"]); self.uploads.append(("masks", S["masks"]))
         d_level = up("level", S["level"]); self.uploads.append(("level", S["level"]))
         d_lrm = up("lr_mask", S["lr_mask"]); self.uploads.append(("lr_mask", S["lr_mask"]))
-        lf = j.lf
-        lf.pic = p0
-        for p in range(3):
-            lf.plane_off[p] = S["off"][p]; lf.stride[p] = S["stride"][p]
-        lf.w4, lf.h4, lf.sb128w, lf.b4_stride = S["w4"], S["h4"], S["sb128w"], S["b4_stride"]
-        lf.ss_hor, lf.ss_ver, lf.sb128, lf.filter_y, lf.filter_uv = S["ss_hor"], S["ss_ver"], S["sb128"], 1, 1
-        lf.mask, lf.level = d_masks, d_level
-        for k in range(64):
-            lf.lut.e[k], lf.lut.i[k] = int(S["lut_e"][k]), int(S["lut_i"][k])
-        lf.lut.sharp[0], lf.lut.sharp[1] = S["lut_sharp"]
-        cd = j.cdef
-        cd.src, cd.dst = p0, p1
-        for p in range(3):
-            cd.plane_off[p] = S["off"][p]; cd.stride[p] = S["stride"][p]
-        cd.bw, cd.bh, cd.sb128w, cd.ss_hor, cd.ss_ver, cd.damping = S["bw"], S["bh"], S["sb128w"], S["ss_hor"], S["ss_ver"], S["damping"]
-        for i in range(8):
-            cd.y_strength[i], cd.uv_strength[i] = S["y_strength"][i], S["uv_strength"][i]
-        cd.mask = d_masks
-        lr = j.lr
-        lr.cdef, lr.dbl, lr.dst = (p1 if run_cdef else p0), p0, p2
-        for p in range(3):
-            lr.plane_off[p] = S["off"][p]; lr.stride[p] = S["stride"][p]
-        lr.w, lr.h, lr.ss_hor, lr.ss_ver, lr.sb128 = S["W"], S["H"], S["ss_hor"], S["ss_ver"], S["sb128"]
-        lr.sr_sb128w = (S["W"] + 127) >> 7
-        lr.unit_size_log2[0], lr.unit_size_log2[1] = S["us"]
-        lr.restore_planes, lr.lr_mask = S["rp"], d_lrm
+        j.lf = lf_frame(S, p0, d_masks, d_level)
+        j.cdef = cdef_frame(S, p0, p1, d_masks)
+        j.lr = lr_frame(S, p1 if run_cdef else p0, p0, p2, d_lrm)
         self.out_name = "p2" if run_lr else ("p1" if run_cdef else "p0")
         if self.bands is not None and len(self.bands) > 1 and j.n_intra:
             # the pre-filter bottom rows of the bands, which the first row of intra records of the next band reads
             edge = zeros("intra_edge", self.lib.b200_band_edge_bytes(C.byref(j)))
             for b in self.bands:
                 b.intra_edge = edge
-        n_fg = 0
         self.ref_name = self.out_name          # the picture later frames predict from (never the grained copy)
         if S.get("fg") is not None:
             # film grain goes into a separate display copy; the un-grained picture stays the reference picture
-            fg = j.fg
+            j.fg = fg_frame(S, self.keep[self.out_name][1], zeros("p3", nbytes))
             j.run_fg = 1
-            fg.in_, fg.out = self.keep[self.out_name][1], zeros("p3", nbytes)
-            for p in range(3):
-                fg.plane_off[p] = S["off"][p]; fg.stride[p] = S["stride"][p]
-            fg.w, fg.h, fg.ss_hor, fg.ss_ver, fg.is_id = S["W"], S["H"], S["ss_hor"], S["ss_ver"], 0
-            fg.data = S["fg"]
-            fg.scratch = zeros("fg_scratch", 256 * 1024)
+            j.fg.scratch = zeros("fg_scratch", 256 * 1024)
             self.ref_name, self.out_name = self.out_name, "p3"
-            n_fg = 2
         self.job = j
-        self.n_launches = (1 if j.n_pred else 0) + (1 if j.n_comp else 0) + (1 if j.n_comp2 else 0) + \
-            (1 if j.n_warp else 0) + (1 if j.n_blend else 0) + (1 if j.n_blend2 else 0) + \
-            (1 if j.n_cfused else 0) + (1 if j.n_cfused2 else 0) + \
-            (1 if any(j.n_itx[tx] for tx in (4, 11, 12, 17, 18)) else 0) + \
-            (1 if any(j.n_itx[tx] for tx in range(19) if tx not in (4, 11, 12, 17, 18)) else 0) + 2 * int(run_lf) + int(run_cdef) + int(run_lr) + n_fg + n_intra
         self._host = None
 
     # ---- device-resident run (records already in HBM) ----

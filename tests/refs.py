@@ -66,6 +66,12 @@ def emu_lib():
     return _cache["emu"]
 
 
+def lib_alloc(gpu):
+    """(library, alloc): the CUDA build with buffers in HBM, or the host emulator with buffers in host memory"""
+    from dav1d_b200 import frame, get_lib
+    return (get_lib(), frame.TorchAlloc()) if gpu else (emu_lib(), frame.NumpyAlloc())
+
+
 # ---------------------------------------------------------------- reference DSP tables
 FT8 = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_int)
 FT16 = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_int, C.c_int)

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 import refs
-from dav1d_b200 import _lib, synth
+from dav1d_b200 import frame, synth
 
 
 def init_tmp(rng, n, bd, dt):
@@ -105,30 +105,26 @@ def make_cdef_frame(rng, bpc, W, H, ssh, ssv):
     return S
 
 
-def cdef_frame_struct(S, src_ptr, dst_ptr, mask_ptr):
-    fr = _lib.CdefFrame()
-    fr.src, fr.dst = src_ptr, dst_ptr
-    for p in range(3):
-        fr.plane_off[p] = S["off"][p]; fr.stride[p] = S["stride"][p]
-    fr.bw, fr.bh, fr.sb128w, fr.ss_hor, fr.ss_ver, fr.damping = S["bw"], S["bh"], S["sb128w"], S["ss_hor"], S["ss_ver"], S["damping"]
-    for i in range(8):
-        fr.y_strength[i], fr.uv_strength[i] = S["y_strength"][i], S["uv_strength"][i]
-    fr.mask = mask_ptr
-    return fr
-
-
 def cdef_frame_oracle(S):
     dst = S["pic"].copy()
-    fr = cdef_frame_struct(S, S["pic"].ctypes.data, dst.ctypes.data, S["masks"].ctypes.data)
+    fr = frame.cdef_frame(S, S["pic"].ctypes.data, dst.ctypes.data, S["masks"].ctypes.data)
     refs.oracle().oracle_cdef_frame(S["bd"], C.byref(fr))
     return dst
 
 
 def cdef_frame_reference(S):
     pic = S["pic"].copy()
-    fr = cdef_frame_struct(S, pic.ctypes.data, None, S["masks"].ctypes.data)
+    fr = frame.cdef_frame(S, pic.ctypes.data, None, S["masks"].ctypes.data)
     (refs.ref().refdrv_cdef_frame_8bpc if S["bpc"] == 8 else refs.ref().refdrv_cdef_frame_16bpc)(S["bd"], C.byref(fr))
     return pic
+
+
+def cdef_frame_lib(S, lib, alloc):
+    """b200_cdef_frame on S's picture and masks placed by `alloc`"""
+    src, dst, mask = alloc.upload(S["pic"]), alloc.zeros(S["pic"].nbytes), alloc.upload(S["masks"])
+    lib.check(lib.b200_cdef_frame(S["bd"], C.byref(frame.cdef_frame(S, src[1], dst[1], mask[1])), None), "b200_cdef_frame")
+    alloc.sync()
+    return alloc.download(dst[0], S["pic"])
 
 
 def frame_area_equal(S, a, b):
@@ -173,12 +169,7 @@ def test_emu_cdef_level1(bpc):
                                                 (12, 68, 36, 0, 0), (10, 204, 100, 1, 1)])
 def test_emu_cdef_frame(bpc, W, H, ssh, ssv):
     S = make_cdef_frame(np.random.default_rng(430 + bpc + W), bpc, W, H, ssh, ssv)
-    exp = cdef_frame_oracle(S)
-    dst = np.zeros_like(S["pic"])
-    lib = refs.emu_lib()
-    fr = cdef_frame_struct(S, S["pic"].ctypes.data, dst.ctypes.data, S["masks"].ctypes.data)
-    lib.check(lib.b200_cdef_frame(S["bd"], C.byref(fr), None), "cdef_frame")
-    assert frame_area_equal(S, dst, exp)
+    assert frame_area_equal(S, cdef_frame_lib(S, *refs.lib_alloc(False)), cdef_frame_oracle(S))
 
 
 @pytest.mark.gpu
@@ -192,17 +183,8 @@ def test_gpu_cdef_level1(bpc):
 @pytest.mark.gpu
 @pytest.mark.parametrize("bpc,W,H,ssh,ssv", [(8, 1920, 1080, 1, 1), (10, 1280, 720, 1, 0), (12, 648, 360, 0, 0), (8, 3840, 2160, 1, 1)])
 def test_gpu_cdef_frame(bpc, W, H, ssh, ssv):
-    import torch
-    from dav1d_b200 import get_lib
     S = make_cdef_frame(np.random.default_rng(450 + bpc + W), bpc, W, H, ssh, ssv)
     exp = cdef_frame_reference(S) if refs.have_ref() else cdef_frame_oracle(S)
-    lib = get_lib()
-    d_src = torch.from_numpy(S["pic"].view(np.uint8).copy()).cuda()
-    d_dst = torch.zeros_like(d_src)
-    d_mask = torch.from_numpy(S["masks"].view(np.uint8).copy()).cuda()
-    fr = cdef_frame_struct(S, d_src.data_ptr(), d_dst.data_ptr(), d_mask.data_ptr())
-    lib.check(lib.b200_cdef_frame(S["bd"], C.byref(fr), None), "cdef_frame")
-    torch.cuda.synchronize()
-    got = d_dst.cpu().numpy().view(S["pic"].dtype)
+    got = cdef_frame_lib(S, *refs.lib_alloc(True))
     assert frame_area_equal(S, got, exp)
     assert frame_area_equal(S, got, cdef_frame_oracle(S))

@@ -20,7 +20,7 @@ import pytest
 
 import refs
 from dav1d_b200 import _lib, synth
-from test_loopfilter import lf_frame_struct
+from test_loopfilter import lf_frame_buffers, lf_frame_lib, lf_frame_oracle, lf_frame_reference
 
 BRANCHES = ("fm_fail", "narrow_hev", "narrow", "flat6", "flat8", "flat8_of16", "flat16", "narrow_clip")
 LAYOUTS = {"420": (1, 1), "422": (1, 0), "444": (0, 0), "400": (1, 1)}
@@ -139,20 +139,6 @@ def case_frame(c):
     return make_case(*c, seed=900 + sum(c[1:4]) + 10 * c[4] + 1000 * list(LAYOUTS).index(c[0]))
 
 
-def lf_struct(S, pic_ptr, mask_ptr, level_ptr, sb128=0):
-    fr = lf_frame_struct(S, pic_ptr, mask_ptr, level_ptr)
-    fr.filter_uv = S["filter_uv"]
-    fr.sb128 = sb128
-    return fr
-
-
-def run_oracle(S, masks=None):
-    pic = S["pic"].copy()
-    masks = S["masks"] if masks is None else masks
-    refs.oracle().oracle_lf_frame(S["bd"], C.byref(lf_struct(S, pic.ctypes.data, masks.ctypes.data, S["level"].ctypes.data)))
-    return pic
-
-
 def branch_counts():
     """oracle counters since the last call: {(plane class, direction): {branch: lines}}"""
     out = np.zeros(2 * 2 * len(BRANCHES), np.int64)
@@ -161,51 +147,16 @@ def branch_counts():
     return {(pc, d): dict(zip(BRANCHES, map(int, out[pc, d]))) for pc in range(2) for d in range(2)}
 
 
-def run_reference(S, sb128):
-    pic = S["pic"].copy()
-    masks = S["masks"].copy()     # the real driver patches masks at tile edges in place
-    fr = lf_struct(S, pic.ctypes.data, masks.ctypes.data, S["level"].ctypes.data, sb128)
-    (refs.ref().refdrv_lf_frame_8bpc if S["bpc"] == 8 else refs.ref().refdrv_lf_frame_16bpc)(S["bd"], C.byref(fr))
-    return pic
-
-
-class Device:
-    """the picture, masks and levels of a case where the library reads them: host memory for the emulator, HBM for the GPU"""
-
-    def __init__(self, S, gpu):
-        self.S, self.gpu = S, gpu
-        if gpu:
-            import torch
-            from dav1d_b200 import get_lib
-            self.lib = get_lib()
-            self.pic = torch.from_numpy(S["pic"].view(np.uint8).copy()).cuda()
-            self.mask = torch.from_numpy(S["masks"].view(np.uint8).copy()).cuda()
-            self.level = torch.from_numpy(S["level"].reshape(-1).copy()).cuda()
-            ptrs = self.pic.data_ptr(), self.mask.data_ptr(), self.level.data_ptr()
-        else:
-            self.lib = refs.emu_lib()
-            self.pic, self.mask, self.level = S["pic"].copy(), S["masks"], S["level"]
-            ptrs = self.pic.ctypes.data, self.mask.ctypes.data, self.level.ctypes.data
-        self.fr = lf_struct(S, *ptrs)
-
-    def result(self):
-        if not self.gpu:
-            return self.pic
-        import torch
-        torch.cuda.synchronize()
-        return self.pic.cpu().numpy().view(self.S["pic"].dtype)
-
-
 def run_frame(S, gpu):
-    d = Device(S, gpu)
-    d.lib.check(d.lib.b200_lf_frame(S["bd"], C.byref(d.fr), None), "b200_lf_frame")
-    return d.result()
+    return lf_frame_lib(S, *refs.lib_alloc(gpu))
 
 
-def lf_job(d):
-    job = _lib.FrameJob()           # no reconstruction records: band_recon enqueues nothing
-    job.bitdepth_max, job.run_lf, job.lf = d.S["bd"], 1, d.fr
-    return job
+def lf_job(S, alloc):
+    """a frame job that only deblocks (no reconstruction records: band_recon enqueues nothing), and its buffers"""
+    bufs, fr = lf_frame_buffers(S, alloc)
+    job = _lib.FrameJob()
+    job.bitdepth_max, job.run_lf, job.lf = S["bd"], 1, fr
+    return job, bufs
 
 
 def band(y0, y1, last):
@@ -215,12 +166,13 @@ def band(y0, y1, last):
 
 
 def run_bands(S, gpu, band_rows):
-    d = Device(S, gpu)
-    job, H = lf_job(d), S["h4"] * 4
+    lib, A = refs.lib_alloc(gpu)
+    (job, bufs), H = lf_job(S, A), S["h4"] * 4
     for y0 in range(0, H, band_rows):
         y1 = min(y0 + band_rows, H)
-        d.lib.check(d.lib.b200_frame_run_band(C.byref(job), C.byref(band(y0, y1, int(y1 == H))), None), "b200_frame_run_band")
-    return d.result()
+        lib.check(lib.b200_frame_run_band(C.byref(job), C.byref(band(y0, y1, int(y1 == H))), None), "b200_frame_run_band")
+    A.sync()
+    return A.download(bufs[0][0], S["pic"])
 
 
 def chroma_untouched(S, got):
@@ -282,7 +234,7 @@ def area_fallbacks(S):
 def test_content_reaches_every_branch(case):
     S = case_frame(case)
     branch_counts()
-    run_oracle(S)
+    lf_frame_oracle(S)
     counts = branch_counts()
     assert not below_floor(counts, S["filter_uv"]), (below_floor(counts, S["filter_uv"]), counts)
     fb = area_fallbacks(S)
@@ -305,10 +257,10 @@ def test_oracle_vs_reference_driver(case):
     if not refs.have_ref():
         pytest.skip("reference build (oracle/_ref) not present")
     S = case_frame(case)
-    exp = run_oracle(S)
+    exp = lf_frame_oracle(S)
     assert (exp != S["pic"]).mean() > 0.01
     for sb128 in (0, 1):
-        assert np.array_equal(run_reference(S, sb128), exp), sb128
+        assert np.array_equal(lf_frame_reference(S, sb128), exp), sb128
     if not S["filter_uv"]:
         assert chroma_untouched(S, exp)
 
@@ -317,7 +269,7 @@ def test_oracle_vs_reference_driver(case):
 @pytest.mark.parametrize("case", CASES + ODD, ids=case_id)
 def test_emu_lf_frame(case):
     S = case_frame(case)
-    check_case(S, run_frame(S, False), run_oracle(S))
+    check_case(S, run_frame(S, False), lf_frame_oracle(S))
 
 
 # ---------------------------------------------------------------------------------------- band seams
@@ -336,7 +288,7 @@ def seam_flat16(S, out):
     rows_off = S["masks"].copy()
     rows_off["filter_y"][:, 1] = 0
     rows_off["filter_uv"][:, 1] = 0
-    cols_only = plane(S, run_oracle(S, rows_off), 0)
+    cols_only = plane(S, lf_frame_oracle(dict(S, masks=rows_off)), 0)
     out = plane(S, out, 0)
     by, lh = S["til_y"][1], S["til_y"][3]
     res = []
@@ -350,7 +302,7 @@ def seam_flat16(S, out):
 
 def check_bands(S, gpu):
     whole = run_frame(S, gpu)
-    exp = run_oracle(S)
+    exp = lf_frame_oracle(S)
     assert np.array_equal(whole, exp)
     for rows in (64, 128, 192):
         got = run_bands(S, gpu, rows)
@@ -363,7 +315,7 @@ def test_band_seams_take_flat16(case):
     """the wide row filter really fires at every 64-row seam: band k's row pass rewrites band k - 1's bottom rows"""
     S = band_frame(*case)
     assert S["h4"] & 1
-    assert min(seam_flat16(S, run_oracle(S))) >= 3, seam_flat16(S, run_oracle(S))
+    assert min(seam_flat16(S, lf_frame_oracle(S))) >= 3, seam_flat16(S, lf_frame_oracle(S))
 
 
 @pytest.mark.emu
@@ -373,12 +325,13 @@ def test_emu_band_seams(case):
 
 
 def check_bad_bands(S, gpu):
-    d = Device(S, gpu)
-    job, H = lf_job(d), S["h4"] * 4
+    lib, A = refs.lib_alloc(gpu)
+    (job, bufs), H = lf_job(S, A), S["h4"] * 4
     for y0, y1, last in ((0, 68, 0), (4, 64, 0), (64, 96, 0), (0, H - 4, 1), (32, H, 1)):
-        assert d.lib.b200_frame_run_band(C.byref(job), C.byref(band(y0, y1, last)), None) == -2, (y0, y1, last)
-        assert b"64-row aligned" in d.lib.b200_last_error()
-    assert np.array_equal(d.result(), S["pic"])
+        assert lib.b200_frame_run_band(C.byref(job), C.byref(band(y0, y1, last)), None) == -2, (y0, y1, last)
+        assert b"64-row aligned" in lib.b200_last_error()
+    A.sync()
+    assert np.array_equal(A.download(bufs[0][0], S["pic"]), S["pic"])
 
 
 @pytest.mark.emu
@@ -399,7 +352,7 @@ GPU_BANDS = [("420", 8, 1918, 1084), ("422", 10, 1280, 724), ("444", 12, 1284, 7
 def test_gpu_lf_frame_cases():
     for case in CASES + ODD:
         S = case_frame(case)
-        check_case(S, run_frame(S, True), run_oracle(S))
+        check_case(S, run_frame(S, True), lf_frame_oracle(S))
 
 
 @pytest.mark.gpu
@@ -407,11 +360,11 @@ def test_gpu_lf_frame_cases():
 def test_gpu_lf_frame_large(case):
     S = case_frame(case)
     branch_counts()
-    exp = run_oracle(S)
+    exp = lf_frame_oracle(S)
     counts = branch_counts()
     assert not below_floor(counts, S["filter_uv"]), counts
     if refs.have_ref():
-        assert np.array_equal(run_reference(S, 1), exp)
+        assert np.array_equal(lf_frame_reference(S, 1), exp)
     check_case(S, run_frame(S, True), exp)
 
 

@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 import refs
-from dav1d_b200 import _lib
+from dav1d_b200 import _lib, frame
 
 GW, GH = 82, 73
 LAYOUTS = [(1, 1), (1, 0), (0, 0)]          # table index -> (ss_hor, ss_ver): 420, 422, 444
@@ -173,13 +173,10 @@ def make_fg_frame(rng, w, h, ss, bpc, d=None):
     off = [0, st0 * (h + 1), st0 * (h + 1) + st1 * (ch + 1)]
     total = off[2] + st1 * (ch + 1)
     pic = rng.integers(0, bd + 1, total).astype(pdt)
-    fr = _lib.FgFrame()
-    for i in range(3):
-        fr.plane_off[i] = off[i]
-        fr.stride[i] = st0 if i == 0 else st1
-    fr.w, fr.h, fr.ss_hor, fr.ss_ver = w, h, sx, sy
-    fr.is_id = int(rng.integers(0, 2))
-    fr.data = d if d is not None else rand_fg_data(rng)
+    is_id = int(rng.integers(0, 2))
+    fr = frame.fg_frame(dict(off=off, stride=[st0, st1, st1], W=w, H=h, ss_hor=sx, ss_ver=sy,
+                             fg=d if d is not None else rand_fg_data(rng)), None, None)
+    fr.is_id = is_id
     return fr, pic
 
 

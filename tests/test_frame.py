@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import refs
-from dav1d_b200 import _lib, synth, frame
+from dav1d_b200 import synth, frame
 import test_loopfilter as TLF
 import test_cdef as TCD
 import test_looprestoration as TLR
@@ -20,15 +20,10 @@ def oracle_frame(S, run_lf=True, run_cdef=True, run_lr=True):
     pic = np.zeros_like(S["pic"])
     tmp = np.zeros(S["tmp_len"], np.int16)
     mask = S["mask"].copy()
-    fr = _lib.McFrame()
+    fr = frame.mc_frame(S)
     keep = [r.copy() for r in S["refs"]]
     for i, r in enumerate(keep):
         fr.ref[i] = r.ctypes.data
-    ssh, ssv = [0, S["ss_hor"], S["ss_hor"]], [0, S["ss_ver"], S["ss_ver"]]
-    for p in range(3):
-        fr.ref_plane_off[p] = S["off"][p]; fr.ref_stride[p] = S["stride"][p]
-        fr.ref_w[p] = (S["W"] + ssh[p]) >> ssh[p]; fr.ref_h[p] = (S["H"] + ssv[p]) >> ssv[p]
-        fr.dst_stride[p] = S["stride"][p]
     fr.dst, fr.tmp, fr.mask = pic.ctypes.data, tmp.ctypes.data, mask.ctypes.data
     px_tmp = np.zeros(S.get("px_tmp_len", 1), pic.dtype)
     fr.px_tmp = px_tmp.ctypes.data
@@ -48,8 +43,7 @@ def oracle_frame(S, run_lf=True, run_cdef=True, run_lr=True):
             assert o.oracle_itx_add_batch(bd, tx, a.ctypes.data, len(a), coefs.ctypes.data, pic.ctypes.data, st, 0) == 0
     if S.get("intra_tx") is not None and len(S["intra_tx"]):
         # intra blocks of a mixed frame: record by record, after every inter block is in the picture
-        import test_intra as TI
-        fr_i = TI.intra_frame_struct(S, pic, coefs)
+        fr_i = frame.intra_frame(S, pic.ctypes.data, coefs.ctypes.data)
         fr_i.mask = mask.ctypes.data
         tx = np.ascontiguousarray(S["intra_tx_decode_order"])
         fn = o.oracle_intra_frame
@@ -70,12 +64,7 @@ def oracle_frame(S, run_lf=True, run_cdef=True, run_lr=True):
         out["lr"] = TLR.lr_frame_oracle(S3)
     if S.get("fg") is not None:
         import test_filmgrain as TFG
-        fr = _lib.FgFrame()
-        for p in range(3):
-            fr.plane_off[p] = S["off"][p]; fr.stride[p] = S["stride"][p]
-        fr.w, fr.h, fr.ss_hor, fr.ss_ver, fr.is_id = S["W"], S["H"], S["ss_hor"], S["ss_ver"], 0
-        fr.data = S["fg"]
-        out["fg"] = TFG.run_oracle_frame(fr, np.ascontiguousarray(out["lr"]), S["bpc"])
+        out["fg"] = TFG.run_oracle_frame(frame.fg_frame(S, None, None), np.ascontiguousarray(out["lr"]), S["bpc"])
     return out
 
 

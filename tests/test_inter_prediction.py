@@ -34,8 +34,7 @@ import pytest
 import refs
 from dav1d_b200 import _lib
 from test_mc import mct_input
-from test_scaled_prediction import LAYOUTS, _align, _emu_dev, _torch_dev, _torch_host, _torch_sync, _window_pos, checker, \
-    picture_geom
+from test_scaled_prediction import LAYOUTS, _align, _window_pos, checker, picture_geom
 
 EMU_W = 192                       # dav1d's emu_edge scratch (t->scratch.emu_edge) is 192 samples wide
 COUNTS = ("put_clip_lo", "put_clip_hi", "prep_max_8", "prep_max_10", "prep_max_12", "wmask_38", "wmask_64",
@@ -634,20 +633,20 @@ def counted_reference(B):
 
 
 # ------------------------------------------------------------------ the kernels
-def _records(recs, cls, to_dev):
+def _records(recs, cls, alloc):
     if not recs:
         return None, 0
     arr = (cls * len(recs))(*recs)
-    return to_dev(np.frombuffer(bytes(arr), np.uint8).copy()), len(recs)
+    return alloc.upload(np.frombuffer(arr, np.uint8)), len(recs)
 
 
-def run(B, lib, to_dev, from_dev, sync, fused=False):
+def run(B, lib, alloc, fused=False):
     """the stages on the library: the separate prediction / compound / blend / warp stages, or (fused) only the two
     fused compound stages"""
     names = ("dst", "mask") if fused else ("dst", "tmp", "mask", "px_tmp")
     init = dict(dst=B.dst, tmp=B.tmp, mask=B.mask_buf, px_tmp=B.px_tmp)
-    dev = {k: to_dev(init[k]) for k in names}
-    pics = [to_dev(p) for p in B.pics]
+    dev = {k: alloc.upload(init[k]) for k in names}
+    pics = [alloc.upload(p) for p in B.pics]
     fr = _lib.McFrame()
     g = B.g
     for p in range(3):
@@ -666,12 +665,14 @@ def run(B, lib, to_dev, from_dev, sync, fused=False):
         stages = [(lib.b200_mc_batch, B.pred, _lib.McBlock), (lib.b200_mc_comp_batch, B.comp, _lib.CompBlock),
                   (lib.b200_mc_comp_batch, B.comp2, _lib.CompBlock), (lib.b200_mc_blend_batch, B.blend, _lib.BlendBlock),
                   (lib.b200_mc_blend_batch, B.blend2, _lib.BlendBlock), (lib.b200_mc_warp_batch, B.warp, _lib.WarpBlock)]
+    held = []
     for fn, recs, cls in stages:
-        d, n = _records(recs, cls, to_dev)
+        d, n = _records(recs, cls, alloc)
+        held.append(d)
         if n:
             lib.check(fn(bd, C.byref(fr), d[1], n, None), fn.__name__)
-    sync()
-    return {k: from_dev(v, init[k]) for k, v in dev.items()}
+    alloc.sync()
+    return {k: alloc.download(v[0], init[k]) for k, v in dev.items()}
 
 
 def compare(exp, got, what):
@@ -719,12 +720,12 @@ COUNT_FLOORS = dict(put_clip_lo=30, put_clip_hi=30, wmask_38=300, wmask_64=16, h
                     h_identity=50, v_identity=50)
 
 
-def _case(bpc, layout, W, H, n, geom, n_refs, seed, lib, to_dev, from_dev, sync, split_floor):
+def _case(bpc, layout, W, H, n, geom, n_refs, seed, gpu, split_floor):
     rng = np.random.default_rng(seed)
     B = make_batch(rng, bpc, layout, W, H, n, geom, n_refs)
     (exp, exp_fused), counts = counted_reference(B)
-    compare(exp, run(B, lib, to_dev, from_dev, sync), "stages")
-    compare(exp_fused, run(B, lib, to_dev, from_dev, sync, fused=True), "fused")
+    compare(exp, run(B, *refs.lib_alloc(gpu)), "stages")
+    compare(exp_fused, run(B, *refs.lib_alloc(gpu), fused=True), "fused")
     check_coverage(B, counts, dict(split=split_floor))
     return B, counts
 
@@ -737,9 +738,7 @@ EMU_CASES = [(bpc, lay) + ((201, 137), (135, 73))[i % 2] + (("hooks", "tight", "
 @pytest.mark.emu
 @pytest.mark.parametrize("bpc,layout,W,H,geom,n_refs", EMU_CASES)
 def test_emu_inter_prediction(bpc, layout, W, H, geom, n_refs):
-    keep = []
-    _case(bpc, layout, W, H, 400, geom, n_refs, 2000 + 10 * bpc + list(LAYOUTS).index(layout), refs.emu_lib(),
-          _emu_dev(keep), lambda v, like: v[0], lambda: None, split_floor=5)
+    _case(bpc, layout, W, H, 400, geom, n_refs, 2000 + 10 * bpc + list(LAYOUTS).index(layout), False, split_floor=5)
 
 
 GPU_CASES = [(8, "420", 1920, 1080, "hooks", 8, 14000), (10, "420", 3840, 2160, "tight", 7, 14000),
@@ -750,9 +749,7 @@ GPU_CASES = [(8, "420", 1920, 1080, "hooks", 8, 14000), (10, "420", 3840, 2160, 
 @pytest.mark.gpu
 @pytest.mark.parametrize("bpc,layout,W,H,geom,n_refs,n", GPU_CASES)
 def test_gpu_inter_prediction(bpc, layout, W, H, geom, n_refs, n):
-    from dav1d_b200 import get_lib
-    B, _ = _case(bpc, layout, W, H, n, geom, n_refs, 2100 + W + bpc, get_lib(), _torch_dev, _torch_host, _torch_sync,
-                 split_floor=200)
+    B, _ = _case(bpc, layout, W, H, n, geom, n_refs, 2100 + W + bpc, True, split_floor=200)
     assert len(B.pred) + len(B.comp) + len(B.comp2) + len(B.blend) + len(B.blend2) + len(B.warp) >= 20000
 
 
@@ -763,7 +760,7 @@ import numpy as np
 sys.path[:0] = [{root!r}, {tests!r}]
 import refs
 import test_inter_prediction as T
-from dav1d_b200 import _lib
+from dav1d_b200 import _lib, frame
 
 libc = C.CDLL(None, use_errno=True)
 libc.mmap.restype = C.c_void_p
@@ -786,11 +783,8 @@ for bpc in (8, 10):
         base = m + n - end
         C.memmove(base, pic.ctypes.data, end)
         bases.append(base)
-    keep = []
-    def to_dev(a):
-        c = a.copy(); keep.append(c)
-        return (c, c.ctypes.data)
-    dst, tmp = to_dev(B.dst), to_dev(B.tmp)
+    A = frame.NumpyAlloc()
+    dst, tmp = A.upload(B.dst), A.upload(B.tmp)
     fr = _lib.McFrame()
     for p in range(3):
         fr.ref_plane_off[p], fr.ref_stride[p], fr.ref_w[p], fr.ref_h[p] = B.g["off"][p], B.g["stride"][p], B.g["w"][p], B.g["h"][p]
@@ -798,9 +792,10 @@ for bpc in (8, 10):
     for k, b in enumerate(bases):
         fr.ref[k] = b
     fr.dst, fr.tmp = dst[1], tmp[1]
-    recs, n = T._records(B.pred, _lib.McBlock, to_dev)
+    recs, n = T._records(B.pred, _lib.McBlock, A)
     lib.check(lib.b200_mc_batch(B.bd, C.byref(fr), recs[1], n, None), "b200_mc_batch")
-    assert np.array_equal(dst[0], exp["dst"]) and np.array_equal(tmp[0], exp["tmp"]), "wrong bytes at bpc %d" % bpc
+    assert np.array_equal(A.download(dst[0], B.dst), exp["dst"]) and np.array_equal(A.download(tmp[0], B.tmp), exp["tmp"]), \
+        "wrong bytes at bpc %d" % bpc
 print("ok")
 '''
 

@@ -16,19 +16,9 @@ from dav1d_b200 import _lib, synth, frame
 CASES = [(8, 136, 72, 1, 1), (10, 200, 136, 1, 1), (12, 72, 136, 0, 0), (8, 264, 136, 1, 0)]
 
 
-def intra_frame_struct(S, pic, coefs):
-    fr = _lib.IntraFrame()
-    ssh, ssv = [0, S["ss_hor"], S["ss_hor"]], [0, S["ss_ver"], S["ss_ver"]]
-    fr.pic, fr.d_coef, fr.zero_coefs = pic.ctypes.data, coefs.ctypes.data, 0
-    fr.ss_hor, fr.ss_ver = S["ss_hor"], S["ss_ver"]
-    for p in range(3):
-        fr.stride[p] = S["stride"][p]; fr.w4[p] = S["w4"] >> ssh[p]; fr.h4[p] = S["h4"] >> ssv[p]
-    return fr
-
-
 def run_cpu(fn, S, order="intra_tx"):
     pic = np.zeros_like(S["pic"]); coefs = S["coefs"].copy()
-    fr = intra_frame_struct(S, pic, coefs)
+    fr = frame.intra_frame(S, pic.ctypes.data, coefs.ctypes.data)
     tx = np.ascontiguousarray(S[order])
     fn.restype = None
     fn(C.c_int(S["bd"]), C.byref(fr), C.c_void_p(tx.ctypes.data), C.c_int(len(tx)))
@@ -262,10 +252,8 @@ def make_mixed(S, rng, p_pal=0.2, p_ii=0.25):
 
 def run_mixed(fn, S, emu=None):
     pic = S["mixed_pic0"].copy(); coefs = S["coefs"].copy()
-    fr = intra_frame_struct(S, pic, coefs)
+    fr = frame.intra_frame(S, pic.ctypes.data, coefs.ctypes.data)
     fr.mask, fr.pal = S["mixed_mask"].ctypes.data, S["mixed_pal"].ctypes.data
-    for p in range(3):
-        fr.plane_off[p] = S["off"][p]
     tx = np.ascontiguousarray(S["mixed_tx"])
     if emu is None:
         fn.restype = None

@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 import refs
-from dav1d_b200 import _lib, synth
+from dav1d_b200 import _lib, frame, synth
 
 
 def clipp(v, bd):
@@ -105,35 +105,36 @@ def run_lpf_checks(new, chk, bpc, seed, reps=6):
 
 
 # ------------------------------------------------------------------ frame level helpers
-def lf_frame_struct(S, pic_ptr, mask_ptr, level_ptr, cls=None):
-    fr = (cls or _lib.LfFrame)()
-    fr.pic = pic_ptr
-    for p in range(3):
-        fr.plane_off[p] = S["off"][p]; fr.stride[p] = S["stride"][p]
-    fr.w4, fr.h4, fr.sb128w, fr.b4_stride = S["w4"], S["h4"], S["sb128w"], S["b4_stride"]
-    fr.ss_hor, fr.ss_ver, fr.sb128 = S["ss_hor"], S["ss_ver"], S.get("sb128", 0)
-    fr.filter_y, fr.filter_uv = 1, 1
-    fr.mask, fr.level = mask_ptr, level_ptr + S["b4_stride"] * 4 * 0
-    for k in range(64):
-        fr.lut.e[k], fr.lut.i[k] = int(S["lut_e"][k]), int(S["lut_i"][k])
-    fr.lut.sharp[0], fr.lut.sharp[1] = S["lut_sharp"]
-    return fr
-
-
 def lf_frame_oracle(S):
     pic = S["pic"].copy()
-    fr = lf_frame_struct(S, pic.ctypes.data, S["masks"].ctypes.data, S["level"].ctypes.data)
-    refs.oracle().oracle_lf_frame(S["bd"], C.byref(fr))
+    refs.oracle().oracle_lf_frame(S["bd"], C.byref(frame.lf_frame(S, pic.ctypes.data, S["masks"].ctypes.data, S["level"].ctypes.data)))
     return pic
 
 
-def lf_frame_reference(S):
+def lf_frame_reference(S, sb128=None):
+    """dav1d's own driver; sb128 (default: S's) is the superblock walk order"""
     pic = S["pic"].copy()
     masks = S["masks"].copy()     # the real driver patches masks at tile edges in place
-    fr = lf_frame_struct(S, pic.ctypes.data, masks.ctypes.data, S["level"].ctypes.data)
-    fn = refs.ref().refdrv_lf_frame_8bpc if S["bpc"] == 8 else refs.ref().refdrv_lf_frame_16bpc
-    fn(S["bd"], C.byref(fr))
+    fr = frame.lf_frame(S, pic.ctypes.data, masks.ctypes.data, S["level"].ctypes.data)
+    if sb128 is not None:
+        fr.sb128 = sb128
+    (refs.ref().refdrv_lf_frame_8bpc if S["bpc"] == 8 else refs.ref().refdrv_lf_frame_16bpc)(S["bd"], C.byref(fr))
     return pic
+
+
+def lf_frame_buffers(S, alloc):
+    """S's picture, masks and levels placed by `alloc` (keep the handles while the library uses them), and the
+    B200LfFrame over them"""
+    bufs = [alloc.upload(S[k]) for k in ("pic", "masks", "level")]
+    return bufs, frame.lf_frame(S, *(ptr for _, ptr in bufs))
+
+
+def lf_frame_lib(S, lib, alloc):
+    """b200_lf_frame on S's picture, masks and levels placed by `alloc`"""
+    bufs, fr = lf_frame_buffers(S, alloc)
+    lib.check(lib.b200_lf_frame(S["bd"], C.byref(fr), None), "b200_lf_frame")
+    alloc.sync()
+    return alloc.download(bufs[0][0], S["pic"])
 
 
 @pytest.mark.parametrize("bpc", [8, 10, 12])
@@ -167,12 +168,7 @@ def test_emu_lpf_level1(bpc):
 @pytest.mark.parametrize("bpc,W,H,ssh,ssv", [(8, 200, 136, 1, 1), (10, 136, 72, 0, 0)])
 def test_emu_lf_frame(bpc, W, H, ssh, ssv):
     S = synth.make_lf_frame(np.random.default_rng(320 + bpc), bpc, W, H, ssh, ssv)
-    exp = lf_frame_oracle(S)
-    pic = S["pic"].copy()
-    lib = refs.emu_lib()
-    fr = lf_frame_struct(S, pic.ctypes.data, S["masks"].ctypes.data, S["level"].ctypes.data)
-    lib.check(lib.b200_lf_frame(S["bd"], C.byref(fr), None), "lf_frame")
-    assert np.array_equal(pic, exp)
+    assert np.array_equal(lf_frame_lib(S, *refs.lib_alloc(False)), lf_frame_oracle(S))
 
 
 @pytest.mark.gpu
@@ -188,17 +184,7 @@ def test_gpu_lpf_level1(bpc):
 @pytest.mark.parametrize("bpc,W,H,ssh,ssv", [(8, 1920, 1080, 1, 1), (10, 1280, 720, 1, 0), (12, 648, 360, 0, 0),
                                              (8, 3840, 2160, 1, 1)])
 def test_gpu_lf_frame(bpc, W, H, ssh, ssv):
-    import torch
-    from dav1d_b200 import get_lib
     S = synth.make_lf_frame(np.random.default_rng(330 + bpc + W), bpc, W, H, ssh, ssv)
     exp = lf_frame_reference(S) if refs.have_ref() else lf_frame_oracle(S)
     assert np.array_equal(exp, lf_frame_oracle(S))
-    lib = get_lib()
-    d_pic = torch.from_numpy(S["pic"].view(np.uint8).copy()).cuda()
-    d_mask = torch.from_numpy(S["masks"].view(np.uint8).copy()).cuda()
-    d_lvl = torch.from_numpy(S["level"].reshape(-1).copy()).cuda()
-    fr = lf_frame_struct(S, d_pic.data_ptr(), d_mask.data_ptr(), d_lvl.data_ptr())
-    lib.check(lib.b200_lf_frame(S["bd"], C.byref(fr), None), "lf_frame")
-    torch.cuda.synchronize()
-    got = d_pic.cpu().numpy().view(S["pic"].dtype)
-    assert np.array_equal(got, exp)
+    assert np.array_equal(lf_frame_lib(S, *refs.lib_alloc(True)), exp)

@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 import refs
-from dav1d_b200 import _lib, synth
+from dav1d_b200 import frame, synth
 
 
 class LrParams(C.Union):
@@ -123,29 +123,26 @@ def make_lr_frame(rng, bpc, W, H, ssh, ssv, sb128, us, rp):
     return S
 
 
-def lr_frame_struct(S, cdef, dbl, dst, lrm):
-    fr = _lib.LrFrame()
-    fr.cdef, fr.dbl, fr.dst = cdef, dbl, dst
-    for p in range(3):
-        fr.plane_off[p] = S["off"][p]; fr.stride[p] = S["stride"][p]
-    fr.w, fr.h, fr.ss_hor, fr.ss_ver, fr.sb128, fr.sr_sb128w = S["W"], S["H"], S["ss_hor"], S["ss_ver"], S["sb128"], (S["W"] + 127) >> 7
-    fr.unit_size_log2[0], fr.unit_size_log2[1] = S["us"]
-    fr.restore_planes, fr.lr_mask = S["rp"], lrm
-    return fr
-
-
 def lr_frame_oracle(S):
     dst = np.zeros_like(S["cdef"])
-    fr = lr_frame_struct(S, S["cdef"].ctypes.data, S["dbl"].ctypes.data, dst.ctypes.data, S["lr_mask"].ctypes.data)
+    fr = frame.lr_frame(S, S["cdef"].ctypes.data, S["dbl"].ctypes.data, dst.ctypes.data, S["lr_mask"].ctypes.data)
     refs.oracle().oracle_lr_frame(S["bd"], C.byref(fr))
     return dst
 
 
 def lr_frame_reference(S):
     c2 = S["cdef"].copy()
-    fr = lr_frame_struct(S, c2.ctypes.data, S["dbl"].ctypes.data, None, S["lr_mask"].ctypes.data)
+    fr = frame.lr_frame(S, c2.ctypes.data, S["dbl"].ctypes.data, None, S["lr_mask"].ctypes.data)
     (refs.ref().refdrv_lr_frame_8bpc if S["bpc"] == 8 else refs.ref().refdrv_lr_frame_16bpc)(S["bd"], C.byref(fr))
     return c2
+
+
+def lr_frame_lib(S, lib, alloc):
+    """b200_lr_frame on S's CDEF and deblocked pictures and restoration units placed by `alloc`"""
+    cdef, dbl, dst, lrm = alloc.upload(S["cdef"]), alloc.upload(S["dbl"]), alloc.zeros(S["cdef"].nbytes), alloc.upload(S["lr_mask"])
+    lib.check(lib.b200_lr_frame(S["bd"], C.byref(frame.lr_frame(S, cdef[1], dbl[1], dst[1], lrm[1])), None), "b200_lr_frame")
+    alloc.sync()
+    return alloc.download(dst[0], S["cdef"])
 
 
 def picture_equal(S, a, b):
@@ -192,12 +189,7 @@ def test_emu_lr_level1(bpc):
 @pytest.mark.parametrize("case", [FRAME_CASES[0], FRAME_CASES[2], FRAME_CASES[5]])
 def test_emu_lr_frame(case):
     S = make_lr_frame(np.random.default_rng(530 + case[1]), *case)
-    exp = lr_frame_oracle(S)
-    dst = np.zeros_like(S["cdef"])
-    lib = refs.emu_lib()
-    fr = lr_frame_struct(S, S["cdef"].ctypes.data, S["dbl"].ctypes.data, dst.ctypes.data, S["lr_mask"].ctypes.data)
-    lib.check(lib.b200_lr_frame(S["bd"], C.byref(fr), None), "lr_frame")
-    assert picture_equal(S, dst, exp)
+    assert picture_equal(S, lr_frame_lib(S, *refs.lib_alloc(False)), lr_frame_oracle(S))
 
 
 @pytest.mark.gpu
@@ -211,17 +203,6 @@ def test_gpu_lr_level1(bpc):
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", FRAME_CASES + [(8, 1920, 1080, 1, 1, 0, (6, 6), 7), (10, 3840, 2160, 1, 1, 1, (8, 7), 7)])
 def test_gpu_lr_frame(case):
-    import torch
-    from dav1d_b200 import get_lib
     S = make_lr_frame(np.random.default_rng(550 + case[1]), *case)
     exp = lr_frame_reference(S) if refs.have_ref() else lr_frame_oracle(S)
-    lib = get_lib()
-    d_c = torch.from_numpy(S["cdef"].view(np.uint8).copy()).cuda()
-    d_d = torch.from_numpy(S["dbl"].view(np.uint8).copy()).cuda()
-    d_o = torch.zeros_like(d_c)
-    d_m = torch.from_numpy(S["lr_mask"].view(np.uint8).copy()).cuda()
-    fr = lr_frame_struct(S, d_c.data_ptr(), d_d.data_ptr(), d_o.data_ptr(), d_m.data_ptr())
-    lib.check(lib.b200_lr_frame(S["bd"], C.byref(fr), None), "lr_frame")
-    torch.cuda.synchronize()
-    got = d_o.cpu().numpy().view(S["cdef"].dtype)
-    assert picture_equal(S, got, exp)
+    assert picture_equal(S, lr_frame_lib(S, *refs.lib_alloc(True)), exp)

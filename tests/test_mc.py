@@ -438,14 +438,13 @@ def dedupe_writes(S):
     return S
 
 
-def run_mc_frame_lib(S, lib, to_dev, from_dev, sync):
+def run_mc_frame_lib(S, lib, alloc):
     import ctypes as C
-    dev = {k: to_dev(S[k]) for k in ("refpic", "dst", "tmp", "mask", "px_tmp")}
+    dev = {k: alloc.upload(S[k]) for k in ("refpic", "dst", "tmp", "mask", "px_tmp")}
     fr = mc_frame_struct(S, {k: v[1] for k, v in dev.items()})
 
     def up(arr, n, cls):
-        raw = np.frombuffer(bytes(arr), np.uint8)[:max(1, n) * C.sizeof(cls)].copy()
-        return to_dev(raw)
+        return alloc.upload(np.frombuffer(arr, np.uint8)[:max(1, n) * C.sizeof(cls)])
     d_b = up(S["blocks"], S["n_pred"], type(S["blocks"][0]))
     d_c = up(S["carr"], S["n_comp"], type(S["carr"][0]))
     d_l = up(S["bl"], S["nb"], type(S["bl"][0]))
@@ -454,8 +453,8 @@ def run_mc_frame_lib(S, lib, to_dev, from_dev, sync):
     lib.check(lib.b200_mc_comp_batch(S["bd"], C.byref(fr), d_c[1], S["n_comp"], None), "comp")
     lib.check(lib.b200_mc_blend_batch(S["bd"], C.byref(fr), d_l[1], S["nb"], None), "blend")
     lib.check(lib.b200_mc_warp_batch(S["bd"], C.byref(fr), d_w[1], S["nw"], None), "warp")
-    sync()
-    return {k: from_dev(v, S[k]) for k, v in dev.items()}
+    alloc.sync()
+    return {k: alloc.download(v[0], S[k]) for k, v in dev.items()}
 
 
 def compare_mc_frame(exp, got):
@@ -469,27 +468,13 @@ def test_emu_mc_frame(bpc):
     rng = np.random.default_rng(90 + bpc)
     S = dedupe_writes(make_mc_frame(rng, bpc, n_pred=60))
     exp = run_mc_frame_oracle(S)
-    keep = []
-
-    def to_dev(a):
-        c = a.copy(); keep.append(c)
-        return (c, c.ctypes.data)
-    got = run_mc_frame_lib(S, refs.emu_lib(), to_dev, lambda v, like: v[0], lambda: None)
-    compare_mc_frame(exp, got)
+    compare_mc_frame(exp, run_mc_frame_lib(S, *refs.lib_alloc(False)))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("bpc", [8, 10, 12])
 def test_gpu_mc_frame(bpc):
-    import torch
-    from dav1d_b200 import get_lib
     rng = np.random.default_rng(95 + bpc)
     S = dedupe_writes(make_mc_frame(rng, bpc, W=320, H=192, n_pred=900))
     exp = run_mc_frame_oracle(S)
-
-    def to_dev(a):
-        t = torch.from_numpy(a.view(np.uint8).copy()).cuda()
-        return (t, t.data_ptr())
-    got = run_mc_frame_lib(S, get_lib(), to_dev, lambda v, like: v[0].cpu().numpy().view(like.dtype),
-                           torch.cuda.synchronize)
-    compare_mc_frame(exp, got)
+    compare_mc_frame(exp, run_mc_frame_lib(S, *refs.lib_alloc(True)))

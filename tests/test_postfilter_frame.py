@@ -25,11 +25,13 @@ import numpy as np
 import pytest
 
 import refs
-from dav1d_b200 import _lib, get_lib, synth
-from test_cdef import cdef_frame_struct
-from test_looprestoration import lr_frame_struct
-from test_postfilter_mapping import WIENER_EXTREMES
+from dav1d_b200 import _lib, frame, synth
+from test_cdef import cdef_frame_oracle, cdef_frame_reference
+from test_looprestoration import lr_frame_oracle, lr_frame_reference
+from test_loopfilter import lf_frame_oracle
+from test_postfilter_mapping import WIENER_EXTREMES, run_cdef, run_lr
 import test_deblock_frame as TDF
+from test_deblock_frame import plane
 
 LAYOUTS = {"420": (1, 1), "422": (1, 0), "444": (0, 0), "400": (1, 1)}
 
@@ -37,10 +39,6 @@ CDEF_COUNTERS = ("skip_idx", "skip_noskip", "skip_zero", "pri_sec", "pri", "sec"
                  *("dir%d" % d for d in range(8)), "edge_l", "edge_r", "edge_t", "edge_b", "clamp_px", "tap_dropped")
 LR_COUNTERS = ("none", "wiener", "sgr5", "sgr3", "sgr_mix", "ext_h", "pulled_up", "hor_clip_lo", "hor_clip_hi",
                "out_clip_lo", "out_clip_hi", "z0", "z255", "sgr_big", "top", "no_top", "bot", "no_bot", "bot_clamp")
-
-
-def plane(S, pic, p):
-    return pic[S["off"][p]:S["off"][p] + S["stride"][p] * S["rows"][p]].reshape(S["rows"][p], S["stride"][p])
 
 
 def base_frame(rng, lay, bpc, W, H):
@@ -138,19 +136,6 @@ def make_cdef_case(lay, bpc, W, H, damping, seed):
     return S
 
 
-def cdef_oracle(S):
-    dst = S["pic"].copy()
-    refs.oracle().oracle_cdef_frame(S["bd"], C.byref(cdef_frame_struct(S, S["pic"].ctypes.data, dst.ctypes.data, S["masks"].ctypes.data)))
-    return dst
-
-
-def cdef_reference(S):
-    pic = S["pic"].copy()
-    fr = cdef_frame_struct(S, pic.ctypes.data, None, S["masks"].ctypes.data)
-    (refs.ref().refdrv_cdef_frame_8bpc if S["bpc"] == 8 else refs.ref().refdrv_cdef_frame_16bpc)(S["bd"], C.byref(fr))
-    return pic
-
-
 def cdef_counts():
     out = np.zeros(2 * len(CDEF_COUNTERS), np.int64)
     assert refs.oracle().oracle_cdef_counts(C.c_void_p(out.ctypes.data)) == len(CDEF_COUNTERS)
@@ -213,7 +198,7 @@ def cdef_below_floor(S, counts):
 def test_cdef_content_reaches_every_branch(case):
     S = cdef_frame(case)
     cdef_counts()
-    cdef_oracle(S)
+    cdef_frame_oracle(S)
     counts = cdef_counts()
     assert not cdef_below_floor(S, counts), (cdef_below_floor(S, counts), counts)
 
@@ -222,7 +207,7 @@ def test_cdef_edges_over_the_cases():
     total = np.zeros((2, 4), np.int64)
     for case in CDEF_CASES:
         cdef_counts()
-        cdef_oracle(cdef_frame(case))
+        cdef_frame_oracle(cdef_frame(case))
         total += [[c[k] for k in ("edge_l", "edge_r", "edge_t", "edge_b")] for c in cdef_counts()]
     assert (total >= 50).all(), total
 
@@ -241,47 +226,16 @@ def test_cdef_oracle_vs_reference_driver(case):
     if not refs.have_ref():
         pytest.skip("reference build (oracle/_ref) not present")
     S = cdef_frame(case)
-    exp = cdef_oracle(S)
-    assert cdef_area_diff(S, exp, cdef_reference(S)) == [0, 0, 0]
+    exp = cdef_frame_oracle(S)
+    assert cdef_area_diff(S, exp, cdef_frame_reference(S)) == [0, 0, 0]
     assert sum(cdef_area_diff(S, exp, S["pic"])[:1 if S["lay"] == "400" else 3]) > 0
 
 
-class Pics:
-    """named pictures of a case where the library reads them: host memory for the emulator, HBM for the GPU"""
-
-    def __init__(self, gpu, **arrays):
-        self.gpu, self.dtype = gpu, next(iter(arrays.values())).dtype
-        self.lib = get_lib() if gpu else refs.emu_lib()
-        self.a = {}
-        for k, v in arrays.items():
-            if gpu:
-                import torch
-                self.a[k] = torch.from_numpy(np.ascontiguousarray(v).view(np.uint8).copy()).cuda()
-            else:
-                self.a[k] = np.ascontiguousarray(v).copy()
-
-    def ptr(self, k):
-        return self.a[k].data_ptr() if self.gpu else self.a[k].ctypes.data
-
-    def get(self, k):
-        if not self.gpu:
-            return self.a[k].copy()
-        import torch
-        torch.cuda.synchronize()
-        return self.a[k].cpu().numpy().view(self.dtype)
-
-
-def run_cdef(S, gpu):
-    d = Pics(gpu, src=S["pic"], dst=np.zeros_like(S["pic"]), mask=S["masks"].view(np.uint8))
-    d.lib.check(d.lib.b200_cdef_frame(S["bd"], C.byref(cdef_frame_struct(S, d.ptr("src"), d.ptr("dst"), d.ptr("mask"))), None), "b200_cdef_frame")
-    return d.get("dst")
-
-
 def check_cdef(S, gpu, reference=False):
-    got, exp = run_cdef(S, gpu), cdef_oracle(S)
+    got, exp = run_cdef(S, gpu), cdef_frame_oracle(S)
     assert cdef_area_diff(S, got, exp) == [0, 0, 0]
     if reference and refs.have_ref():
-        assert cdef_area_diff(S, got, cdef_reference(S)) == [0, 0, 0]
+        assert cdef_area_diff(S, got, cdef_frame_reference(S)) == [0, 0, 0]
 
 
 @pytest.mark.emu
@@ -293,11 +247,12 @@ def test_emu_cdef_frame(case):
 def check_cdef_misaligned(gpu):
     """stride / plane offsets that are not 4-sample multiples: -2, and dst untouched"""
     S = relayout(cdef_frame(CDEF_CASES[0]), 1)
-    d = Pics(gpu, src=S["pic"], dst=np.full_like(S["pic"], 7), mask=S["masks"].view(np.uint8))
-    fr = cdef_frame_struct(S, d.ptr("src"), d.ptr("dst"), d.ptr("mask"))
-    assert d.lib.b200_cdef_frame(S["bd"], C.byref(fr), None) == -2
-    assert b"4-sample aligned" in d.lib.b200_last_error()
-    assert (d.get("dst") == 7).all()
+    lib, A = refs.lib_alloc(gpu)
+    src, dst, mask = A.upload(S["pic"]), A.upload(np.full_like(S["pic"], 7)), A.upload(S["masks"])
+    assert lib.b200_cdef_frame(S["bd"], C.byref(frame.cdef_frame(S, src[1], dst[1], mask[1])), None) == -2
+    assert b"4-sample aligned" in lib.b200_last_error()
+    A.sync()
+    assert (A.download(dst[0], S["pic"]) == 7).all()
 
 
 @pytest.mark.emu
@@ -425,20 +380,6 @@ def last_stripe_rows(S, p):
     return y1 - y0
 
 
-def lr_oracle(S):
-    dst = np.zeros_like(S["cdef"])
-    fr = lr_frame_struct(S, S["cdef"].ctypes.data, S["dbl"].ctypes.data, dst.ctypes.data, S["lr_mask"].ctypes.data)
-    refs.oracle().oracle_lr_frame(S["bd"], C.byref(fr))
-    return dst
-
-
-def lr_reference(S):
-    c2 = S["cdef"].copy()
-    fr = lr_frame_struct(S, c2.ctypes.data, S["dbl"].ctypes.data, None, S["lr_mask"].ctypes.data)
-    (refs.ref().refdrv_lr_frame_8bpc if S["bpc"] == 8 else refs.ref().refdrv_lr_frame_16bpc)(S["bd"], C.byref(fr))
-    return c2
-
-
 def lr_counts():
     out = np.zeros(2 * len(LR_COUNTERS), np.int64)
     assert refs.oracle().oracle_lr_counts(C.c_void_p(out.ctypes.data)) == len(LR_COUNTERS)
@@ -504,7 +445,7 @@ def lr_below_floor(total):
 def test_lr_stripes_and_units_follow_the_geometry(case):
     S = lr_frame(case)
     lr_counts()
-    lr_oracle(S)
+    lr_frame_oracle(S)
     counts = lr_counts()
     assert not lr_geometry_mismatch(S, counts), (lr_geometry_mismatch(S, counts), counts)
 
@@ -513,7 +454,7 @@ def test_lr_content_reaches_every_branch():
     total = [dict.fromkeys(LR_COUNTERS, 0) for _ in range(2)]
     for case in LR_CASES:
         lr_counts()
-        lr_oracle(lr_frame(case))
+        lr_frame_oracle(lr_frame(case))
         for pc, c in enumerate(lr_counts()):
             for k, v in c.items():
                 total[pc][k] += v if k != "sgr_big" or case[1] == 12 else 0
@@ -551,22 +492,15 @@ def test_lr_oracle_vs_reference_driver(case):
     S = lr_frame(case)
     for sb128 in (0, 1) if sb128_legal(S) else (0,):
         S["sb128"] = sb128
-        exp = lr_oracle(S)
-        assert lr_diff(S, exp, lr_reference(S)) == [0, 0, 0], sb128
-
-
-def run_lr(S, gpu):
-    d = Pics(gpu, cdef=S["cdef"], dbl=S["dbl"], dst=np.zeros_like(S["cdef"]), mask=S["lr_mask"].view(np.uint8))
-    fr = lr_frame_struct(S, d.ptr("cdef"), d.ptr("dbl"), d.ptr("dst"), d.ptr("mask"))
-    d.lib.check(d.lib.b200_lr_frame(S["bd"], C.byref(fr), None), "b200_lr_frame")
-    return d.get("dst")
+        exp = lr_frame_oracle(S)
+        assert lr_diff(S, exp, lr_frame_reference(S)) == [0, 0, 0], sb128
 
 
 def check_lr(S, gpu, reference=False):
-    got, exp = run_lr(S, gpu), lr_oracle(S)
+    got, exp = run_lr(S, gpu), lr_frame_oracle(S)
     assert lr_diff(S, got, exp) == [0, 0, 0]
     if reference and refs.have_ref():
-        assert lr_diff(S, got, lr_reference(S)) == [0, 0, 0]
+        assert lr_diff(S, got, lr_frame_reference(S)) == [0, 0, 0]
 
 
 @pytest.mark.emu
@@ -607,12 +541,12 @@ def band_frame(lay, bpc, W, H):
 
 def chain_oracle(S, run_lf, run_cdef, run_lr):
     """the oracle's pictures after each enabled stage, as the hooks wire them: LR reads p0 when CDEF is off"""
-    p0 = TDF.run_oracle(S) if run_lf else S["pic"].copy()
+    p0 = lf_frame_oracle(S) if run_lf else S["pic"].copy()
     T = dict(S, pic=p0)
-    p1 = cdef_oracle(T) if run_cdef else None
+    p1 = cdef_frame_oracle(T) if run_cdef else None
     p2 = None
     if run_lr:
-        p2 = lr_oracle(dict(S, cdef=p1 if run_cdef else p0, dbl=p0))
+        p2 = lr_frame_oracle(dict(S, cdef=p1 if run_cdef else p0, dbl=p0))
     return p0, p1, p2
 
 
@@ -621,25 +555,30 @@ class Job:
 
     def __init__(self, S, gpu, run_lf, run_cdef, run_lr):
         self.S = S
-        z = np.zeros_like(S["pic"])
-        self.d = Pics(gpu, p0=S["pic"], p1=z, p2=z, mask=S["masks"].view(np.uint8), level=S["level"].reshape(-1),
-                      lrm=S["lr_mask"].view(np.uint8))
-        d = self.d
+        self.lib, self.A = refs.lib_alloc(gpu)
+        n = S["pic"].nbytes
+        self.b = dict(p0=self.A.upload(S["pic"]), p1=self.A.zeros(n), p2=self.A.zeros(n), mask=self.A.upload(S["masks"]),
+                      level=self.A.upload(S["level"]), lrm=self.A.upload(S["lr_mask"]))
+        ptr = {k: v[1] for k, v in self.b.items()}
         job = _lib.FrameJob()
         job.bitdepth_max, job.run_lf, job.run_cdef, job.run_lr = S["bd"], run_lf, run_cdef, run_lr
-        job.lf = TDF.lf_struct(S, d.ptr("p0"), d.ptr("mask"), d.ptr("level"))      # lf.h4 / ss_ver: the band geometry
-        job.cdef = cdef_frame_struct(S, d.ptr("p0"), d.ptr("p1"), d.ptr("mask"))
-        job.lr = lr_frame_struct(S, d.ptr("p1" if run_cdef else "p0"), d.ptr("p0"), d.ptr("p2"), d.ptr("lrm"))
+        job.lf = frame.lf_frame(S, ptr["p0"], ptr["mask"], ptr["level"])      # lf.h4 / ss_ver: the band geometry
+        job.cdef = frame.cdef_frame(S, ptr["p0"], ptr["p1"], ptr["mask"])
+        job.lr = frame.lr_frame(S, ptr["p1" if run_cdef else "p0"], ptr["p0"], ptr["p2"], ptr["lrm"])
         self.job, self.out = job, "p2" if run_lr else "p1" if run_cdef else "p0"
 
     def run(self):
-        self.d.lib.check(self.d.lib.b200_frame_run(C.byref(self.job), None), "b200_frame_run")
+        self.lib.check(self.lib.b200_frame_run(C.byref(self.job), None), "b200_frame_run")
 
     def run_band(self, y0, y1, last):
-        self.d.lib.check(self.d.lib.b200_frame_run_band(C.byref(self.job), C.byref(TDF.band(y0, y1, last)), None), "b200_frame_run_band")
+        self.lib.check(self.lib.b200_frame_run_band(C.byref(self.job), C.byref(TDF.band(y0, y1, last)), None), "b200_frame_run_band")
 
     def progress(self, y1, last, p):
-        return self.d.lib.b200_band_progress(C.byref(self.job), y1, last, p)
+        return self.lib.b200_band_progress(C.byref(self.job), y1, last, p)
+
+    def output(self):
+        self.A.sync()
+        return self.A.download(self.b[self.out][0], self.S["pic"])
 
 
 def final_diff(S, a, b, rows=None):
@@ -658,7 +597,7 @@ def check_bands(S, gpu, sets=FILTER_SETS):
         exp = chain_oracle(S, *flags)[2 if flags[2] else 1 if flags[1] else 0]
         j = Job(S, gpu, *flags)
         j.run()
-        assert final_diff(S, j.d.get(j.out), exp) == [0, 0, 0], (name, "whole frame")
+        assert final_diff(S, j.output(), exp) == [0, 0, 0], (name, "whole frame")
         for rows in (64, 128, 192):
             j = Job(S, gpu, *flags)
             prev = [0, 0, 0]
@@ -668,10 +607,10 @@ def check_bands(S, gpu, sets=FILTER_SETS):
                 claim = [j.progress(y1, last, p) for p in range(3)]
                 # rows reported final are final; the claim moves forward and reaches the plane height at the last band
                 assert all(prev[p] <= claim[p] for p in range(3)), (name, rows, y1, prev, claim)
-                assert final_diff(S, j.d.get(j.out), exp, claim) == [0, 0, 0], (name, rows, y1, claim)
+                assert final_diff(S, j.output(), exp, claim) == [0, 0, 0], (name, rows, y1, claim)
                 prev = claim
             assert prev == [plane_dims(S, p)[1] for p in range(3)], (name, rows, prev)
-            assert final_diff(S, j.d.get(j.out), exp) == [0, 0, 0], (name, rows)
+            assert final_diff(S, j.output(), exp) == [0, 0, 0], (name, rows)
 
 
 def test_band_cases_cover_layouts_and_short_stripes():

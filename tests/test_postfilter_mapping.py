@@ -8,14 +8,13 @@ Loop restoration: every sgr_idx, Wiener taps at the ends of their legal ranges, 
 that end inside a 32-bit word of samples (the tiles' word staging, word copy and row stores).
 Each case runs on the host emulator and on the GPU.
 """
-import ctypes as C
 import numpy as np
 import pytest
 
 import refs
 from dav1d_b200 import synth
-from test_cdef import make_cdef_frame, cdef_frame_struct, cdef_frame_oracle, frame_area_equal, oracle_cdef
-from test_looprestoration import make_lr_frame, lr_frame_struct, lr_frame_oracle, picture_equal
+from test_cdef import make_cdef_frame, cdef_frame_lib, cdef_frame_oracle, frame_area_equal, oracle_cdef
+from test_looprestoration import make_lr_frame, lr_frame_lib, lr_frame_oracle, picture_equal
 
 CDEF_WIDTHS = [(8, 64 + 4 * k, 44, 1, 1) for k in range(1, 17)] + [(10, 100, 52, 1, 0), (12, 76, 36, 0, 0)]
 # (y, uv) strength tables: pri + sec, pri only, sec only, neither, at the extremes (pri 15 / 1, sec 4 / 1)
@@ -34,22 +33,7 @@ def cdef_case(bpc, W, H, ssh, ssv, seed, damping=None, strengths=None):
 
 
 def run_cdef(S, gpu):
-    if not gpu:
-        dst = np.zeros_like(S["pic"])
-        lib = refs.emu_lib()
-        fr = cdef_frame_struct(S, S["pic"].ctypes.data, dst.ctypes.data, S["masks"].ctypes.data)
-        lib.check(lib.b200_cdef_frame(S["bd"], C.byref(fr), None), "cdef_frame")
-        return dst
-    import torch
-    from dav1d_b200 import get_lib
-    lib = get_lib()
-    d_src = torch.from_numpy(S["pic"].view(np.uint8).copy()).cuda()
-    d_dst = torch.zeros_like(d_src)
-    d_mask = torch.from_numpy(S["masks"].view(np.uint8).copy()).cuda()
-    fr = cdef_frame_struct(S, d_src.data_ptr(), d_dst.data_ptr(), d_mask.data_ptr())
-    lib.check(lib.b200_cdef_frame(S["bd"], C.byref(fr), None), "cdef_frame")
-    torch.cuda.synchronize()
-    return d_dst.cpu().numpy().view(S["pic"].dtype)
+    return cdef_frame_lib(S, *refs.lib_alloc(gpu))
 
 
 def oriented_blocks(bpc):
@@ -93,23 +77,7 @@ def lr_case(bpc, W, H, ssh, ssv, us, seed, types=None, taps=None):
 
 
 def run_lr(S, gpu):
-    if not gpu:
-        dst = np.zeros_like(S["cdef"])
-        lib = refs.emu_lib()
-        fr = lr_frame_struct(S, S["cdef"].ctypes.data, S["dbl"].ctypes.data, dst.ctypes.data, S["lr_mask"].ctypes.data)
-        lib.check(lib.b200_lr_frame(S["bd"], C.byref(fr), None), "lr_frame")
-        return dst
-    import torch
-    from dav1d_b200 import get_lib
-    lib = get_lib()
-    d_c = torch.from_numpy(S["cdef"].view(np.uint8).copy()).cuda()
-    d_d = torch.from_numpy(S["dbl"].view(np.uint8).copy()).cuda()
-    d_o = torch.zeros_like(d_c)
-    d_m = torch.from_numpy(S["lr_mask"].view(np.uint8).copy()).cuda()
-    fr = lr_frame_struct(S, d_c.data_ptr(), d_d.data_ptr(), d_o.data_ptr(), d_m.data_ptr())
-    lib.check(lib.b200_lr_frame(S["bd"], C.byref(fr), None), "lr_frame")
-    torch.cuda.synchronize()
-    return d_o.cpu().numpy().view(S["cdef"].dtype)
+    return lr_frame_lib(S, *refs.lib_alloc(gpu))
 
 
 # every sgr_idx (types 3 .. 18) and Wiener with none mixed in, at 8 and 10 bit

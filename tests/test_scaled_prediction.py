@@ -200,9 +200,9 @@ def scaled_batch_reference(B, ctx):
     return out
 
 
-def run_scaled_batch(B, lib, to_dev, from_dev, sync):
-    dev = {k: to_dev(B[k]) for k in ("dst", "tmp", "px_tmp")}
-    pics = [to_dev(p) for p in B["pics"]]
+def run_scaled_batch(B, lib, alloc):
+    dev = {k: alloc.upload(B[k]) for k in ("dst", "tmp", "px_tmp")}
+    pics = [alloc.upload(p) for p in B["pics"]]
     fr = _lib.McFrame()
     f = B["frame"]
     for p in range(3):
@@ -216,10 +216,10 @@ def run_scaled_batch(B, lib, to_dev, from_dev, sync):
                 rg.plane_off[p], rg.stride[p], rg.w[p], rg.h[p] = g["off"][p], g["stride"][p], g["w"][p], g["h"][p]
     fr.scaled_mask = B["mask"]
     fr.dst, fr.tmp, fr.px_tmp = dev["dst"][1], dev["tmp"][1], dev["px_tmp"][1]
-    recs = to_dev(np.frombuffer(bytes(B["recs"]), np.uint8).copy())
+    recs = alloc.upload(np.frombuffer(B["recs"], np.uint8))
     lib.check(lib.b200_mc_scaled_batch(B["bd"], C.byref(fr), recs[1], B["n"], None), "b200_mc_scaled_batch")
-    sync()
-    return {k: from_dev(v, B[k]) for k, v in dev.items()}
+    alloc.sync()
+    return {k: alloc.download(v[0], B[k]) for k, v in dev.items()}
 
 
 def compare(B, exp, got):
@@ -231,28 +231,6 @@ def compare(B, exp, got):
     assert ops.min() > 0, ops
 
 
-def _emu_dev(keep):
-    def to_dev(a):
-        c = a.copy(); keep.append(c)
-        return (c, c.ctypes.data)
-    return to_dev
-
-
-def _torch_dev(a):
-    import torch
-    t = torch.from_numpy(a.view(np.uint8).copy()).cuda()
-    return (t, t.data_ptr())
-
-
-def _torch_host(v, like):
-    return v[0].cpu().numpy().view(like.dtype)
-
-
-def _torch_sync():
-    import torch
-    torch.cuda.synchronize()
-
-
 # ------------------------------------------------------------------ 1. b200_mc_scaled_batch
 SCALED_EMU = [(bpc, lay) for bpc in (8, 10, 12) for lay in ("420", "422", "444", "400")]
 
@@ -262,9 +240,7 @@ SCALED_EMU = [(bpc, lay) for bpc in (8, 10, 12) for lay in ("420", "422", "444",
 def test_emu_scaled_batch(bpc, layout):
     B = make_scaled_batch(np.random.default_rng(1100 + 10 * bpc + list(LAYOUTS).index(layout)), bpc, layout, 200, 136, 300)
     exp = scaled_batch_reference(B, checker(bpc))
-    keep = []
-    got = run_scaled_batch(B, refs.emu_lib(), _emu_dev(keep), lambda v, like: v[0], lambda: None)
-    compare(B, exp, got)
+    compare(B, exp, run_scaled_batch(B, *refs.lib_alloc(False)))
 
 
 def test_oracle_scaled_batch_matches_reference():
@@ -283,11 +259,9 @@ def test_oracle_scaled_batch_matches_reference():
 @pytest.mark.parametrize("bpc,layout,W,H,n", [(8, "420", 1920, 1080, 3000), (10, "420", 3840, 2160, 5000),
                                               (12, "444", 1280, 720, 2500), (10, "422", 1280, 720, 2500)])
 def test_gpu_scaled_batch(bpc, layout, W, H, n):
-    from dav1d_b200 import get_lib
     B = make_scaled_batch(np.random.default_rng(1200 + W + bpc), bpc, layout, W, H, n)
     exp = scaled_batch_reference(B, checker(bpc))
-    got = run_scaled_batch(B, get_lib(), _torch_dev, _torch_host, _torch_sync)
-    compare(B, exp, got)
+    compare(B, exp, run_scaled_batch(B, *refs.lib_alloc(True)))
 
 
 # ------------------------------------------------------------------ 2. b200_resize_frame
@@ -331,13 +305,13 @@ def resize_reference(R, ctx):
     return dst
 
 
-def run_resize(R, lib, to_dev, from_dev, sync):
-    src, dst = to_dev(R["src"]), to_dev(R["dst"])
+def run_resize(R, lib, alloc):
+    src, dst = alloc.upload(R["src"]), alloc.upload(R["dst"])
     fr = _lib.ResizeFrame.from_buffer_copy(R["fr"])
     fr.src, fr.dst = src[1], dst[1]
     lib.check(lib.b200_resize_frame(R["bd"], C.byref(fr), None), "b200_resize_frame")
-    sync()
-    return from_dev(dst, R["dst"])
+    alloc.sync()
+    return alloc.download(dst[0], R["dst"])
 
 
 def check_resize(R, exp, got):
@@ -368,17 +342,15 @@ RESIZE_GPU = [(8, "420", 1921, 1080, 9), (10, "420", 3839, 2160, 10), (10, "420"
 def test_emu_resize_frame(bpc, layout, out_w, H, den):
     R = make_resize_frame(np.random.default_rng(1300 + out_w), bpc, layout, out_w, H, den)
     exp = resize_reference(R, checker(bpc))
-    keep = []
-    check_resize(R, exp, run_resize(R, refs.emu_lib(), _emu_dev(keep), lambda v, like: v[0], lambda: None))
+    check_resize(R, exp, run_resize(R, *refs.lib_alloc(False)))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("bpc,layout,out_w,H,den", RESIZE_GPU)
 def test_gpu_resize_frame(bpc, layout, out_w, H, den):
-    from dav1d_b200 import get_lib
     R = make_resize_frame(np.random.default_rng(1400 + out_w), bpc, layout, out_w, H, den)
     exp = resize_reference(R, checker(bpc))
-    check_resize(R, exp, run_resize(R, get_lib(), _torch_dev, _torch_host, _torch_sync))
+    check_resize(R, exp, run_resize(R, *refs.lib_alloc(True)))
 
 
 def _resize_arguments(lib):
