@@ -379,14 +379,14 @@ class ExportJob(C.Structure):
 
 class TensorJob(C.Structure):
     """B200TensorJob: export of a decoded picture as a resized, normalised float tensor (dtype 0 fp32, 1 fp16, 2 bf16;
-    layout 0 CHW, 1 HWC) into caller memory"""
+    layout 0 CHW, 1 HWC; flip 1 mirrors it horizontally) into caller memory"""
     _fields_ = [("src", C.c_void_p), ("plane_off", C.c_uint32 * 3), ("stride", C.c_int32 * 3), ("w", C.c_int32), ("h", C.c_int32),
                 ("ss_hor", C.c_int32), ("ss_ver", C.c_int32), ("mono", C.c_int32), ("bitdepth_max", C.c_int32),
                 ("out_w", C.c_int32), ("out_h", C.c_int32), ("dtype", C.c_int32), ("layout", C.c_int32),
                 ("full_range", C.c_int32), ("identity", C.c_int32), ("siting_x", C.c_int32), ("siting_y", C.c_int32),
                 ("cy", C.c_int32), ("rv", C.c_int32), ("gu", C.c_int32), ("gv", C.c_int32), ("bu", C.c_int32),
                 ("scale", C.c_float * 3), ("bias", C.c_float * 3), ("antialias", C.c_int32),
-                ("dst", C.c_void_p), ("pitch_c", C.c_int64), ("pitch_y", C.c_int64)]
+                ("dst", C.c_void_p), ("pitch_c", C.c_int64), ("pitch_y", C.c_int64), ("flip", C.c_int32), ("pad", C.c_int32)]
 
 
 ABI_STRUCTS = [McFrame, McBlock, CompBlock, BlendBlock, WarpBlock, ItxBlock, LfFrame, CdefFrame, LrFrame, FrameJob,

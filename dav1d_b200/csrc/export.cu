@@ -183,9 +183,47 @@ B200_DEV typename TensorElem<DT>::type tensor_value(int v, float scale, float bi
     else return f;
 }
 
+// The stores of tensor_store: output pixel i of the run at x goes to x + i, or with MIRROR (B200TensorJob.flip) to
+// out_w - 1 - x - i. A mirrored run of 4 is the reversed run at out_w - 4 - x, stored like any other; a ragged one (n < 4,
+// the row's right end) lands at the row's left end one value at a time.
+template <bool MIRROR, bool HWC, class E>
+B200_DEV void store_pixels(const B200TensorJob &j, E *row, int x, int n, const E (&o)[3][4])
+{
+    if (MIRROR && n < 4) {
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+            if (i < n) {
+                const int64_t at = j.out_w - 1 - x - i;
+#pragma unroll
+                for (int c = 0; c < 3; c++) row[HWC ? 3 * at + c : c * j.pitch_c + at] = o[c][i];
+            }
+        return;
+    }
+    const int px = MIRROR ? j.out_w - 4 - x : x;
+    if constexpr (HWC) {
+        // the run is 12 contiguous values: R G B of pixel 0, then of pixel 1, ...
+        E v[3][4];
+#pragma unroll
+        for (int e = 0; e < 12; e++) v[e >> 2][e & 3] = o[e % 3][MIRROR ? 3 - e / 3 : e / 3];
+#pragma unroll
+        for (int r = 0; r < 3; r++) store_run(row + 3 * px + 4 * r, imin(4, 3 * n - 4 * r), v[r]);
+    } else {
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            if constexpr (MIRROR) {
+                const E v[4] = {o[c][3], o[c][2], o[c][1], o[c][0]};
+                store_run(row + c * j.pitch_c + px, n, v);
+            } else {
+                store_run(row + c * j.pitch_c + px, n, o[c]);
+            }
+        }
+    }
+}
+
 // The epilogue of both tensor kernels: Q of a run of n (<= 4) output pixels at (x, y), per plane, through the matrix, the
-// clip, scale / bias and rounding into the destination (yoff, coff, qmax as include/b200av1.h defines them for the job)
-template <int DT, bool HWC>
+// clip, scale / bias and rounding into the destination (yoff, coff, qmax as include/b200av1.h defines them for the job);
+// MIRROR = j.flip, a parameter of the kernels: jobs with and without a flip take kernels of their own
+template <int DT, bool HWC, bool MIRROR>
 B200_DEV void tensor_store(const B200TensorJob &j, int x, int y, int n, const int (&qy)[4], const int (&qu)[4], const int (&qv)[4],
                            int yoff, int coff, int qmax)
 {
@@ -206,17 +244,7 @@ B200_DEV void tensor_store(const B200TensorJob &j, int x, int y, int n, const in
         for (int c = 0; c < 3; c++) o[c][i] = tensor_value<DT>(rgb[c], j.scale[c], j.bias[c]);
     }
     E *const row = (E *)j.dst + y * j.pitch_y;
-    if constexpr (HWC) {
-        // the run is 12 contiguous values: R G B of pixel 0, then of pixel 1, ...
-        E v[3][4];
-#pragma unroll
-        for (int e = 0; e < 12; e++) v[e >> 2][e & 3] = o[e % 3][e / 3];
-#pragma unroll
-        for (int r = 0; r < 3; r++) store_run(row + 3 * x + 4 * r, imin(4, 3 * n - 4 * r), v[r]);
-    } else {
-#pragma unroll
-        for (int c = 0; c < 3; c++) store_run(row + c * j.pitch_c + x, n, o[c]);
-    }
+    store_pixels<MIRROR, HWC>(j, row, x, n, o);
 }
 
 // The jobs of one launch travel in the kernel's parameter block (no staging copy): B200_TENSOR_BATCH_MAX of them fit the
@@ -230,7 +258,7 @@ static_assert(sizeof(TensorBatch<B200_TENSOR_BATCH_MAX>) <= 4096, "the jobs of o
 // output of the launch, z selects the job. A thread converts its run of 4 columns on kTensorRows rows 8 apart, so the
 // column taps are worked out once for all of them
 constexpr int kTensorRows = 4;
-template <bool HBD, int DT, bool HWC, int N>
+template <bool HBD, int DT, bool HWC, int N, bool MIRROR>
 __global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constant__ TensorBatch<N> b)
 {
     B200_PDL_ENTRY();
@@ -257,7 +285,7 @@ __global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constan
             run_samples(qu, src + j.plane_off[1], j.stride[1], crow, ch, ct);
             run_samples(qv, src + j.plane_off[2], j.stride[2], crow, ch, ct);
         }
-        tensor_store<DT, HWC>(j, x, y, n, qy, qu, qv, yoff, coff, qmax);
+        tensor_store<DT, HWC, MIRROR>(j, x, y, n, qy, qu, qv, yoff, coff, qmax);
     }
 }
 
@@ -319,7 +347,7 @@ struct AaAxis {
 // memory, then each thread adds wy * H' into the vertical sums of its output pixels. Shared memory does not depend on the
 // reduction factor; source samples are read straight from global memory, each source row once per tile.
 constexpr int kAaCols = 32, kAaRowsMax = 32, kAaChunk = 32, kAaTaps = 64;
-template <bool HBD, int DT, bool HWC, int N>
+template <bool HBD, int DT, bool HWC, int N, bool MIRROR>
 __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_constant__ TensorBatch<N> b, int th)
 {
     B200_PDL_ENTRY();
@@ -414,7 +442,7 @@ __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_cons
             qy[i] = qs[0][t][c + i];
             if (!j.mono) { qu[i] = qs[1][t][c + i]; qv[i] = qs[2][t][c + i]; }
         }
-        tensor_store<DT, HWC>(j, x, y0 + t, imin(4, j.out_w - x), qy, qu, qv, yoff, coff, 4 * bdmax);
+        tensor_store<DT, HWC, MIRROR>(j, x, y0 + t, imin(4, j.out_w - x), qy, qu, qv, yoff, coff, 4 * bdmax);
     }
 }
 
@@ -456,9 +484,9 @@ static int check_tensor_job(const B200TensorJob &j, const char *who)
     if (!j.src || !in_range(j.w, 1, 65536) || !in_range(j.h, 1, 65536) || !in_range(j.out_w, 1, 65536) || !in_range(j.out_h, 1, 65536) ||
         !in_range(j.ss_hor, 0, 1) || !in_range(j.ss_ver, 0, 1) || !in_range(j.siting_x, 0, 1) || !in_range(j.siting_y, 0, 1) ||
         !in_range(j.dtype, B200_TENSOR_F32, B200_TENSOR_BF16) || !in_range(j.layout, B200_TENSOR_CHW, B200_TENSOR_HWC) ||
-        !in_range(j.antialias, 0, 1)) {
-        b200_set_error("%s: bad arguments (%d x %d -> %d x %d, dtype %d, layout %d, antialias %d)", who, j.w, j.h, j.out_w,
-                       j.out_h, j.dtype, j.layout, j.antialias);
+        !in_range(j.antialias, 0, 1) || !in_range(j.flip, 0, 1)) {
+        b200_set_error("%s: bad arguments (%d x %d -> %d x %d, dtype %d, layout %d, antialias %d, flip %d)", who, j.w, j.h,
+                       j.out_w, j.out_h, j.dtype, j.layout, j.antialias, j.flip);
         return -2;
     }
     if (j.identity && (j.mono || j.ss_hor || j.ss_ver)) { b200_set_error("%s: identity matrix needs 4:4:4", who); return -2; }
@@ -498,15 +526,18 @@ static int launch_tensor_aa_jobs(const TensorBatch<N> &b, int n, int out_w, int 
     const dim3 grid(xt, (out_h + th - 1) / th, n);
     return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, stream, [&](auto hbd) {
         constexpr bool H = decltype(hbd)::value;
-        void (*const k[3][2])(TensorBatch<N>, int) = {
-            {export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N>},
-            {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N>},
-            {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N>}};
-        return std::make_tuple(k[j.dtype][j.layout], b, th);
+        void (*const k[2][3][2])(TensorBatch<N>, int) = {
+            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, false>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, false>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, false>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, false>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, false>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, false>}},
+            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, true>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, true>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, true>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, true>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, true>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, true>}}};
+        return std::make_tuple(k[j.flip][j.dtype][j.layout], b, th);
     });
 }
 
-// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype, layout and kernel (aa)
+// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype, layout, kernel (aa) and flip
 template <int N>
 static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, bool aa, cudaStream_t stream)
 {
@@ -522,11 +553,14 @@ static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, bool aa, 
     const dim3 grid((runs + 31) / 32, (out_h + 8 * kTensorRows - 1) / (8 * kTensorRows), n);
     return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, stream, [&](auto hbd) {
         constexpr bool H = decltype(hbd)::value;
-        void (*const k[3][2])(TensorBatch<N>) = {
-            {export_tensor_kernel<H, B200_TENSOR_F32, false, N>, export_tensor_kernel<H, B200_TENSOR_F32, true, N>},
-            {export_tensor_kernel<H, B200_TENSOR_F16, false, N>, export_tensor_kernel<H, B200_TENSOR_F16, true, N>},
-            {export_tensor_kernel<H, B200_TENSOR_BF16, false, N>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N>}};
-        return std::make_tuple(k[j.dtype][j.layout], b);
+        void (*const k[2][3][2])(TensorBatch<N>) = {
+            {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, false>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, false>},
+             {export_tensor_kernel<H, B200_TENSOR_F16, false, N, false>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, false>},
+             {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, false>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, false>}},
+            {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, true>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, true>},
+             {export_tensor_kernel<H, B200_TENSOR_F16, false, N, true>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, true>},
+             {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, true>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, true>}}};
+        return std::make_tuple(k[j.flip][j.dtype][j.layout], b);
     });
 }
 static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, bool aa, cudaStream_t stream)
@@ -549,15 +583,15 @@ extern "C" int b200_export_tensor_batch(const B200TensorJob *jobs, int n, void *
             return -2;
         }
     }
-    // one launch per bit-depth class and kernel (bilinear, antialiased) present and per B200_TENSOR_BATCH_MAX jobs of it,
-    // jobs in their order
-    for (int group = 0; group < 4; group++) {
-        const int hbd = group & 1;
-        const bool aa = group >> 1;
+    // one launch per bit-depth class, kernel (bilinear, antialiased) and flip present and per B200_TENSOR_BATCH_MAX jobs of
+    // it, jobs in their order
+    for (int group = 0; group < 8; group++) {
+        const int hbd = group & 1, flip = group >> 2;
+        const bool aa = (group >> 1) & 1;
         const B200TensorJob *part[B200_TENSOR_BATCH_MAX];
         int m = 0;
         for (int i = 0; i < n; i++) {
-            if ((jobs[i].bitdepth_max > 255) != hbd || tensor_job_aa(jobs[i]) != aa) continue;
+            if ((jobs[i].bitdepth_max > 255) != hbd || tensor_job_aa(jobs[i]) != aa || jobs[i].flip != flip) continue;
             part[m++] = &jobs[i];
             if (m == B200_TENSOR_BATCH_MAX) {
                 if (int r = launch_tensor_jobs(part, m, aa, (cudaStream_t)stream)) return r;

@@ -278,6 +278,39 @@ def tensor_reference(planes, bpc, layout, size=None, matrix="bt709", full_range=
     return rgb.astype(np.float32) * scale[:, None, None] + bias[:, None, None]
 
 
+def crop_planes(planes, layout, box):
+    """the planes of the box (top, left, height, width) of a picture (layout = enum Dav1dPixelLayout), the source a cropped
+    tensor export reads (include/b200av1.h B200TensorJob): luma [top, top + height) x [left, left + width), chroma the
+    samples from top >> ssv, left >> ssh that cover it"""
+    top, left, height, width = box
+    ssh, ssv = int(layout in (1, 2)), int(layout == 1)
+    return [planes[0][top:top + height, left:left + width]] + \
+        [p[top >> ssv:(top + height + ssv) >> ssv, left >> ssh:(left + width + ssh) >> ssh] for p in planes[1:]]
+
+
+def align_crop(box, w, h, layout):
+    """the box (top, left, height, width) of a w x h picture that the tensor export takes for `box`: on a chroma-subsampled
+    axis (layout = enum Dav1dPixelLayout) an odd top / left is moved up / left by one sample and the height / width grown
+    by one, so that the bottom / right edge stays put and the box's chroma keeps the picture's siting. ValueError when box
+    is not 4 integers with height, width >= 1 inside the picture."""
+    if not _is_box(box):
+        raise ValueError("a crop box is 4 integers (top, left, height, width), not %r" % (box,))
+    top, left, height, width = (int(v) for v in box)
+    if top < 0 or left < 0 or height < 1 or width < 1 or top + height > h or left + width > w:
+        raise ValueError("crop box (top %d, left %d, height %d, width %d) is not inside the %dx%d picture" % (top, left, height, width, w, h))
+    ssh, ssv = int(layout in (1, 2)), int(layout == 1)
+    dt, dl = top & ssv, left & ssh
+    return top - dt, left - dl, height + dt, width + dl
+
+
+def _is_box(b):
+    return isinstance(b, (tuple, list, np.ndarray)) and len(b) == 4 and all(isinstance(v, (int, np.integer)) for v in b)
+
+
+def _is_flag(f):
+    return isinstance(f, (bool, np.bool_))
+
+
 class DeviceDecoder:
     """dav1d front end + B200 back end whose output pictures never leave the device: each one is exported by one kernel from
     its HBM copy into memory the caller allocates, and released at once.
@@ -308,8 +341,8 @@ class DeviceDecoder:
         d.refdrv_stream_close.argtypes = [C.c_void_p]
         d.b200hook_set_device_only.argtypes = [C.c_void_p, C.c_int]
         d.b200hook_export_picture.argtypes = [C.c_void_p, C.POINTER(ExportJob), C.c_void_p]
-        d.b200hook_export_tensor.argtypes = [C.c_void_p, C.POINTER(TensorJob), C.c_void_p]
-        d.b200hook_export_tensor_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        d.b200hook_export_tensor.argtypes = [C.c_void_p, C.POINTER(TensorJob), C.c_void_p, C.c_void_p]
+        d.b200hook_export_tensor_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         d.refdrv_stream_chroma_position.argtypes = [C.c_void_p]
 
     def stats(self, reset=False):
@@ -335,7 +368,7 @@ class DeviceDecoder:
         yield from self._decode(tus, lambda h, info: self._export(h, info, format, matrix, full_range, alloc, stream))
 
     def tensors(self, tus, size=None, dtype="float32", layout="chw", mean=None, std=None, matrix="auto", full_range=None,
-                chroma_siting="auto", batch=None, alloc=None, stream=None, antialias=False):
+                chroma_siting="auto", batch=None, alloc=None, stream=None, antialias=False, crop=None, flip=False):
         """Decodes the temporal units `tus` and yields every output picture as a model input: R, G, B resized to
         size = (height, width) (default: the picture's own) by bilinear sampling at half-sample centres, like
         torch.nn.functional.interpolate(mode="bilinear", align_corners=False) (chroma upsampling is part of the same
@@ -349,7 +382,13 @@ class DeviceDecoder:
         matrix and full_range: as in pictures(). chroma_siting: "auto" (the sequence header's chroma_sample_position:
         colocated -> "topleft", vertical or unknown -> "left", the MPEG-2 convention), "left", "topleft" or "center".
         alloc(shape, dtype) receives "float32", "float16" or "bfloat16"; alloc and stream otherwise mean what they mean in
-        pictures()."""
+        pictures().
+        crop: a box (top, left, height, width) in luma samples of the picture, or a callable (k, height, width) -> box for
+        output picture k of that size: the export reads the box alone as its picture, taps stopping at its edge
+        (torchvision's resized_crop; RandomResizedCrop with a random box). On a chroma-subsampled axis an odd top / left
+        is rounded down and the box grown to keep its bottom / right edge (align_crop). size=None exports the box at that
+        (aligned) size. flip: True, or a callable k -> bool, mirrors the output horizontally after resizing
+        (torchvision's hflip). ValueError, naming the picture, for a box outside the picture."""
         if dtype not in TENSOR_DTYPES or layout not in TENSOR_LAYOUTS:
             raise ValueError("dtype must be one of %s, layout 'chw' or 'hwc'" % ", ".join(TENSOR_DTYPES))
         if matrix != "auto" and matrix != "identity" and matrix not in MATRICES:
@@ -362,18 +401,28 @@ class DeviceDecoder:
                 raise ValueError("size must be (height, width), each 1 .. 65536")
         if batch is not None and int(batch) < 1:
             raise ValueError("batch must be >= 1")
+        if crop is not None and not callable(crop) and not _is_box(crop):
+            raise ValueError("crop must be None, a box (top, left, height, width) or a callable")
+        if not callable(flip) and not _is_flag(flip):
+            raise ValueError("flip must be a bool or a callable")
         tensor_scale_bias(8, mean, std)                          # checks mean / std
         alloc, stream = _default_alloc(alloc, stream)
         esize = 4 if dtype == "float32" else 2
-        state = {"buf": None, "n": 0, "shape": None}
+        state = {"buf": None, "n": 0, "shape": None, "k": 0}
 
         def export(h, info):
-            oh, ow = size or (int(info[1]), int(info[0]))
+            k = state["k"]
+            state["k"] += 1
+            box = _picture_box(crop(k, int(info[1]), int(info[0])) if callable(crop) else crop, info, "picture %d" % k)
+            fl = flip(k) if callable(flip) else flip
+            if not _is_flag(fl):
+                raise ValueError("picture %d: flip must be a bool, not %r" % (k, fl))
+            oh, ow = size or ((box[2], box[3]) if box else (int(info[1]), int(info[0])))
             shape = (3, oh, ow) if layout == "chw" else (oh, ow, 3)
             if batch is None:
                 out = alloc(shape, dtype)
                 self._export_tensor(h, info, _data_ptr(out), oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
-                                    antialias, stream)
+                                    antialias, stream, box, fl)
                 return [out]
             done = []
             if state["buf"] is not None and state["shape"] != shape:       # another size closes the batch
@@ -382,7 +431,8 @@ class DeviceDecoder:
             if state["buf"] is None:
                 state.update(buf=alloc((int(batch),) + shape, dtype), n=0, shape=shape)
             dst = _data_ptr(state["buf"]) + state["n"] * 3 * oh * ow * esize
-            self._export_tensor(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, antialias, stream)
+            self._export_tensor(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, antialias, stream,
+                                box, fl)
             state["n"] += 1
             if state["n"] == batch:
                 done.append(state["buf"])
@@ -395,12 +445,16 @@ class DeviceDecoder:
             yield state["buf"][:state["n"]]
 
     def clips(self, streams, frames, step=1, start=0, size=None, dtype="float32", layout="chw", mean=None, std=None,
-              matrix="auto", full_range=None, chroma_siting="auto", workers=None, alloc=None, stream=None, antialias=False):
+              matrix="auto", full_range=None, chroma_siting="auto", workers=None, alloc=None, stream=None, antialias=False,
+              crop=None, flip=False):
         """Decodes N streams (each a list of temporal units) concurrently and returns one clip per stream as a
         [N, frames, 3, OH, OW] tensor (layout="hwc": [N, frames, OH, OW, 3]): x[i, t] is output picture
         start_i + t * step of stream i, exported exactly as tensors() exports it. `start` is one int or one per stream.
         size=None needs every sampled picture to have the same size. The tensor options (antialias included), alloc and
         stream mean what they mean in tensors(); "auto" matrix, range and siting are resolved per stream from its own headers.
+        crop: one box (top, left, height, width) for every stream, one box per stream, or a callable (i, height, width) -> box
+        called once per stream i on its first sampled picture; flip: one bool, or one per stream. Every picture of a clip
+        takes its stream's box and flip (tensors() says what they do), so a clip stays consistent in time.
         Each stream has a dav1d context of its own (this decoder's n_threads / max_frame_delay) driven by a host thread of
         its own; at most `workers` streams are open at once (default min(N, CLIP_WORKERS), at most CLIP_MAX_WORKERS).
         Pictures that are not sampled are released unexported, and a stream is closed once its last sampled picture is
@@ -426,6 +480,18 @@ class DeviceDecoder:
             size = tuple(int(v) for v in size)
             if len(size) != 2 or not all(1 <= v <= 65536 for v in size):
                 raise ValueError("size must be (height, width), each 1 .. 65536")
+        if crop is None or callable(crop) or _is_box(crop):
+            crops = [crop] * n
+        elif isinstance(crop, (list, tuple)) and len(crop) == n and all(_is_box(b) for b in crop):
+            crops = list(crop)
+        else:
+            raise ValueError("crop must be None, a box (top, left, height, width), one box per stream or a callable")
+        if _is_flag(flip):
+            flips = [bool(flip)] * n
+        elif isinstance(flip, (list, tuple, np.ndarray)) and len(flip) == n and all(_is_flag(f) for f in flip):
+            flips = [bool(f) for f in flip]
+        else:
+            raise ValueError("flip must be a bool or one bool per stream")
         tensor_scale_bias(8, mean, std)                          # checks mean / std
         alloc, stream = _default_alloc(alloc, stream)
         self._hooked._bind()
@@ -454,8 +520,14 @@ class DeviceDecoder:
                         raise errors[0]
                     jobs = (TensorJob * len(items))()
                     pics = (C.c_void_p * len(items))()
+                    boxes = (C.c_int32 * (4 * len(items)))() if crop is not None else None
                     for k, (i, t, h, info, _) in enumerate(items):
-                        oh, ow = size or (int(info[1]), int(info[0]))
+                        if callable(crops[i]):                  # the stream's box, from its first sampled picture
+                            crops[i] = crops[i](i, int(info[1]), int(info[0]))
+                        box = _picture_box(crops[i], info, "stream %d picture %d" % (i, starts[i] + t * step))
+                        if box:
+                            boxes[4 * k:4 * k + 4] = box
+                        oh, ow = size or ((box[2], box[3]) if box else (int(info[1]), int(info[0])))
                         if out is None:
                             hw = (oh, ow)
                             out = alloc((n, frames) + ((3, oh, ow) if layout == "chw" else (oh, ow, 3)), dtype)
@@ -464,9 +536,9 @@ class DeviceDecoder:
                                              "pictures of different sizes" % (i, starts[i] + t * step, ow, oh, hw[1], hw[0]))
                         dst = _data_ptr(out) + (i * frames + t) * 3 * oh * ow * esize
                         jobs[k] = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
-                                                   antialias)
+                                                   antialias, flips[i])
                         pics[k] = self.dll.refdrv_stream_picture(h)
-                    if self.dll.b200hook_export_tensor_batch(pics, jobs, len(items), C.c_void_p(stream)) != 0:
+                    if self.dll.b200hook_export_tensor_batch(pics, jobs, boxes, len(items), C.c_void_p(stream)) != 0:
                         raise RuntimeError("exporting pictures failed (see stderr)")
                     left -= len(items)
                 finally:
@@ -567,12 +639,14 @@ class DeviceDecoder:
             name = "bt709"
         return name
 
-    def _export_tensor(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, stream):
-        job = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias)
-        if self.dll.b200hook_export_tensor(self.dll.refdrv_stream_picture(h), C.byref(job), C.c_void_p(stream)) != 0:
+    def _export_tensor(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, stream, box,
+                       flip):
+        job = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip)
+        box = (C.c_int32 * 4)(*box) if box else None
+        if self.dll.b200hook_export_tensor(self.dll.refdrv_stream_picture(h), C.byref(job), box, C.c_void_p(stream)) != 0:
             raise RuntimeError("exporting a picture failed (see stderr)")
 
-    def _tensor_job(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias=False):
+    def _tensor_job(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip):
         """the B200TensorJob of the picture stream h holds (info as _decode gives it): "auto" matrix, range and siting come
         from that stream's own headers"""
         w, hh, bpc, pl, mtrx, color_range = (int(v) for v in info)
@@ -590,6 +664,7 @@ class DeviceDecoder:
         for c in range(3):
             job.scale[c], job.bias[c] = float(scale[c]), float(bias[c])
         job.antialias = int(bool(antialias))
+        job.flip = int(flip)
         job.dst = dst
         job.pitch_y, job.pitch_c = (ow, oh * ow) if layout == "chw" else (3 * ow, 1)
         return job
@@ -635,6 +710,16 @@ def _default_alloc(alloc, stream):
         if stream is None:
             stream = torch.cuda.current_stream()
     return alloc, getattr(stream, "cuda_stream", stream) or 0
+
+
+def _picture_box(box, info, who):
+    """align_crop of box (None: no crop) on the picture of `info`; ValueError naming `who`"""
+    if box is None:
+        return None
+    try:
+        return align_crop(box, int(info[0]), int(info[1]), int(info[3]))
+    except ValueError as e:
+        raise ValueError("%s: %s" % (who, e)) from None
 
 
 def _data_ptr(a):

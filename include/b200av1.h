@@ -823,7 +823,17 @@ B200_API int b200_export_picture(const B200ExportJob *job, void *stream);
  *     scale = f32(1 / (4 * bdmax * std)), bias = f32(-mean / std); mean 0 and std 1 give outputs in [0, 1].
  * Destination (pitches in elements): CHW: dst + c * pitch_c + y * pitch_y + x, pitch_y >= out_w and
  * pitch_c >= (out_h - 1) * pitch_y + out_w (channels may not overlap); HWC: dst + y * pitch_y + 3 * x + c,
- * pitch_y >= 3 * out_w, pitch_c unused. dst aligned to the element size. One launch on `stream`; -2 on bad arguments. */
+ * pitch_y >= 3 * out_w, pitch_c unused. dst aligned to the element size.
+ *   flip = 1 mirrors the output horizontally after resizing: out'[c][y][x] = out[c][y][out_w - 1 - x] (torchvision's hflip
+ *     applied after resized_crop). It is not the export of a mirrored source: positions are floored to 1/256 sample and
+ *     chroma is sited left / top, neither of which is symmetric.
+ *   Crops are a change of source: the box (top, left, height, width) of the visible picture is the picture whose planes
+ *     start at the box (plane_off[0] += top * stride[0] + left, chroma plane_off[p] += (top >> ss_ver) * stride[p] +
+ *     (left >> ss_hor)) and whose visible size is w = width, h = height. Taps then stop at the box's edge, as in
+ *     torchvision's resized_crop, with the bilinear and the antialiased definition alike. The chroma of the box keeps the
+ *     picture's siting only when top is even where ss_ver and left is even where ss_hor: the hooks' boxes
+ *     (b200hook_export_tensor_batch, integration/dav1d/b200_hooks.c) are rejected otherwise.
+ * One launch on `stream`; -2 on bad arguments. */
 enum { B200_TENSOR_F32 = 0, B200_TENSOR_F16 = 1, B200_TENSOR_BF16 = 2 };
 enum { B200_TENSOR_CHW = 0, B200_TENSOR_HWC = 1 };
 typedef struct B200TensorJob {
@@ -840,13 +850,15 @@ typedef struct B200TensorJob {
     int32_t antialias;             /* 0: bilinear; 1: triangle filter on reduced axes (see above) */
     void *dst;                     /* device */
     int64_t pitch_c, pitch_y;      /* elements */
+    int32_t flip;                  /* 0, or 1: mirrored horizontally (see above) */
+    int32_t pad;
 } B200TensorJob;
 B200_API int b200_export_tensor(const B200TensorJob *job, void *stream);
 /* n >= 1 tensor jobs at once, e.g. the pictures of a clip batch taken from several streams: each job is exactly what
  * b200_export_tensor(&jobs[i]) writes, with its own source, geometry, bit depth, matrix, range, siting, scale / bias and
  * destination, but all jobs must share dtype and layout. The destinations must not overlap each other (jobs run in no
- * particular order). One launch on `stream` per bit-depth class present (8 bit, above 8 bit) and per
- * B200_TENSOR_BATCH_MAX jobs of it; the jobs ride in the kernel's parameter block. -2 when jobs is NULL, n < 1, dtype or
+ * particular order). One launch on `stream` per bit-depth class (8 bit, above 8 bit), kernel (bilinear,
+ * antialiased) and flip present, and per B200_TENSOR_BATCH_MAX jobs of it; the jobs ride in the kernel's parameter block. -2 when jobs is NULL, n < 1, dtype or
  * layout differ, or any job is bad (checked as b200_export_tensor checks it): then nothing is launched. b200_export_tensor
  * is the n = 1 case. */
 #define B200_TENSOR_BATCH_MAX 24

@@ -415,14 +415,17 @@ API int b200hook_export_picture(const Dav1dPicture *const p, const B200ExportJob
     if (!p || !tmpl || !p->data[0]) return -1;
     return p->p.bpc > 8 ? b200hook_export_picture_16bpc(p, tmpl, stream) : b200hook_export_picture_8bpc(p, tmpl, stream);
 }
-HookRefPic *b200hook_tensor_source_8bpc(const Dav1dPicture *p, B200TensorJob *j);
-HookRefPic *b200hook_tensor_source_16bpc(const Dav1dPicture *p, B200TensorJob *j);
+HookRefPic *b200hook_tensor_source_8bpc(const Dav1dPicture *p, const int32_t *box, B200TensorJob *j);
+HookRefPic *b200hook_tensor_source_16bpc(const Dav1dPicture *p, const int32_t *box, B200TensorJob *j);
 /* The same for the tensor export, for n pictures at once (one kernel launch per bit-depth class, include/b200av1.h
- * b200_export_tensor_batch): `tmpls[i]` carries picture i's output size, dtype, layout, siting, matrix, scale / bias and
- * destination; the source geometry is the picture's own. The stream waits once for each picture's job, and every picture's
- * export-done event is recorded behind the launch, so each entry keeps its device buffer until its export has completed. */
-API int b200hook_export_tensor_batch(const Dav1dPicture *const *const pics, const B200TensorJob *const tmpls, const int n,
-                                     void *const stream)
+ * b200_export_tensor_batch): `tmpls[i]` carries picture i's output size, dtype, layout, siting, matrix, scale / bias, flip
+ * and destination; the source is the picture, or with `boxes` (NULL: none) the box boxes[4i .. 4i + 3] = top, left,
+ * height, width of it (the upscaled picture with super-resolution). A box must lie inside the picture, and its top / left
+ * must be even on a chroma-subsampled axis (include/b200av1.h): else -1 and nothing is launched. The stream waits once for
+ * each picture's job, and every picture's export-done event is recorded behind the launch, so each entry keeps its device
+ * buffer until its export has completed. */
+API int b200hook_export_tensor_batch(const Dav1dPicture *const *const pics, const B200TensorJob *const tmpls,
+                                     const int32_t *const boxes, const int n, void *const stream)
 {
     if (!pics || !tmpls || n < 1) return -1;
     B200TensorJob *const jobs = malloc((size_t)n * sizeof(*jobs));
@@ -432,16 +435,18 @@ API int b200hook_export_tensor_batch(const Dav1dPicture *const *const pics, cons
         const Dav1dPicture *const p = pics[i];
         if (!p || !p->data[0]) { rc = -1; break; }
         jobs[i] = tmpls[i];
-        refs[i] = p->p.bpc > 8 ? b200hook_tensor_source_16bpc(p, &jobs[i]) : b200hook_tensor_source_8bpc(p, &jobs[i]);
+        const int32_t *const box = boxes ? boxes + 4 * i : NULL;
+        refs[i] = p->p.bpc > 8 ? b200hook_tensor_source_16bpc(p, box, &jobs[i]) : b200hook_tensor_source_8bpc(p, box, &jobs[i]);
         if (!refs[i]) rc = -1;
     }
     if (!rc) rc = b200hook_export_submit(refs, n, 1, jobs, stream);
     free(jobs); free(refs);
     return rc;
 }
-API int b200hook_export_tensor(const Dav1dPicture *const p, const B200TensorJob *const tmpl, void *const stream)
+API int b200hook_export_tensor(const Dav1dPicture *const p, const B200TensorJob *const tmpl, const int32_t *const box,
+                               void *const stream)
 {
-    return b200hook_export_tensor_batch(&p, tmpl, 1, stream);
+    return b200hook_export_tensor_batch(&p, tmpl, box, 1, stream);
 }
 void b200hook_refpic_set_ready(HookRefPic *r, int ready)
 {

@@ -1267,12 +1267,31 @@ int bitfn(b200hook_export_picture)(const Dav1dPicture *const p, const B200Export
     EXPORT_SOURCE(j, r, g, p);
     return b200hook_export_submit(&r, 1, 0, &j, stream);
 }
-/* fills the source fields of tensor job *j from the picture's device copy: that entry, NULL when it has none */
-HookRefPic *bitfn(b200hook_tensor_source)(const Dav1dPicture *const p, B200TensorJob *const j)
+/* fills the source fields of tensor job *j from the picture's device copy: that entry, NULL when it has none or when `box`
+ * (top, left, height, width, or NULL for the whole picture) is not a box of the picture whose chroma keeps its siting
+ * (include/b200av1.h B200TensorJob); the box's sub-picture is then the source */
+HookRefPic *bitfn(b200hook_tensor_source)(const Dav1dPicture *const p, const int32_t *const box, B200TensorJob *const j)
 {
+    if (box) {
+        const int mono = p->p.layout == DAV1D_PIXEL_LAYOUT_I400;
+        const int ssh = !mono && p->p.layout != DAV1D_PIXEL_LAYOUT_I444, ssv = p->p.layout == DAV1D_PIXEL_LAYOUT_I420;
+        const int64_t top = box[0], left = box[1], bh = box[2], bw = box[3];
+        if (top < 0 || left < 0 || bh < 1 || bw < 1 || top + bh > p->p.h || left + bw > p->p.w || (top & ssv) || (left & ssh)) {
+            fprintf(stderr, "b200hook: export: bad crop box (top %lld, left %lld, %lld x %lld) of a %d x %d picture\n",
+                    (long long)top, (long long)left, (long long)bw, (long long)bh, p->p.w, p->p.h);
+            return NULL;
+        }
+    }
     PicGeom g;
     HookRefPic *const r = bitfn(export_source)(p, &g);
-    if (r) EXPORT_SOURCE(*j, r, g, p);
+    if (!r) return NULL;
+    EXPORT_SOURCE(*j, r, g, p);
+    if (box) {
+        j->plane_off[0] += (uint32_t)((int64_t)box[0] * j->stride[0] + box[1]);
+        for (int k = 1; k < 3 && !j->mono; k++)
+            j->plane_off[k] += (uint32_t)((int64_t)(box[0] >> j->ss_ver) * j->stride[k] + (box[1] >> j->ss_hor));
+        j->h = box[2]; j->w = box[3];
+    }
     return r;
 }
 #undef EXPORT_SOURCE

@@ -1,6 +1,7 @@
 """The tensor export (b200_export_tensor) against the torch chain it replaces (run on a GPU machine):
 
-    python tools/bench_tensor_export.py [--launches 200] [--rounds 5] [--reps 3] [--antialias] [--kernel-only] [--out FILE]
+    python tools/bench_tensor_export.py [--launches 200] [--rounds 5] [--reps 3] [--antialias | --crop-flip] [--kernel-only]
+                                        [--baseline-lib SO] [--out FILE]
 
 Kernel level, one JSON line per configuration, on synthetic device pictures (random planes, 4:2:0):
   fused        one b200_export_tensor launch
@@ -18,6 +19,12 @@ Decoder level, one JSON line per stream workload of bench.py: pictures per secon
 --antialias: the kernel level only, on AA_CONFIGS, with B200TensorJob.antialias = 1 against the chain with
   interpolate(..., antialias=True); a config with a batch runs that many pictures as one b200_export_tensor_batch call
   (the chain then loops over them). --kernel-only skips the decoder level.
+--crop-flip: the kernel level only, on CROP_FLIP_CONFIGS: a RandomResizedCrop-style box (area 1/2, aspect 4:3) exported to
+  224 x 224 bf16 CHW, antialiased and flipped (B200TensorJob source moved to the box, flip = 1), against the chain a user
+  writes otherwise: the RGB export of the whole picture, the slice, interpolate(antialias=True), (x - mean) / std,
+  .flip(-1), .to(bfloat16).
+--baseline-lib SO: the kernel level times the same jobs (flip = 0) through another build of the library (an earlier
+  commit's libb200av1.so) instead of the torch chain, alternated with this tree's, as `fused_baseline`.
 The GPU's name, power limit and SM clock are read in the same run."""
 import argparse
 import ctypes as C
@@ -48,6 +55,9 @@ CONFIGS = [  # (name, source w, h, bpc, output (h, w) or None, dtype, layout)
     ("1080p8 -> 640x360 fp16 chw", 1920, 1080, 8, (360, 640), "float16", "chw"),
 ]
 
+# the batched launch (B200_TENSOR_BATCH_MAX jobs per launch) of the bilinear kernel, fields as in AA_CONFIGS
+BATCH_CONFIG = ("64 x 1080p8 -> 224x224 bf16 chw, one batch call", 1920, 1080, 8, (224, 224), "bfloat16", "chw", 64)
+
 
 AA_CONFIGS = [  # (name, source w, h, bpc, output (h, w), dtype, layout, pictures per call)
     ("aa 1080p8 -> 224x224 bf16 chw", 1920, 1080, 8, (224, 224), "bfloat16", "chw", 1),
@@ -58,19 +68,29 @@ AA_CONFIGS = [  # (name, source w, h, bpc, output (h, w), dtype, layout, picture
 ]
 
 
-def torch_chain(rgb, bdmax, size, dtype, layout, mean, std, antialias=False):
+CROP_FLIP_CONFIGS = [  # AA_CONFIGS' fields, then the box (top, left, height, width)
+    ("crop+flip 1080p8 -> 224x224 bf16 chw", 1920, 1080, 8, (224, 224), "bfloat16", "chw", 1, (100, 372, 882, 1176)),
+    ("crop+flip 4k10 -> 224x224 bf16 chw", 3840, 2160, 10, (224, 224), "bfloat16", "chw", 1, (200, 744, 1764, 2352)),
+]
+
+
+def torch_chain(rgb, bdmax, size, dtype, layout, mean, std, antialias=False, flip=False):
     x = rgb.float() / bdmax
     if size is not None:
         x = F.interpolate(x[None], size=size, mode="bilinear", align_corners=False, antialias=antialias)[0]
-    x = ((x - mean) / std).to(getattr(torch, dtype))
+    x = (x - mean) / std
+    x = (x.flip(-1) if flip else x).to(getattr(torch, dtype))
     return x.permute(1, 2, 0).contiguous() if layout == "hwc" else x
 
 
-def chain_bytes(w, h, sb, size, dtype, layout):
+def chain_bytes(w, h, sb, size, dtype, layout, box=None):
     """algorithmic bytes of the torch chain: each step reads its input and writes its output once"""
     px, (oh, ow) = w * h, size or (h, w)
     op = oh * ow
     b = w * h * 3 // 2 * sb + 3 * px * sb            # export: YUV in, RGB out
+    if box is not None:                              # the steps after the export see the box
+        px = box[2] * box[3]
+        b += 2 * 3 * op * 4                          # .flip(-1)
     b += 3 * px * sb + 3 * px * 4 + 2 * 3 * px * 4   # .float(), / bdmax
     if size is not None:
         b += 3 * px * 4 + 3 * op * 4                 # interpolate
@@ -81,12 +101,31 @@ def chain_bytes(w, h, sb, size, dtype, layout):
     return b
 
 
+def baseline_lib(path):
+    """the tensor export entry points of another build of the library, whose B200TensorJob may be of another size (so not
+    through _lib.B200Lib, which insists on this tree's layout)"""
+    dll = C.CDLL(os.path.abspath(path))
+    dll.b200_struct_size.restype = C.c_int
+    dll.b200_export_tensor.argtypes = [C.c_void_p, C.c_void_p]
+    dll.b200_export_tensor_batch.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    dll.b200_last_error.restype = C.c_char_p
+
+    def check(rc, what):
+        if rc != 0:
+            raise RuntimeError("%s failed (%d): %s" % (what, rc, dll.b200_last_error().decode()))
+    dll.check = check
+    return dll
+
+
 def kernel_level(args):
     lib = _lib.get_lib()
     s = torch.cuda.Stream()
     lines = []
-    configs = AA_CONFIGS if args.antialias else [c + (1,) for c in CONFIGS]
-    for name, w, h, bpc, size, dtype, layout, pics in configs:
+    configs = CROP_FLIP_CONFIGS if args.crop_flip else AA_CONFIGS if args.antialias else [c + (1,) for c in CONFIGS] + [BATCH_CONFIG]
+    base = baseline_lib(args.baseline_lib) if args.baseline_lib else None
+    for name, w, h, bpc, size, dtype, layout, pics, *box in configs:
+        box = box[0] if box else None
+        antialias = args.antialias or box is not None
         rng = np.random.default_rng(w + bpc)
         bdmax, sb = (1 << bpc) - 1, 1 if bpc == 8 else 2
         planes = [rng.integers(0, bdmax + 1, (ph, pw)).astype(np.uint8 if bpc == 8 else np.int16) for pw, ph in stream.plane_dims(w, h, 1)]
@@ -107,7 +146,13 @@ def kernel_level(args):
         for c in range(3):
             tj.scale[c], tj.bias[c] = float(scale[c]), float(bias[c])
         tj.dst, tj.pitch_c, tj.pitch_y = out.data_ptr(), (oh * ow if layout == "chw" else 1), (ow if layout == "chw" else 3 * ow)
-        tj.antialias = int(args.antialias)
+        tj.antialias = int(antialias)
+        if box is not None:                      # the box is the source; the output is mirrored
+            top, left, tj.h, tj.w = box
+            tj.plane_off[0] += top * tj.stride[0] + left
+            for k in (1, 2):
+                tj.plane_off[k] += (top >> 1) * tj.stride[k] + (left >> 1)
+            tj.flip = 1
         if pics > 1:                             # the same picture into pics slots, one call
             out = torch.empty((pics,) + shape, dtype=getattr(torch, dtype), device="cuda")
             tjs = (stream.TensorJob * pics)()
@@ -135,15 +180,31 @@ def kernel_level(args):
         def chain():
             for _ in range(pics):
                 lib.check(lib.b200_export_picture(C.byref(ej), sp), "b200_export_picture")
-                torch_chain(rgb, bdmax, size, dtype, layout, mean, std, args.antialias)
+                x = rgb if box is None else rgb[:, box[0]:box[0] + box[2], box[1]:box[1] + box[3]]
+                torch_chain(x, bdmax, size, dtype, layout, mean, std, antialias, box is not None)
 
-        times = {"fused": [], "torch_chain": []}
+        arms = {"fused": fused}
+        if base is not None:                     # the same jobs in the other build's struct layout
+            bsz = base.b200_struct_size(23)
+            packed = (C.c_char * (bsz * pics))()
+            for k in range(pics):
+                C.memmove(C.addressof(packed) + k * bsz, C.addressof(tjs[k] if pics > 1 else tj), bsz)
+
+            def fused_baseline():
+                if pics > 1:
+                    base.check(base.b200_export_tensor_batch(packed, pics, sp), "b200_export_tensor_batch")
+                else:
+                    base.check(base.b200_export_tensor(packed, sp), "b200_export_tensor")
+            arms["fused_baseline"] = fused_baseline
+        else:
+            arms["torch_chain"] = chain
+        times = {k: [] for k in arms}
         with torch.cuda.stream(s):
-            for f in (fused, chain):
+            for f in arms.values():
                 for _ in range(20):
                     f()
             for _ in range(args.rounds):
-                for key, f in (("fused", fused), ("torch_chain", chain)):
+                for key, f in arms.items():
                     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                     torch.cuda._sleep(50_000_000)            # holds the stream while the launches are enqueued
                     a.record(s)
@@ -152,17 +213,25 @@ def kernel_level(args):
                     b.record(s)
                     b.synchronize()
                     times[key].append(1e3 * a.elapsed_time(b) / args.launches)
-        fused_bytes = pics * (w * h * 3 // 2 * sb + 3 * oh * ow * ESIZE[dtype])
+        sw, sh = (box[3], box[2]) if box else (w, h)
+        fused_bytes = pics * (sw * sh * 3 // 2 * sb + 3 * oh * ow * ESIZE[dtype])
         line = {"config": name, "gpu": gpu_info(), "launches_per_round": args.launches, "rounds": args.rounds, "us": {}, "bytes": {
-            "fused": fused_bytes, "torch_chain": pics * chain_bytes(w, h, sb, size, dtype, layout)}, "GBps": {}, "share_of_3.35TBps": {}}
-        if args.antialias:
+            "fused": fused_bytes, "fused_baseline": fused_bytes, "torch_chain": pics * chain_bytes(w, h, sb, size, dtype, layout, box)},
+            "GBps": {}, "share_of_3.35TBps": {}}
+        line["bytes"] = {k: v for k, v in line["bytes"].items() if k in times}
+        if antialias:
             line["antialias"] = True
+        if box is not None:
+            line["crop_box"], line["flip"] = list(box), True
+        if base is not None:
+            line["baseline_lib"] = args.baseline_lib
         for key, v in times.items():
             med = float(np.median(v))
             line["us"][key] = {"median": round(med, 2), "min": round(min(v), 2)}
             line["GBps"][key] = round(line["bytes"][key] / (med * 1e-6) / 1e9, 1)
             line["share_of_3.35TBps"][key] = round(line["bytes"][key] / (med * 1e-6) / HBM_BYTES_PER_S, 3)
-        line["speedup_median"] = round(line["us"]["torch_chain"]["median"] / line["us"]["fused"]["median"], 2)
+        other = "fused_baseline" if base is not None else "torch_chain"
+        line["speedup_median"] = round(line["us"][other]["median"] / line["us"]["fused"]["median"], 3)
         print(json.dumps(line), flush=True)
         lines.append(line)
     return lines
@@ -226,11 +295,13 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--antialias", action="store_true")
+    ap.add_argument("--crop-flip", action="store_true")
+    ap.add_argument("--baseline-lib", help="another build of libb200av1.so: time its export of the same jobs instead of the chain")
     ap.add_argument("--kernel-only", action="store_true")
     ap.add_argument("--out")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
-    lines = kernel_level(args) + ([] if args.antialias or args.kernel_only else decoder_level(args))
+    lines = kernel_level(args) + ([] if args.antialias or args.crop_flip or args.kernel_only else decoder_level(args))
     if args.out:
         with open(args.out, "w") as fh:
             for line in lines:
