@@ -4,9 +4,9 @@
 // memory as vertical pixel pairs with a sentinel for samples outside the picture (see the frame kernel).
 // Eight lanes per 8x8 block find its direction / variance from the (pre-CDEF) luma samples and derive the
 // strengths exactly like dav1d_cdef_brow; the filter then reads every tap from the tile. Unfiltered blocks
-// are copied through. The Level-1 direction search runs the same cdef_dir8; the Level-1 block filter
-// (cdef_fb_kernel) is still a scalar restatement that skips the taps outside the block's available
-// rectangle, which is what the reference's INT16_MIN padding achieves.
+// are copied through. The Level-1 slots run the same code: cdef.dir the same cdef_dir8, cdef.fb the same
+// cdef_filter4 / cdef_store2 on a tile holding one block, the sentinel in every sample the edges flags mark
+// unavailable (the reference's INT16_MIN padding).
 #include "host_util.h"
 
 namespace b200 {
@@ -18,56 +18,6 @@ __constant__ int8_t c_cdef_off[8][2][2] = {
 };
 __constant__ uint16_t c_cdef_div[7] = { 840, 420, 280, 210, 168, 140, 120 };
 __constant__ uint8_t c_uv_dir422[8] = { 7, 0, 2, 4, 5, 6, 6, 6 };
-
-B200_DEV int cdef_constrain(int diff, int threshold, int shift) {
-    const int adiff = iabs(diff);
-    const int v = imin(adiff, imax(0, threshold - (adiff >> shift)));
-    return diff < 0 ? -v : v;
-}
-
-struct CdefRect { int xmin, xmax, ymin, ymax; };   // available samples: [xmin, xmax) x [ymin, ymax)
-
-template <bool HBD>
-B200_DEV int cdef_pixel(const typename Bd<HBD>::pixel *__restrict__ plane, int stride, int ax, int ay,
-                        const CdefRect &r, int pri, int sec, int dir, int pri_shift, int sec_shift, int pri_tap0)
-{
-    const int px = plane[(ptrdiff_t)ay * stride + ax];
-    int sum = 0, mx = px, mn = px;
-#pragma unroll
-    for (int k = 0; k < 2; k++) {
-        if (pri) {
-            const int tap = k ? ((pri_tap0 & 3) | 2) : pri_tap0;
-            const int dy = c_cdef_off[dir][k][0], dx = c_cdef_off[dir][k][1];
-#pragma unroll
-            for (int s = -1; s <= 1; s += 2) {
-                const int x = ax + s * dx, y = ay + s * dy;
-                if (x < r.xmin || x >= r.xmax || y < r.ymin || y >= r.ymax) continue;
-                const int p = plane[(ptrdiff_t)y * stride + x];
-                sum += tap * cdef_constrain(p - px, pri, pri_shift);
-                mn = imin(mn, p); mx = imax(mx, p);
-            }
-        }
-        if (sec) {
-            const int tap = 2 - k;
-#pragma unroll
-            for (int j = 0; j < 2; j++) {
-                const int d2 = (dir + (j ? 6 : 2)) & 7;
-                const int dy = c_cdef_off[d2][k][0], dx = c_cdef_off[d2][k][1];
-#pragma unroll
-                for (int s = -1; s <= 1; s += 2) {
-                    const int x = ax + s * dx, y = ay + s * dy;
-                    if (x < r.xmin || x >= r.xmax || y < r.ymin || y >= r.ymax) continue;
-                    const int p = plane[(ptrdiff_t)y * stride + x];
-                    sum += tap * cdef_constrain(p - px, sec, sec_shift);
-                    mn = imin(mn, p); mx = imax(mx, p);
-                }
-            }
-        }
-    }
-    int v = px + ((sum - (sum < 0) + 8) >> 4);
-    if (pri && sec) v = iclip(v, mn, mx);
-    return v;
-}
 
 // Direction search (cdef_find_dir_c) of one 8x8 block by an aligned group of 8 lanes of one warp; lane y supplies row y
 // as v[x] = (px >> (bitdepth - 8)) - 128. bins is the block's zeroed 8 x 16 int scratch in shared memory: bins[d * 16 + n]
@@ -145,8 +95,9 @@ B200_DEV int cdef_adjust_strength(int strength, unsigned var) {
 //
 // constrain(diff) = sign(diff) * min(|diff|, max(0, thr - (|diff| >> shift))) is accumulated as
 //   P = relu(min(diff, t)), N = relu(min(-diff, t)), t = thr - (|diff| >> shift)   (sum = sum(P) - sum(N)),
-// which needs no sign restore. The sentinel (-16384) keeps diff inside int16 and makes t <= 0 for every
-// legal damping, so out-of-picture taps contribute nothing and are ignored by the signed max / unsigned min.
+// which needs no sign restore. The sentinel (-16384) keeps diff inside int16 and makes t <= 0 for the strengths
+// and damping dav1d derives (damping 2 + b8 .. 6 + b8, pri <= 15 << b8, sec in {0, 1, 2, 4} << b8), so
+// out-of-picture taps contribute nothing and are ignored by the signed max / unsigned min.
 constexpr int kCdefTW = 64, kCdefTH = 32, kCdefPitch = kCdefTW + 8, kCdefRows = kCdefTH + 3;
 constexpr int kCdefThreads = 256;
 constexpr unsigned kCdefSentinel = 0xC000u;
@@ -184,6 +135,57 @@ B200_DEV void cdef_tap2(const uint32_t *t, int idx, int off, unsigned negpx, uns
 // 8-bit: the low bytes of four packed pairs' halves as one row word (sel 0x0040 / 0x0062 picks the low / high halves)
 B200_DEV unsigned cdef_row8(const unsigned (&o)[4], unsigned sel) {
     return __byte_perm(__byte_perm(o[0], o[1], sel), __byte_perm(o[2], o[3], sel), 0x5410);
+}
+
+// The filter of one item: o[] are the 4 packed pairs at word idx of a staged tile t (pitch kCdefPitch, off[d][k] the word
+// offset of tap k of direction d), filtered in place with the block's strengths (pri | sec != 0), direction and
+// constrain shifts.
+B200_DEV void cdef_filter4(const uint32_t *t, int idx, const int16_t (&off)[8][2], int pri, int sec, int dir,
+                           int pshift, int sshift, int b8, unsigned (&o)[4])
+{
+    const unsigned pthr1 = (unsigned)(pri + 1) * 0x00010001u, psmask = (0xffffu >> pshift) * 0x00010001u;
+    const unsigned sthr1 = (unsigned)(sec + 1) * 0x00010001u, ssmask = (0xffffu >> sshift) * 0x00010001u;
+    const int tap0 = 4 - ((pri >> b8) & 1);
+    const int d2 = (dir + 2) & 7, d6 = (dir + 6) & 7;
+    const int op0 = off[dir][0], op1 = off[dir][1];
+    const int os20 = off[d2][0], os60 = off[d6][0], os21 = off[d2][1], os61 = off[d6][1];
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+        const unsigned px2 = o[c];
+        const unsigned negpx = __vadd2(~px2, 0x00010001u);
+        unsigned mn = px2, mx = px2, sumN = 0, sumP = 0;
+        if (pri) {
+            cdef_tap2(t, idx + c, op0, negpx, pthr1, pshift, psmask, tap0, sumP, sumN, mx, mn);
+            cdef_tap2(t, idx + c, op1, negpx, pthr1, pshift, psmask, (tap0 & 3) | 2, sumP, sumN, mx, mn);
+        }
+        if (sec) {
+            cdef_tap2(t, idx + c, os20, negpx, sthr1, sshift, ssmask, 2, sumP, sumN, mx, mn);
+            cdef_tap2(t, idx + c, os60, negpx, sthr1, sshift, ssmask, 2, sumP, sumN, mx, mn);
+            cdef_tap2(t, idx + c, os21, negpx, sthr1, sshift, ssmask, 1, sumP, sumN, mx, mn);
+            cdef_tap2(t, idx + c, os61, negpx, sthr1, sshift, ssmask, 1, sumP, sumN, mx, mn);
+        }
+        const int s0 = (int)(sumP & 0xffff) - (int)(sumN & 0xffff), s1 = (int)(sumP >> 16) - (int)(sumN >> 16);
+        int o0 = (int)(px2 & 0xffff) + ((s0 - (s0 < 0) + 8) >> 4);
+        int o1 = (int)(px2 >> 16) + ((s1 - (s1 < 0) + 8) >> 4);
+        if (pri && sec) {
+            o0 = iclip(o0, (int)(mn & 0xffff), (int)(mx & 0xffff));
+            o1 = iclip(o1, (int)(mn >> 16), (int)(mx >> 16));
+        }
+        o[c] = (unsigned)o0 | (unsigned)o1 << 16;
+    }
+}
+
+// an item's two rows of 4 pixels: row y at op, row y + 1 at op + st
+template <bool HBD>
+B200_DEV void cdef_store2(typename Bd<HBD>::pixel *op, int st, const unsigned (&o)[4])
+{
+    if (HBD) {
+        *(uint2 *)op = make_uint2(__byte_perm(o[0], o[1], 0x5410), __byte_perm(o[2], o[3], 0x5410));
+        *(uint2 *)(op + st) = make_uint2(__byte_perm(o[0], o[1], 0x7632), __byte_perm(o[2], o[3], 0x7632));
+    } else {
+        *(unsigned *)op = cdef_row8(o, 0x0040);
+        *(unsigned *)(op + st) = cdef_row8(o, 0x0062);
+    }
 }
 
 template <bool HBD>
@@ -328,67 +330,42 @@ __global__ void __launch_bounds__(kCdefThreads, B200_CDEF_MINB) cdef_frame_kerne
         const uint4 pw = *(const uint4 *)&t[idx];
         unsigned o[4] = { pw.x, pw.y, pw.z, pw.w };              // (row y | row y + 1 << 16) per column
         const int pri = pl ? bi.uv_pri : bi.y_pri, sec = pl ? bi.uv_sec : bi.y_sec, dir = pl ? bi.uv_dir : bi.y_dir;
-        if (pri | sec) {
-            const int pshift = pl ? bi.uv_pri_shift : bi.y_pri_shift, sshift = pl ? bi.uv_sec_shift : bi.y_sec_shift;
-            const unsigned pthr1 = (unsigned)(pri + 1) * 0x00010001u, psmask = (0xffffu >> pshift) * 0x00010001u;
-            const unsigned sthr1 = (unsigned)(sec + 1) * 0x00010001u, ssmask = (0xffffu >> sshift) * 0x00010001u;
-            const int tap0 = 4 - ((pri >> b8) & 1);
-            const int d2 = (dir + 2) & 7, d6 = (dir + 6) & 7;
-            const int op0 = S.off[dir][0], op1 = S.off[dir][1];
-            const int os20 = S.off[d2][0], os60 = S.off[d6][0], os21 = S.off[d2][1], os61 = S.off[d6][1];
-#pragma unroll
-            for (int c = 0; c < 4; c++) {
-                const unsigned px2 = o[c];
-                const unsigned negpx = __vadd2(~px2, 0x00010001u);
-                unsigned sumP = 0, sumN = 0, mx = px2, mn = px2;
-                if (pri) {
-                    cdef_tap2(t, idx + c, op0, negpx, pthr1, pshift, psmask, tap0, sumP, sumN, mx, mn);
-                    cdef_tap2(t, idx + c, op1, negpx, pthr1, pshift, psmask, (tap0 & 3) | 2, sumP, sumN, mx, mn);
-                }
-                if (sec) {
-                    cdef_tap2(t, idx + c, os20, negpx, sthr1, sshift, ssmask, 2, sumP, sumN, mx, mn);
-                    cdef_tap2(t, idx + c, os60, negpx, sthr1, sshift, ssmask, 2, sumP, sumN, mx, mn);
-                    cdef_tap2(t, idx + c, os21, negpx, sthr1, sshift, ssmask, 1, sumP, sumN, mx, mn);
-                    cdef_tap2(t, idx + c, os61, negpx, sthr1, sshift, ssmask, 1, sumP, sumN, mx, mn);
-                }
-                const int s0 = (int)(sumP & 0xffff) - (int)(sumN & 0xffff), s1 = (int)(sumP >> 16) - (int)(sumN >> 16);
-                int o0 = (int)(px2 & 0xffff) + ((s0 - (s0 < 0) + 8) >> 4);
-                int o1 = (int)(px2 >> 16) + ((s1 - (s1 < 0) + 8) >> 4);
-                if (pri && sec) {
-                    o0 = iclip(o0, (int)(mn & 0xffff), (int)(mx & 0xffff));
-                    o1 = iclip(o1, (int)(mn >> 16), (int)(mx >> 16));
-                }
-                o[c] = (unsigned)o0 | (unsigned)o1 << 16;
-            }
-        }
+        if (pri | sec)
+            cdef_filter4(t, idx, S.off, pri, sec, dir, pl ? bi.uv_pri_shift : bi.y_pri_shift,
+                         pl ? bi.uv_sec_shift : bi.y_sec_shift, b8, o);
         const int st = f.stride[pl];
-        pixel *op = dst + f.plane_off[pl] + (ptrdiff_t)((by0 * 4 >> sv) + y) * st + (bx0 * 4 >> sh) + x;
-        if (HBD) {
-            *(uint2 *)op = make_uint2(__byte_perm(o[0], o[1], 0x5410), __byte_perm(o[2], o[3], 0x5410));
-            *(uint2 *)(op + st) = make_uint2(__byte_perm(o[0], o[1], 0x7632), __byte_perm(o[2], o[3], 0x7632));
-        } else {
-            *(unsigned *)op = cdef_row8(o, 0x0040);
-            *(unsigned *)(op + st) = cdef_row8(o, 0x0062);
-        }
+        cdef_store2<HBD>(dst + f.plane_off[pl] + (ptrdiff_t)((by0 * 4 >> sv) + y) * st + (bx0 * 4 >> sh) + x, st, o);
     }
 }
 
 // Level-1 kernels ---------------------------------------------------------------------------
+// One w x h block (cdef.fb) on the frame kernel's filter: win is the block's dense (w+4) x (h+4) window with the block at
+// (2, 2) and kCdefSentinel in every sample the edges flags mark unavailable. Its rows are staged as pair words at the
+// frame tile's pitch with the block at the tile's origin, so the same tap offsets apply; out is the dense w x h result.
 template <bool HBD>
-__global__ void cdef_fb_kernel(const typename Bd<HBD>::pixel *win, typename Bd<HBD>::pixel *out, int w, int h,
-                               int pri, int sec, int dir, int damping, int edges, int bdmax)
+__global__ void cdef_block_kernel(const uint16_t *win, typename Bd<HBD>::pixel *out, int w, int h, int pri, int sec,
+                                  int dir, int damping, int bdmax)
 {
-    // win: dense (w+4) x (h+4) window, block at (2,2)
+    __shared__ uint32_t tile[(8 + 3) * kCdefPitch];
+    __shared__ int16_t off[8][2];
     const int b8 = HBD ? (32 - __clz(bdmax)) - 8 : 0;
-    CdefRect r;
-    r.xmin = (edges & B200_CDEF_HAVE_LEFT) ? 0 : 2; r.xmax = w + 2 + ((edges & B200_CDEF_HAVE_RIGHT) ? 2 : 0);
-    r.ymin = (edges & B200_CDEF_HAVE_TOP) ? 0 : 2;  r.ymax = h + 2 + ((edges & B200_CDEF_HAVE_BOTTOM) ? 2 : 0);
-    const int pri_tap0 = 4 - ((pri >> b8) & 1);
-    const int pri_shift = pri ? imax(0, damping - ulog2(pri)) : 0;
-    const int sec_shift = sec ? damping - ulog2(sec) : 0;
-    for (int i = threadIdx.x; i < w * h; i += blockDim.x)
-        out[i] = (typename Bd<HBD>::pixel)cdef_pixel<HBD>(win, w + 4, 2 + (i % w), 2 + (i / w), r, pri, sec, dir,
-                                                          pri_shift, sec_shift, pri_tap0);
+    const int ww = w + 4;
+    for (int i = threadIdx.x; i < (h + 3) * ww; i += blockDim.x) {
+        const int r = i / ww, c = i - r * ww;
+        tile[r * kCdefPitch + 2 + c] = win[r * ww + c] | (unsigned)win[(r + 1) * ww + c] << 16;
+    }
+    if (threadIdx.x < 16) {
+        const int d = threadIdx.x >> 1, k = threadIdx.x & 1;
+        off[d][k] = (int16_t)(c_cdef_off[d][k][0] * kCdefPitch + c_cdef_off[d][k][1]);
+    }
+    __syncthreads();
+    const int i = threadIdx.x, gw = w >> 2;
+    if (i >= gw * (h >> 1)) return;
+    const int y = i / gw * 2, x = i % gw * 4, idx = (y + 2) * kCdefPitch + x + 4;
+    unsigned o[4] = { tile[idx], tile[idx + 1], tile[idx + 2], tile[idx + 3] };
+    cdef_filter4(tile, idx, off, pri, sec, dir, pri ? imax(0, damping - ulog2(pri)) : 0, sec ? damping - ulog2(sec) : 0,
+                 b8, o);
+    cdef_store2<HBD>(out + y * w + x, w, o);
 }
 
 template <bool HBD>
@@ -456,13 +433,21 @@ int b200_cdef_fb(void *dst, ptrdiff_t stride, const void *left, const void *top,
                  int sec, int dir, int damping, int w, int h, int edges, int bdmax)
 {
     if (int r = check_bdmax(bdmax, "b200_cdef_fb")) return r;
-    if (!((w == 4 || w == 8) && (h == 4 || h == 8)) || dir < 0 || dir > 7 || (!pri && !sec)) { b200_set_error("b200_cdef_fb: bad arguments"); return -2; }
+    // the strengths and damping for which the sentinel silences the unavailable taps (kCdefSentinel): what dav1d
+    // passes, luma damping 3 + b8 .. 6 + b8 and chroma one less
+    const int b8 = ulog2(bdmax) - 7;
+    const bool sec_ok = sec == 0 || sec == 1 << b8 || sec == 2 << b8 || sec == 4 << b8;
+    if (!((w == 4 || w == 8) && (h == 4 || h == 8)) || dir < 0 || dir > 7 || (!pri && !sec) || pri < 0 || pri > 15 << b8 ||
+        !sec_ok || damping < 2 + b8 || damping > 6 + b8) {
+        b200_set_error("b200_cdef_fb: bad arguments (w=%d h=%d pri=%d sec=%d dir=%d damping=%d)", w, h, pri, sec, dir, damping);
+        return -2;
+    }
     Level1 L;
     const size_t px = bdmax > 255 ? 2 : 1;
     const int ww = w + 4;
-    uint8_t win[12 * 12 * 2];
-    memset(win, 0, sizeof(win));
-    auto put = [&](int wx, int wy, const void *p) { memcpy(win + ((size_t)wy * ww + wx) * px, p, px); };
+    uint16_t win[12 * 12];
+    for (uint16_t &v : win) v = kCdefSentinel;
+    auto put = [&](int wx, int wy, const void *p) { win[wy * ww + wx] = px == 2 ? *(const uint16_t *)p : *(const uint8_t *)p; };
     const int xs = (edges & B200_CDEF_HAVE_LEFT) ? -2 : 0, xe = w + ((edges & B200_CDEF_HAVE_RIGHT) ? 2 : 0);
     for (int y = 0; y < h; y++) {
         for (int x = 0; x < xe; x++) put(2 + x, 2 + y, (const uint8_t *)dst + (ptrdiff_t)y * stride + (ptrdiff_t)x * (ptrdiff_t)px);
@@ -475,10 +460,10 @@ int b200_cdef_fb(void *dst, ptrdiff_t stride, const void *left, const void *top,
         for (int y = 0; y < 2; y++) for (int x = xs; x < xe; x++)
             put(2 + x, 2 + h + y, (const uint8_t *)bottom + (ptrdiff_t)y * stride + (ptrdiff_t)x * (ptrdiff_t)px);
     void *in, *out;
-    if (!(in = L.upload(0, win, (size_t)ww * (h + 4) * px)) || !(out = L.dev(1, 64 * 2))) return -1;
+    if (!(in = L.upload(0, win, (size_t)ww * (h + 4) * sizeof(win[0]))) || !(out = L.dev(1, 64 * 2))) return -1;
     if (int r = launch_hbd(bdmax, Launch::plain, dim3(1), dim3(64), 0, 0, [&](auto hbd) {
-            typedef typename Bd<hbd>::pixel pixel;
-            return std::make_tuple(cdef_fb_kernel<hbd>, (const pixel *)in, (pixel *)out, w, h, pri, sec, dir, damping, edges, bdmax);
+            return std::make_tuple(cdef_block_kernel<hbd>, (const uint16_t *)in, (typename Bd<hbd>::pixel *)out, w, h, pri,
+                                   sec, dir, damping, bdmax);
         }))
         return r;
     return L.download_rect(1, dst, stride, w, h, px);

@@ -326,7 +326,9 @@ typedef struct B200CdefFrame {
 } B200CdefFrame;
 B200_API int b200_cdef_frame(int bitdepth_max, const B200CdefFrame *frame, void *stream);
 
-/* Level 1 (host pointers): cdef.dir and cdef.fb[0..2] = 8x8 / 4x8 / 4x4 */
+/* Level 1 (host pointers): cdef.dir and cdef.fb[0..2] = 8x8 / 4x8 / 4x4. b200_cdef_fb takes what dav1d passes
+ * (b8 = bitdepth - 8): damping 2 + b8 .. 6 + b8, pri_strength 0 .. 15 << b8, sec_strength 0, 1, 2 or 4 << b8, not
+ * both zero; anything else is -2. */
 B200_API int b200_cdef_dir(const void *img, ptrdiff_t stride, unsigned *var, int bitdepth_max);
 B200_API int b200_cdef_fb(void *dst, ptrdiff_t stride, const void *left, const void *top, const void *bottom,
                           int pri_strength, int sec_strength, int dir, int damping, int w, int h, int edges,

@@ -1,7 +1,8 @@
 """Level-1 post-filter slots on the inputs the checkasm-style tests leave to chance.
 
 - CDEF fb: 8, 10 and 12 bit, every block size, edge combination and direction, pri-only / sec-only / both at the
-  largest strengths, the smallest and largest damping, and saturated pixels beside missing edges.
+  largest strengths, the smallest and largest damping, and saturated pixels beside missing edges; strengths and
+  damping outside what dav1d passes are bad arguments.
 - fgy / fguv (the frame kernel's apply arithmetic): every layout, row_num 0 and > 0, overlap on and off, odd widths, and
   the restricted-range clip with and without is_id.
 - resize (the frame job's super-resolution kernel over one plane): widths that are not multiples of 4, with mx0 and dx
@@ -49,6 +50,19 @@ def check_cdef(new, chk, bpc, seed):
                         assert np.array_equal(a, b), ("cdef fb", bpc, w, h, edges, d, pri, sec, damp)
                         n += 1
     return n
+
+
+def check_cdef_rejects(lib, bpc):
+    """b200_cdef_fb outside dav1d's damping 2 + b8 .. 6 + b8, pri <= 15 << b8, sec in {0, 1, 2, 4} << b8: -2, dst untouched"""
+    b8, dt = bpc - 8, refs.pixel_dtype(bpc)
+    left, edge = np.zeros(16, dt), np.zeros(16 * 2 + 16, dt)
+    for pri, sec, damp in ((15 << b8, 0, 1 + b8), (0, 4 << b8, 7 + b8), (16 << b8, 0, 3 + b8), (-1, 1 << b8, 3 + b8),
+                           (0, 3 << b8, 3 + b8), (0, 8 << b8, 3 + b8), (0, (2 << b8) + 1, 3 + b8), (0, -(1 << b8), 3 + b8)):
+        dst = np.full(16 * 10 + 16, 7, dt)
+        args = (dst[8:].ctypes.data, 16 * dst.itemsize, left.ctypes.data, edge[8:].ctypes.data, edge[8:].ctypes.data)
+        assert lib.b200_cdef_fb(*args, pri, sec, 0, damp, 8, 8, 15, (1 << bpc) - 1) == -2, (bpc, pri, sec, damp)
+        assert lib.b200_last_error().startswith(b"b200_cdef_fb: bad arguments")
+        assert (dst == 7).all()
 
 
 def check_fg(new, chk, bpc, seed):
@@ -113,6 +127,7 @@ def check_resize(new, chk, bpc, seed):
 def run_all(lib, bpc, seed):
     from dav1d_b200.dsp import CdefDSPContext, MCDSPContext
     assert check_cdef(CdefDSPContext(bpc, lib=lib), oracle_cdef(bpc), bpc, seed) == 3 * 16 * 8 * 3 * 2
+    check_cdef_rejects(lib, bpc)
     assert check_fg(lib_ctx(lib, bpc), oracle_ctx(bpc), bpc, seed + 1) == 16 * 7
     assert check_resize(MCDSPContext(bpc, lib=lib), refs.oracle_mc_ctx(bpc), bpc, seed + 2) == 7 * 2 * 3 * 2
 
