@@ -386,7 +386,7 @@ class TensorJob(C.Structure):
                 ("full_range", C.c_int32), ("identity", C.c_int32), ("siting_x", C.c_int32), ("siting_y", C.c_int32),
                 ("cy", C.c_int32), ("rv", C.c_int32), ("gu", C.c_int32), ("gv", C.c_int32), ("bu", C.c_int32),
                 ("scale", C.c_float * 3), ("bias", C.c_float * 3), ("antialias", C.c_int32),
-                ("dst", C.c_void_p), ("pitch_c", C.c_int64), ("pitch_y", C.c_int64), ("flip", C.c_int32), ("pad", C.c_int32)]
+                ("dst", C.c_void_p), ("pitch_c", C.c_int64), ("pitch_y", C.c_int64), ("flip", C.c_int32), ("interpolation", C.c_int32)]
 
 
 ABI_STRUCTS = [McFrame, McBlock, CompBlock, BlendBlock, WarpBlock, ItxBlock, LfFrame, CdefFrame, LrFrame, FrameJob,

@@ -4,8 +4,8 @@
 //   export_rgb_kernel     planar R / G / B at the stream's bit depth (nearest chroma sample, integer matrix)
 //   export_tensor_kernel  R / G / B resized (bilinear, chroma upsampling included), normalised, as fp32 / fp16 / bf16 in
 //                         CHW or HWC order: what a model takes, in one pass
-//   export_tensor_aa_kernel  the same with antialiasing (triangle filter) on reduced axes: a separable pass over shared-
-//                         memory tiles, sharing export_tensor_kernel's epilogue
+//   export_tensor_aa_kernel  the same with antialiasing (triangle filter) on reduced axes, or bicubic (plain or
+//                         antialiased): a separable pass over shared-memory tiles, sharing export_tensor_kernel's epilogue
 // Memory bound: a thread owns a run of horizontally adjacent output samples (8 bytes: 8 samples at 8 bit, 4 above), read
 // and written with one 8-byte access where the run is complete and the rows are aligned; the RGB kernel of a vertically
 // sub-sampled picture takes two rows per thread, so that each chroma sample is read once for its 2 x 2 luma quad. The
@@ -341,13 +341,100 @@ struct AaAxis {
     }
 };
 
+// ---- bicubic (B200TensorJob.interpolation = B200_TENSOR_BICUBIC, include/b200av1.h) ----
+// 4 * 256^3 * K(u / 256): the Keys cubic with a = a4 / 4 at u / 256 samples, exact in int32 for 0 <= u
+B200_DEV int keys(int u, int a4)
+{
+    if (u < 256) return ((a4 + 8) * u - (a4 + 12) * 256) * u * u + (1 << 26);
+    if (u < 512) return a4 * ((((u - 1280) * u + 524288) * u) - (1 << 26));
+    return 0;
+}
+
+// One output sample on one axis of one plane: its taps [jlo, jhi] (within [0, n - 1]) and their t_j. Plain (aa = 0): the
+// four taps around P, folded onto the edge (plain_weight); antialiased: every tap with u_j < 512, the weights being the
+// cumulative rounding over them (cubic_weights)
+struct CubicAxis {
+    int64_t P;
+    int sg, a4, jlo, jhi;                            // sg = sigma'
+    B200_DEV CubicAxis(int x, int in, int out, int n, int s, int k, bool aa)
+    {
+        P = floor_div(((int64_t)(2 * x + 1) * in - (int64_t)(1 + k) * out) * (128 >> s), out);
+        if (aa) {
+            sg = imax((int)floor_div((int64_t)in << (8 - s), out), 256); a4 = -2;
+            // u_j < 512 <=> P - 2 sg < 256 j < P + 2 sg
+            jlo = imax((int)(((P - 2 * sg) >> 8) + 1), 0); jhi = imin((int)((P + 2 * sg - 1) >> 8), n - 1);
+        } else {
+            sg = 256; a4 = -3;
+            const int m = (int)(P >> 8);
+            jlo = imax(m - 1, 0); jhi = imin(m + 2, n - 1);
+        }
+    }
+    B200_DEV int t(int j) const
+    {
+        int64_t d = 256 * (int64_t)j - P;
+        d = d < 0 ? -d : d;
+        if (d >= 2 * sg) return 0;
+        return keys(sg == 256 ? (int)d : (int)floor_div(d << 8, sg), a4);
+    }
+    // plain bicubic: the weight of tap j, the sum of the rounded weights of the unclamped taps m - 1 .. m + 2 that clamp to j
+    B200_DEV int plain_weight(int j, int n) const
+    {
+        const int m = (int)(P >> 8);
+        int c = 0, r0 = 0, w = 0;
+        for (int i = m - 1; i <= m + 2; i++) {
+            c += t(i);
+            const int r = (c + (1 << 11)) >> 12;
+            if (iclip(i, 0, n - 1) == j) w += r - r0;
+            r0 = r;
+        }
+        return w;
+    }
+    // antialiased bicubic, called by a whole warp: T, the sum of t_j over the taps
+    B200_DEV int64_t total(int lane) const
+    {
+        int64_t T = 0;
+        for (int i = jlo + lane; i <= jhi; i += 32) T += t(i);
+        for (int o = 16; o; o >>= 1) T += __shfl_xor_sync(0xffffffffu, T, o);
+        return T;
+    }
+    // antialiased bicubic, called by a whole warp: the weight of tap j0 + lane (0 outside [jlo, jhi]). C and R hold C_j and
+    // R_j of tap j0 - 1 (0 and 0 before jlo) and are advanced to tap j0 + 31, so consecutive calls walk the taps in runs of 32
+    B200_DEV int scan_weight(int j0, int lane, int64_t T, int64_t &C, int64_t &R) const
+    {
+        const int jj = j0 + lane;
+        int64_t c = jj >= jlo && jj <= jhi ? t(jj) : 0;
+        for (int o = 1; o < 32; o <<= 1) {
+            const int64_t v = __shfl_up_sync(0xffffffffu, c, o);
+            if (lane >= o) c += v;
+        }
+        c += C;
+        const int64_t r = floor_div(c * 32768 + T, 2 * T);
+        int64_t rp = __shfl_up_sync(0xffffffffu, r, 1);
+        if (lane == 0) rp = R;
+        C = __shfl_sync(0xffffffffu, c, 31); R = __shfl_sync(0xffffffffu, r, 31);
+        return (int)(r - rp);
+    }
+};
+
+// the tensor kernels' filters: export_tensor_kernel's bilinear, export_tensor_aa_kernel's triangle and cubic
+enum { kBilinear = 0, kTriangle = 1, kCubic = 2 };
+template <int F>
+B200_DEV auto filter_axis(const B200TensorJob &j, int x, int in, int out, int n, int s, int k)
+{
+    if constexpr (F == kCubic) return CubicAxis(x, in, out, n, s, k, j.antialias);
+    else return AaAxis(x, in, out, n, s, k);
+}
+
 // A CTA owns kAaCols output columns x th output rows of one job (th = 1 .. kAaRowsMax, chosen per launch so that a single
 // picture still fills the GPU). Per plane it walks the tile's source rows in chunks of kAaChunk: the horizontal sums H' of
 // the chunk (a warp per row, a lane per column; the column weights sit in shared memory, kAaTaps at a time) go to shared
 // memory, then each thread adds wy * H' into the vertical sums of its output pixels. Shared memory does not depend on the
 // reduction factor; source samples are read straight from global memory, each source row once per tile.
+// F = kTriangle: the antialiased bilinear definition; kCubic: both bicubic ones, job.antialias choosing the weight rule
+// in the weight fills alone. The antialiased cubic weights are cumulative sums: a warp owns a column (or an output row)
+// and scans its taps 32 at a time, carrying C_j and R_j in shared memory across tap windows (row chunks).
 constexpr int kAaCols = 32, kAaRowsMax = 32, kAaChunk = 32, kAaTaps = 64;
-template <bool HBD, int DT, bool HWC, int N, bool MIRROR>
+template <bool HBD, int DT, bool HWC, int N, bool MIRROR, int F>
 __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_constant__ TensorBatch<N> b, int th)
 {
     B200_PDL_ENTRY();
@@ -370,19 +457,53 @@ __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_cons
         const int stride = j.stride[p];
         // this lane's column, and the tile's source rows [r_lo, r_hi]
         const bool col_in = x0 + lane < j.out_w;
-        const AaAxis cx(col_in ? x0 + lane : x0, j.w, j.out_w, pw, sh, kx);
+        const auto cx = filter_axis<F>(j, col_in ? x0 + lane : x0, j.w, j.out_w, pw, sh, kx);
         const int ntaps = col_in ? cx.jhi - cx.jlo + 1 : 0;
         int windows = ntaps;                          // tap windows of the widest column
         for (int o = 16; o; o >>= 1) windows = imax(windows, __shfl_xor_sync(0xffffffffu, windows, o));
         windows = (windows + kAaTaps - 1) / kAaTaps;
-        const int r_lo = AaAxis(y0, j.h, j.out_h, ph, sv, ky).jlo, r_hi = AaAxis(y0 + rows - 1, j.h, j.out_h, ph, sv, ky).jhi;
+        const int r_lo = filter_axis<F>(j, y0, j.h, j.out_h, ph, sv, ky).jlo;
+        const int r_hi = filter_axis<F>(j, y0 + rows - 1, j.h, j.out_h, ph, sv, ky).jhi;
         __syncthreads();                              // the previous plane is done with the shared arrays
         if (warp == 0) { cjlo[lane] = cx.jlo; cnt[lane] = ntaps; }
+        // antialiased cubic: T, and C_j / R_j of the last tap weighted so far, of every column (row), each kept by the warp
+        // that owns the column (row): columns and rows warp + 8 q
+        __shared__ int64_t cubic_T[2][kAaCols], cubic_C[2][kAaCols], cubic_R[2][kAaCols];
+        const auto col_axis = [&](int c) { return CubicAxis(x0 + c, j.w, j.out_w, pw, sh, kx, true); };
+        const auto row_axis = [&](int t) { return CubicAxis(y0 + t, j.h, j.out_h, ph, sv, ky, true); };
+        if constexpr (F == kCubic) {
+            if (j.antialias)
+                for (int q = 0; q < kAaCols / 8; q++) {
+                    const int c = warp + 8 * q;
+                    if (x0 + c < j.out_w) cubic_T[0][c] = col_axis(c).total(lane);
+                    if (c < rows) cubic_T[1][c] = row_axis(c).total(lane);
+                    cubic_C[1][c] = cubic_R[1][c] = 0;
+                }
+        }
         const auto fill_wx = [&](int w0) {            // the weights of taps w0 .. w0 + kAaTaps - 1 of every column
+            if constexpr (F == kCubic) {
+                if (j.antialias) {
+                    for (int q = 0; q < kAaCols / 8; q++) {
+                        const int c = warp + 8 * q;
+                        if (x0 + c >= j.out_w) {
+                            wx[c][lane] = wx[c][lane + 32] = 0;
+                            continue;
+                        }
+                        const CubicAxis a = col_axis(c);
+                        int64_t C = w0 ? cubic_C[0][c] : 0, R = w0 ? cubic_R[0][c] : 0;
+                        for (int i = 0; i < kAaTaps; i += 32) wx[c][i + lane] = a.scan_weight(a.jlo + w0 + i, lane, cubic_T[0][c], C, R);
+                        if (lane == 0) { cubic_C[0][c] = C; cubic_R[0][c] = R; }
+                    }
+                    return;
+                }
+            }
             for (int e = tid; e < kAaCols * kAaTaps; e += 256) {
                 const int c = e / kAaTaps, i = e % kAaTaps;
                 const bool in = x0 + c < j.out_w && w0 + i < cnt[c];
-                wx[c][i] = in ? AaAxis(x0 + c, j.w, j.out_w, pw, sh, kx).weight(cjlo[c] + w0 + i) : 0;
+                if constexpr (F == kCubic)
+                    wx[c][i] = in ? CubicAxis(x0 + c, j.w, j.out_w, pw, sh, kx, false).plain_weight(cjlo[c] + w0 + i, pw) : 0;
+                else
+                    wx[c][i] = in ? AaAxis(x0 + c, j.w, j.out_w, pw, sh, kx).weight(cjlo[c] + w0 + i) : 0;
             }
         };
         __syncthreads();
@@ -408,10 +529,24 @@ __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_cons
                 }
             }
 #pragma unroll
-            for (int k = 0; k < kAaChunk / 8; k++) hs[warp + 8 * k][lane] = (h[k] + (1 << 8)) >> 9;
-            for (int e = tid; e < rows * kAaChunk; e += 256) {
-                const int t = e / kAaChunk, r = e % kAaChunk;
-                wy[t][r] = r < nr ? AaAxis(y0 + t, j.h, j.out_h, ph, sv, ky).weight(r0 + r) : 0;
+            for (int k = 0; k < kAaChunk / 8; k++) {
+                if constexpr (F == kCubic) hs[warp + 8 * k][lane] = iclip((h[k] + (1 << 9)) >> 10, 0, 16 * j.bitdepth_max);
+                else hs[warp + 8 * k][lane] = (h[k] + (1 << 8)) >> 9;
+            }
+            if (F == kCubic && j.antialias) {
+                for (int t = warp; t < rows; t += 8) {
+                    int64_t C = cubic_C[1][t], R = cubic_R[1][t];
+                    wy[t][lane] = row_axis(t).scan_weight(r0, lane, cubic_T[1][t], C, R);
+                    if (lane == 0) { cubic_C[1][t] = C; cubic_R[1][t] = R; }
+                }
+            } else {
+                for (int e = tid; e < rows * kAaChunk; e += 256) {
+                    const int t = e / kAaChunk, r = e % kAaChunk;
+                    if constexpr (F == kCubic)
+                        wy[t][r] = r < nr ? CubicAxis(y0 + t, j.h, j.out_h, ph, sv, ky, false).plain_weight(r0 + r, ph) : 0;
+                    else
+                        wy[t][r] = r < nr ? AaAxis(y0 + t, j.h, j.out_h, ph, sv, ky).weight(r0 + r) : 0;
+                }
             }
             __syncthreads();
 #pragma unroll
@@ -426,8 +561,11 @@ __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_cons
             __syncthreads();                          // hs and wy are rewritten by the next chunk
         }
 #pragma unroll
-        for (int k = 0; k < kAaRowsMax / 8; k++)
-            if (warp + 8 * k < rows) qs[p][warp + 8 * k][lane] = (acc[k] + (1 << 16)) >> 17;
+        for (int k = 0; k < kAaRowsMax / 8; k++) {
+            if (warp + 8 * k >= rows) continue;
+            if constexpr (F == kCubic) qs[p][warp + 8 * k][lane] = iclip((acc[k] + (1 << 15)) >> 16, 0, 4 * j.bitdepth_max);
+            else qs[p][warp + 8 * k][lane] = (acc[k] + (1 << 16)) >> 17;
+        }
     }
     __syncthreads();
     const int bdmax = j.bitdepth_max, s = bdmax == 4095 ? 4 : bdmax == 1023 ? 2 : 0;
@@ -484,9 +622,9 @@ static int check_tensor_job(const B200TensorJob &j, const char *who)
     if (!j.src || !in_range(j.w, 1, 65536) || !in_range(j.h, 1, 65536) || !in_range(j.out_w, 1, 65536) || !in_range(j.out_h, 1, 65536) ||
         !in_range(j.ss_hor, 0, 1) || !in_range(j.ss_ver, 0, 1) || !in_range(j.siting_x, 0, 1) || !in_range(j.siting_y, 0, 1) ||
         !in_range(j.dtype, B200_TENSOR_F32, B200_TENSOR_BF16) || !in_range(j.layout, B200_TENSOR_CHW, B200_TENSOR_HWC) ||
-        !in_range(j.antialias, 0, 1) || !in_range(j.flip, 0, 1)) {
-        b200_set_error("%s: bad arguments (%d x %d -> %d x %d, dtype %d, layout %d, antialias %d, flip %d)", who, j.w, j.h,
-                       j.out_w, j.out_h, j.dtype, j.layout, j.antialias, j.flip);
+        !in_range(j.antialias, 0, 1) || !in_range(j.flip, 0, 1) || !in_range(j.interpolation, B200_TENSOR_BILINEAR, B200_TENSOR_BICUBIC)) {
+        b200_set_error("%s: bad arguments (%d x %d -> %d x %d, dtype %d, layout %d, antialias %d, flip %d, interpolation %d)", who,
+                       j.w, j.h, j.out_w, j.out_h, j.dtype, j.layout, j.antialias, j.flip, j.interpolation);
         return -2;
     }
     if (j.identity && (j.mono || j.ss_hor || j.ss_ver)) { b200_set_error("%s: identity matrix needs 4:4:4", who); return -2; }
@@ -507,16 +645,19 @@ static int check_tensor_job(const B200TensorJob &j, const char *who)
     return 0;
 }
 
-// whether a job takes the antialiased kernel: antialias = 1 and a luma axis reduced (sigma > 256, include/b200av1.h)
-static bool tensor_job_aa(const B200TensorJob &j)
+// the kernel a job takes: the bilinear export_tensor_kernel, the tile kernel's triangle (antialias = 1 with a reduced luma
+// axis: sigma > 256, include/b200av1.h) or its cubic (bicubic, plain or antialiased, whatever the scale)
+static int tensor_job_kind(const B200TensorJob &j)
 {
-    return j.antialias && ((int64_t)j.w * 256 / j.out_w > 256 || (int64_t)j.h * 256 / j.out_h > 256);
+    if (j.interpolation == B200_TENSOR_BICUBIC) return kCubic;
+    const bool reduced = (int64_t)j.w * 256 / j.out_w > 256 || (int64_t)j.h * 256 / j.out_h > 256;
+    return j.antialias && reduced ? kTriangle : kBilinear;
 }
 
-// the antialiased kernel's launch: the tallest tile (th output rows) whose grid still has kAaMinCtas CTAs, the SM count of
-// an H100 SXM, so that a single picture reduced to a small output still spreads over the whole GPU
+// the tile kernel's launch: the tallest tile (th output rows) whose grid still has kAaMinCtas CTAs, the SM count of an
+// H100 SXM, so that a single picture reduced to a small output still spreads over the whole GPU
 constexpr int kAaMinCtas = 132;
-template <int N>
+template <int N, int F>
 static int launch_tensor_aa_jobs(const TensorBatch<N> &b, int n, int out_w, int out_h, cudaStream_t stream)
 {
     const B200TensorJob &j = b.job[0];
@@ -527,19 +668,19 @@ static int launch_tensor_aa_jobs(const TensorBatch<N> &b, int n, int out_w, int 
     return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, stream, [&](auto hbd) {
         constexpr bool H = decltype(hbd)::value;
         void (*const k[2][3][2])(TensorBatch<N>, int) = {
-            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, false>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, false>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, false>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, false>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, false>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, false>}},
-            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, true>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, true>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, true>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, true>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, true>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, true>}}};
+            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, false, F>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, false, F>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, false, F>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, false, F>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, false, F>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, false, F>}},
+            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, true, F>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, true, F>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, true, F>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, true, F>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, true, F>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, true, F>}}};
         return std::make_tuple(k[j.flip][j.dtype][j.layout], b, th);
     });
 }
 
-// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype, layout, kernel (aa) and flip
+// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype, layout, kernel kind and flip
 template <int N>
-static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, bool aa, cudaStream_t stream)
+static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, int kind, cudaStream_t stream)
 {
     TensorBatch<N> b{};
     int out_w = 0, out_h = 0;
@@ -547,7 +688,8 @@ static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, bool aa, 
         b.job[i] = *jobs[i];
         out_w = imax(out_w, jobs[i]->out_w); out_h = imax(out_h, jobs[i]->out_h);
     }
-    if (aa) return launch_tensor_aa_jobs(b, n, out_w, out_h, stream);
+    if (kind == kTriangle) return launch_tensor_aa_jobs<N, kTriangle>(b, n, out_w, out_h, stream);
+    if (kind == kCubic) return launch_tensor_aa_jobs<N, kCubic>(b, n, out_w, out_h, stream);
     const B200TensorJob &j = b.job[0];
     const int runs = (out_w + 3) / 4;
     const dim3 grid((runs + 31) / 32, (out_h + 8 * kTensorRows - 1) / (8 * kTensorRows), n);
@@ -563,9 +705,9 @@ static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, bool aa, 
         return std::make_tuple(k[j.flip][j.dtype][j.layout], b);
     });
 }
-static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, bool aa, cudaStream_t stream)
+static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, int kind, cudaStream_t stream)
 {
-    return n == 1 ? launch_tensor_jobs<1>(jobs, n, aa, stream) : launch_tensor_jobs<B200_TENSOR_BATCH_MAX>(jobs, n, aa, stream);
+    return n == 1 ? launch_tensor_jobs<1>(jobs, n, kind, stream) : launch_tensor_jobs<B200_TENSOR_BATCH_MAX>(jobs, n, kind, stream);
 }
 
 extern "C" int b200_export_tensor(const B200TensorJob *job, void *stream)
@@ -583,23 +725,22 @@ extern "C" int b200_export_tensor_batch(const B200TensorJob *jobs, int n, void *
             return -2;
         }
     }
-    // one launch per bit-depth class, kernel (bilinear, antialiased) and flip present and per B200_TENSOR_BATCH_MAX jobs of
-    // it, jobs in their order
-    for (int group = 0; group < 8; group++) {
-        const int hbd = group & 1, flip = group >> 2;
-        const bool aa = (group >> 1) & 1;
+    // one launch per bit-depth class, kernel kind (bilinear, triangle, cubic) and flip present and per
+    // B200_TENSOR_BATCH_MAX jobs of it, jobs in their order
+    for (int group = 0; group < 12; group++) {
+        const int hbd = group & 1, kind = (group >> 1) % 3, flip = group / 6;
         const B200TensorJob *part[B200_TENSOR_BATCH_MAX];
         int m = 0;
         for (int i = 0; i < n; i++) {
-            if ((jobs[i].bitdepth_max > 255) != hbd || tensor_job_aa(jobs[i]) != aa || jobs[i].flip != flip) continue;
+            if ((jobs[i].bitdepth_max > 255) != hbd || tensor_job_kind(jobs[i]) != kind || jobs[i].flip != flip) continue;
             part[m++] = &jobs[i];
             if (m == B200_TENSOR_BATCH_MAX) {
-                if (int r = launch_tensor_jobs(part, m, aa, (cudaStream_t)stream)) return r;
+                if (int r = launch_tensor_jobs(part, m, kind, (cudaStream_t)stream)) return r;
                 m = 0;
             }
         }
         if (m)
-            if (int r = launch_tensor_jobs(part, m, aa, (cudaStream_t)stream)) return r;
+            if (int r = launch_tensor_jobs(part, m, kind, (cudaStream_t)stream)) return r;
     }
     return 0;
 }

@@ -232,6 +232,37 @@ def tensor_weights(out, inn, n, s=0, k=0):
     return np.diff(R, axis=1, prepend=0)
 
 
+TENSOR_INTERPOLATIONS = {"bilinear": 0, "bicubic": 1}
+
+
+def _keys(u, a4):
+    """4 * 256^3 * K(u / 256) of the Keys cubic with a = a4 / 4 (int64 u >= 0), as include/b200av1.h states it"""
+    return np.where(u < 256, (a4 + 8) * u ** 3 - (a4 + 12) * u ** 2 * 256 + 4 * 256 ** 3,
+                    np.where(u < 512, a4 * u ** 3 - 5 * a4 * u ** 2 * 256 + 8 * a4 * u * 256 ** 2 - 4 * a4 * 256 ** 3, 0))
+
+
+def cubic_weights(out, inn, n, s=0, k=0, antialias=False):
+    """[out, n] int64 weights (1/2^14, each row summing to 2^14) of the bicubic tensor export along one axis
+    (include/b200av1.h B200TensorJob, interpolation = B200_TENSOR_BICUBIC); arguments as in tensor_taps. antialias=False:
+    torch's bicubic (a = -3/4), four taps around the unclamped position with the weights of taps beyond the edge added to
+    the edge sample; antialias=True: torch's antialiased bicubic (a = -1/2, half-support 2 * max(scale, 1)), taps clipped
+    at the edges and the weights renormalised. Both with cumulative rounding."""
+    x = np.arange(out, dtype=np.int64)
+    P = ((2 * x + 1) * inn - (1 + k) * out) * (1 << (7 - s)) // out
+    if antialias:
+        sg = max(inn * (1 << (8 - s)) // out, 256)
+        u = np.abs(256 * np.arange(n, dtype=np.int64)[None, :] - P[:, None]) * 256 // sg
+        t = _keys(u, -2)
+        T = t.sum(1, keepdims=True)
+        R = (np.cumsum(t, axis=1) * (1 << 15) + T) // (2 * T)
+        return np.diff(R, axis=1, prepend=0)
+    taps = (P >> 8)[:, None] + np.arange(-1, 3)
+    R = (np.cumsum(_keys(np.abs(256 * taps - P[:, None]), -3), axis=1) + (1 << 11)) >> 12
+    W = np.zeros((out, n), np.int64)
+    np.add.at(W, (np.repeat(x, 4), np.clip(taps, 0, n - 1).ravel()), np.diff(R, axis=1, prepend=0).ravel())
+    return W
+
+
 def tensor_antialiased(w, h, size, antialias):
     """whether an export of a w x h picture to size = (OH, OW) takes the antialiased definition: antialias and a luma axis
     reduced (sigma > 256)"""
@@ -240,19 +271,27 @@ def tensor_antialiased(w, h, size, antialias):
 
 
 def tensor_reference(planes, bpc, layout, size=None, matrix="bt709", full_range=False, siting="left", mean=None, std=None,
-                     antialias=False):
+                     antialias=False, interpolation="bilinear"):
     """numpy statement of the tensor export (include/b200av1.h B200TensorJob) for one picture's planes (layout = enum
     Dav1dPixelLayout): float32 [3, OH, OW] of R, G, B; size = (OH, OW), by default the picture's. antialias=True: the
-    antialiased definition (triangle filter on reduced axes), which leaves exports without a reduced luma axis unchanged."""
+    antialiased definition (triangle filter on reduced axes), which leaves exports without a reduced luma axis unchanged.
+    interpolation="bicubic": the bicubic definition instead, plain or (antialias=True) antialiased on every axis."""
     h, w = planes[0].shape
     oh, ow = size or (h, w)
     ssh, ssv = int(layout in (1, 2)), int(layout == 1)
     kx, ky = SITINGS[siting]
     s, bdmax = bpc - 8, (1 << bpc) - 1
+    _check_interpolation(interpolation)
     aa = tensor_antialiased(w, h, (oh, ow), antialias)
 
     def sample(p, sh, sv, kx, ky):
         p = p.astype(np.int64)
+        if interpolation == "bicubic":
+            wx = cubic_weights(ow, w, p.shape[1], sh, kx if sh else 0, antialias)
+            wy = cubic_weights(oh, h, p.shape[0], sv, ky if sv else 0, antialias)
+            # exact in float64, as below: every partial sum is an integer below 2^31
+            hq = np.clip((np.rint(p.astype(np.float64) @ wx.T.astype(np.float64)).astype(np.int64) + (1 << 9)) >> 10, 0, 16 * bdmax)
+            return np.clip((np.rint(wy.astype(np.float64) @ hq.astype(np.float64)).astype(np.int64) + (1 << 15)) >> 16, 0, 4 * bdmax)
         if aa:
             wx = tensor_weights(ow, w, p.shape[1], sh, kx if sh else 0)
             wy = tensor_weights(oh, h, p.shape[0], sv, ky if sv else 0)
@@ -309,6 +348,11 @@ def _is_box(b):
 
 def _is_flag(f):
     return isinstance(f, (bool, np.bool_))
+
+
+def _check_interpolation(interpolation):
+    if not isinstance(interpolation, str) or interpolation not in TENSOR_INTERPOLATIONS:
+        raise ValueError("interpolation must be 'bilinear' or 'bicubic', not %r" % (interpolation,))
 
 
 class DeviceDecoder:
@@ -368,7 +412,8 @@ class DeviceDecoder:
         yield from self._decode(tus, lambda h, info: self._export(h, info, format, matrix, full_range, alloc, stream))
 
     def tensors(self, tus, size=None, dtype="float32", layout="chw", mean=None, std=None, matrix="auto", full_range=None,
-                chroma_siting="auto", batch=None, alloc=None, stream=None, antialias=False, crop=None, flip=False):
+                chroma_siting="auto", batch=None, alloc=None, stream=None, antialias=False, crop=None, flip=False,
+                interpolation="bilinear"):
         """Decodes the temporal units `tus` and yields every output picture as a model input: R, G, B resized to
         size = (height, width) (default: the picture's own) by bilinear sampling at half-sample centres, like
         torch.nn.functional.interpolate(mode="bilinear", align_corners=False) (chroma upsampling is part of the same
@@ -377,6 +422,10 @@ class DeviceDecoder:
         antialias=True filters reduced axes with a triangle as wide as the reduction, like interpolate(mode="bilinear",
         antialias=True) and torchvision's Resize: what vision models are trained on. It changes nothing when no luma axis
         is reduced.
+        interpolation="bicubic" resamples with a Keys cubic instead, chroma upsampling included: like
+        interpolate(mode="bicubic", align_corners=False) (edge samples replicated), or with antialias=True like
+        interpolate(mode="bicubic", antialias=True), torchvision's Resize(BICUBIC) and PIL's BICUBIC, which filter every
+        axis, enlarged ones too. CLIP, SigLIP and most timm models are trained on the antialiased one.
         batch=N: yields [n, ...] tensors of up to N pictures, each picture exported straight into its slot; a picture of
         another size (size=None with frame-size changes) closes the batch early.
         matrix and full_range: as in pictures(). chroma_siting: "auto" (the sequence header's chroma_sample_position:
@@ -405,6 +454,7 @@ class DeviceDecoder:
             raise ValueError("crop must be None, a box (top, left, height, width) or a callable")
         if not callable(flip) and not _is_flag(flip):
             raise ValueError("flip must be a bool or a callable")
+        _check_interpolation(interpolation)
         tensor_scale_bias(8, mean, std)                          # checks mean / std
         alloc, stream = _default_alloc(alloc, stream)
         esize = 4 if dtype == "float32" else 2
@@ -422,7 +472,7 @@ class DeviceDecoder:
             if batch is None:
                 out = alloc(shape, dtype)
                 self._export_tensor(h, info, _data_ptr(out), oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
-                                    antialias, stream, box, fl)
+                                    antialias, stream, box, fl, interpolation)
                 return [out]
             done = []
             if state["buf"] is not None and state["shape"] != shape:       # another size closes the batch
@@ -432,7 +482,7 @@ class DeviceDecoder:
                 state.update(buf=alloc((int(batch),) + shape, dtype), n=0, shape=shape)
             dst = _data_ptr(state["buf"]) + state["n"] * 3 * oh * ow * esize
             self._export_tensor(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, antialias, stream,
-                                box, fl)
+                                box, fl, interpolation)
             state["n"] += 1
             if state["n"] == batch:
                 done.append(state["buf"])
@@ -446,11 +496,11 @@ class DeviceDecoder:
 
     def clips(self, streams, frames, step=1, start=0, size=None, dtype="float32", layout="chw", mean=None, std=None,
               matrix="auto", full_range=None, chroma_siting="auto", workers=None, alloc=None, stream=None, antialias=False,
-              crop=None, flip=False):
+              crop=None, flip=False, interpolation="bilinear"):
         """Decodes N streams (each a list of temporal units) concurrently and returns one clip per stream as a
         [N, frames, 3, OH, OW] tensor (layout="hwc": [N, frames, OH, OW, 3]): x[i, t] is output picture
         start_i + t * step of stream i, exported exactly as tensors() exports it. `start` is one int or one per stream.
-        size=None needs every sampled picture to have the same size. The tensor options (antialias included), alloc and
+        size=None needs every sampled picture to have the same size. The tensor options (antialias and interpolation included), alloc and
         stream mean what they mean in tensors(); "auto" matrix, range and siting are resolved per stream from its own headers.
         crop: one box (top, left, height, width) for every stream, one box per stream, or a callable (i, height, width) -> box
         called once per stream i on its first sampled picture; flip: one bool, or one per stream. Every picture of a clip
@@ -492,6 +542,7 @@ class DeviceDecoder:
             flips = [bool(f) for f in flip]
         else:
             raise ValueError("flip must be a bool or one bool per stream")
+        _check_interpolation(interpolation)
         tensor_scale_bias(8, mean, std)                          # checks mean / std
         alloc, stream = _default_alloc(alloc, stream)
         self._hooked._bind()
@@ -536,7 +587,7 @@ class DeviceDecoder:
                                              "pictures of different sizes" % (i, starts[i] + t * step, ow, oh, hw[1], hw[0]))
                         dst = _data_ptr(out) + (i * frames + t) * 3 * oh * ow * esize
                         jobs[k] = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
-                                                   antialias, flips[i])
+                                                   antialias, flips[i], interpolation)
                         pics[k] = self.dll.refdrv_stream_picture(h)
                     if self.dll.b200hook_export_tensor_batch(pics, jobs, boxes, len(items), C.c_void_p(stream)) != 0:
                         raise RuntimeError("exporting pictures failed (see stderr)")
@@ -640,13 +691,15 @@ class DeviceDecoder:
         return name
 
     def _export_tensor(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, stream, box,
-                       flip):
-        job = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip)
+                       flip, interpolation):
+        job = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip,
+                               interpolation)
         box = (C.c_int32 * 4)(*box) if box else None
         if self.dll.b200hook_export_tensor(self.dll.refdrv_stream_picture(h), C.byref(job), box, C.c_void_p(stream)) != 0:
             raise RuntimeError("exporting a picture failed (see stderr)")
 
-    def _tensor_job(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip):
+    def _tensor_job(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip,
+                    interpolation="bilinear"):
         """the B200TensorJob of the picture stream h holds (info as _decode gives it): "auto" matrix, range and siting come
         from that stream's own headers"""
         w, hh, bpc, pl, mtrx, color_range = (int(v) for v in info)
@@ -665,6 +718,7 @@ class DeviceDecoder:
             job.scale[c], job.bias[c] = float(scale[c]), float(bias[c])
         job.antialias = int(bool(antialias))
         job.flip = int(flip)
+        job.interpolation = TENSOR_INTERPOLATIONS[interpolation]
         job.dst = dst
         job.pitch_y, job.pitch_c = (ow, oh * ow) if layout == "chw" else (3 * ow, 1)
         return job

@@ -815,6 +815,26 @@ B200_API int b200_export_picture(const B200ExportJob *job, void *stream);
  *       H' = (H + 2^8) >> 9                       5 fractional bits (<= 131040)
  *       V  = sum over rows r of wy_r * H'[r]      int32 (<= 131040 * 2^14)
  *       Q  = (V + 2^16) >> 17                     2 fractional bits, 0 .. 4 * bdmax; the matrix and output below follow
+ *   interpolation = B200_TENSOR_BICUBIC replaces both definitions above (bilinear and triangle) by a Keys cubic, on every
+ *     axis whatever the scale, chroma upsampling included. antialias = 0: torch's interpolate(mode="bicubic",
+ *     align_corners=False), a = -3/4, four taps floor(P / 256) - 1 .. + 2 (P unclamped, unlike pos above) replicated at
+ *     the edge; antialias = 1: interpolate(mode="bicubic", antialias=True), torchvision's Resize(BICUBIC) and PIL's
+ *     BICUBIC, a = -1/2 with half-support 2 * max(scale, 1), taps clipped at the edge and renormalised, on enlarged axes
+ *     too. Per axis and plane, with P and sigma as above:
+ *       sigma' = max(sigma, 256) (antialias = 0: sigma' = 256), a4 = 4a (-3 or -2)
+ *       u_j = floor(|256 j - P| * 256 / sigma')     kernel argument in 1/256
+ *       t_j = 4 * 256^3 * K(u_j / 256), exactly:  (a4 + 8) u^3 - (a4 + 12) u^2 * 256 + 4 * 256^3      for u < 256
+ *                                                 a4 u^3 - 5 a4 u^2 * 256 + 8 a4 u * 256^2 - 4 a4 * 256^3   256 <= u < 512
+ *                                                 0 above
+ *       weights by the cumulative rounding above on the signed t_j, summing to 2^14:
+ *         antialias = 0: over the four unclamped taps (T = 2^26, R_j = (C_j + 2^11) >> 12, a function of P & 255 alone),
+ *           then each weight added to the tap clamped into [0, n - 1]
+ *         antialias = 1: over the taps in [0, n - 1] with u_j < 512 (T > 0: the nearest tap lies within half a sample)
+ *       H  = sum over j of wx_j * S[row][j]             int32
+ *       H' = clip((H + 2^9) >> 10, 0, 16 * bdmax)       4 fractional bits, the per-pass clip of PIL and of torch's uint8 path
+ *       V  = sum over rows r of wy_r * H'[r]            int32 (< 1.3e9 at 12 bit)
+ *       Q  = clip((V + 2^15) >> 16, 0, 4 * bdmax)       the matrix and output below follow
+ *     A same-size 4:4:4 export therefore gives Q = 4 S under either cubic rule, as the bilinear export does.
  *   Matrix, with s = bitdepth - 8: Y' = Qy - (full_range ? 0 : 64 << s), C' = Qc - (512 << s) (mono: Cb' = Cr' = 0), and
  *       R = clip((cy * Y' + rv * Cr' + 8192) >> 14)
  *       G = clip((cy * Y' - gu * Cb' - gv * Cr' + 8192) >> 14)
@@ -832,12 +852,13 @@ B200_API int b200_export_picture(const B200ExportJob *job, void *stream);
  *   Crops are a change of source: the box (top, left, height, width) of the visible picture is the picture whose planes
  *     start at the box (plane_off[0] += top * stride[0] + left, chroma plane_off[p] += (top >> ss_ver) * stride[p] +
  *     (left >> ss_hor)) and whose visible size is w = width, h = height. Taps then stop at the box's edge, as in
- *     torchvision's resized_crop, with the bilinear and the antialiased definition alike. The chroma of the box keeps the
+ *     torchvision's resized_crop, with the bilinear, antialiased and bicubic definitions alike. The chroma of the box keeps the
  *     picture's siting only when top is even where ss_ver and left is even where ss_hor: the hooks' boxes
  *     (b200hook_export_tensor_batch, integration/dav1d/b200_hooks.c) are rejected otherwise.
- * One launch on `stream`; -2 on bad arguments. */
+ * One launch on `stream`; -2 on bad arguments (interpolation included: B200_TENSOR_BILINEAR or B200_TENSOR_BICUBIC). */
 enum { B200_TENSOR_F32 = 0, B200_TENSOR_F16 = 1, B200_TENSOR_BF16 = 2 };
 enum { B200_TENSOR_CHW = 0, B200_TENSOR_HWC = 1 };
+enum { B200_TENSOR_BILINEAR = 0, B200_TENSOR_BICUBIC = 1 };
 typedef struct B200TensorJob {
     const void *src;               /* device picture */
     uint32_t plane_off[3];         /* samples */
@@ -853,14 +874,15 @@ typedef struct B200TensorJob {
     void *dst;                     /* device */
     int64_t pitch_c, pitch_y;      /* elements */
     int32_t flip;                  /* 0, or 1: mirrored horizontally (see above) */
-    int32_t pad;
+    int32_t interpolation;         /* B200_TENSOR_BILINEAR (0) or B200_TENSOR_BICUBIC (see above) */
 } B200TensorJob;
 B200_API int b200_export_tensor(const B200TensorJob *job, void *stream);
 /* n >= 1 tensor jobs at once, e.g. the pictures of a clip batch taken from several streams: each job is exactly what
  * b200_export_tensor(&jobs[i]) writes, with its own source, geometry, bit depth, matrix, range, siting, scale / bias and
  * destination, but all jobs must share dtype and layout. The destinations must not overlap each other (jobs run in no
- * particular order). One launch on `stream` per bit-depth class (8 bit, above 8 bit), kernel (bilinear,
- * antialiased) and flip present, and per B200_TENSOR_BATCH_MAX jobs of it; the jobs ride in the kernel's parameter block. -2 when jobs is NULL, n < 1, dtype or
+ * particular order). One launch on `stream` per bit-depth class (8 bit, above 8 bit), kernel (bilinear; triangle:
+ * antialiased bilinear with a reduced luma axis; cubic: bicubic, plain or antialiased) and flip present, and per
+ * B200_TENSOR_BATCH_MAX jobs of it; the jobs ride in the kernel's parameter block. -2 when jobs is NULL, n < 1, dtype or
  * layout differ, or any job is bad (checked as b200_export_tensor checks it): then nothing is launched. b200_export_tensor
  * is the n = 1 case. */
 #define B200_TENSOR_BATCH_MAX 24

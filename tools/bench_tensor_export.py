@@ -1,7 +1,7 @@
 """The tensor export (b200_export_tensor) against the torch chain it replaces (run on a GPU machine):
 
-    python tools/bench_tensor_export.py [--launches 200] [--rounds 5] [--reps 3] [--antialias | --crop-flip] [--kernel-only]
-                                        [--baseline-lib SO] [--out FILE]
+    python tools/bench_tensor_export.py [--launches 200] [--rounds 5] [--reps 3] [--antialias] [--crop-flip] [--kernel-only]
+                                        [--interpolation bilinear | bicubic] [--baseline-lib SO] [--out FILE]
 
 Kernel level, one JSON line per configuration, on synthetic device pictures (random planes, 4:2:0):
   fused        one b200_export_tensor launch
@@ -23,6 +23,9 @@ Decoder level, one JSON line per stream workload of bench.py: pictures per secon
   224 x 224 bf16 CHW, antialiased and flipped (B200TensorJob source moved to the box, flip = 1), against the chain a user
   writes otherwise: the RGB export of the whole picture, the slice, interpolate(antialias=True), (x - mean) / std,
   .flip(-1), .to(bfloat16).
+--interpolation bicubic: the kernel level only, on BICUBIC_CONFIGS (or CROP_FLIP_CONFIGS with --crop-flip), with
+  B200TensorJob.interpolation = B200_TENSOR_BICUBIC (antialiased with --antialias or --crop-flip) against the chain with
+  interpolate(mode="bicubic", ...).
 --baseline-lib SO: the kernel level times the same jobs (flip = 0) through another build of the library (an earlier
   commit's libb200av1.so) instead of the torch chain, alternated with this tree's, as `fused_baseline`.
 The GPU's name, power limit and SM clock are read in the same run."""
@@ -68,16 +71,24 @@ AA_CONFIGS = [  # (name, source w, h, bpc, output (h, w), dtype, layout, picture
 ]
 
 
+BICUBIC_CONFIGS = [  # AA_CONFIGS' fields: CLIP-style inputs, a downscale to 1080p and an upscale from 720p
+    ("1080p8 -> 224x224 bf16 chw", 1920, 1080, 8, (224, 224), "bfloat16", "chw", 1),
+    ("4k10 -> 398x224 bf16 chw", 3840, 2160, 10, (224, 398), "bfloat16", "chw", 1),
+    ("4k8 -> 1920x1080 fp16 chw", 3840, 2160, 8, (1080, 1920), "float16", "chw", 1),
+    ("720p8 -> 1920x1080 bf16 chw", 1280, 720, 8, (1080, 1920), "bfloat16", "chw", 1),
+]
+
+
 CROP_FLIP_CONFIGS = [  # AA_CONFIGS' fields, then the box (top, left, height, width)
     ("crop+flip 1080p8 -> 224x224 bf16 chw", 1920, 1080, 8, (224, 224), "bfloat16", "chw", 1, (100, 372, 882, 1176)),
     ("crop+flip 4k10 -> 224x224 bf16 chw", 3840, 2160, 10, (224, 224), "bfloat16", "chw", 1, (200, 744, 1764, 2352)),
 ]
 
 
-def torch_chain(rgb, bdmax, size, dtype, layout, mean, std, antialias=False, flip=False):
+def torch_chain(rgb, bdmax, size, dtype, layout, mean, std, antialias=False, flip=False, mode="bilinear"):
     x = rgb.float() / bdmax
     if size is not None:
-        x = F.interpolate(x[None], size=size, mode="bilinear", align_corners=False, antialias=antialias)[0]
+        x = F.interpolate(x[None], size=size, mode=mode, align_corners=False, antialias=antialias)[0]
     x = (x - mean) / std
     x = (x.flip(-1) if flip else x).to(getattr(torch, dtype))
     return x.permute(1, 2, 0).contiguous() if layout == "hwc" else x
@@ -121,7 +132,9 @@ def kernel_level(args):
     lib = _lib.get_lib()
     s = torch.cuda.Stream()
     lines = []
-    configs = CROP_FLIP_CONFIGS if args.crop_flip else AA_CONFIGS if args.antialias else [c + (1,) for c in CONFIGS] + [BATCH_CONFIG]
+    bicubic = args.interpolation == "bicubic"
+    configs = CROP_FLIP_CONFIGS if args.crop_flip else BICUBIC_CONFIGS if bicubic else AA_CONFIGS if args.antialias else \
+        [c + (1,) for c in CONFIGS] + [BATCH_CONFIG]
     base = baseline_lib(args.baseline_lib) if args.baseline_lib else None
     for name, w, h, bpc, size, dtype, layout, pics, *box in configs:
         box = box[0] if box else None
@@ -147,6 +160,7 @@ def kernel_level(args):
             tj.scale[c], tj.bias[c] = float(scale[c]), float(bias[c])
         tj.dst, tj.pitch_c, tj.pitch_y = out.data_ptr(), (oh * ow if layout == "chw" else 1), (ow if layout == "chw" else 3 * ow)
         tj.antialias = int(antialias)
+        tj.interpolation = stream.TENSOR_INTERPOLATIONS[args.interpolation]
         if box is not None:                      # the box is the source; the output is mirrored
             top, left, tj.h, tj.w = box
             tj.plane_off[0] += top * tj.stride[0] + left
@@ -181,7 +195,7 @@ def kernel_level(args):
             for _ in range(pics):
                 lib.check(lib.b200_export_picture(C.byref(ej), sp), "b200_export_picture")
                 x = rgb if box is None else rgb[:, box[0]:box[0] + box[2], box[1]:box[1] + box[3]]
-                torch_chain(x, bdmax, size, dtype, layout, mean, std, antialias, box is not None)
+                torch_chain(x, bdmax, size, dtype, layout, mean, std, antialias, box is not None, args.interpolation)
 
         arms = {"fused": fused}
         if base is not None:                     # the same jobs in the other build's struct layout
@@ -221,6 +235,8 @@ def kernel_level(args):
         line["bytes"] = {k: v for k, v in line["bytes"].items() if k in times}
         if antialias:
             line["antialias"] = True
+        if bicubic:
+            line["interpolation"] = "bicubic"
         if box is not None:
             line["crop_box"], line["flip"] = list(box), True
         if base is not None:
@@ -296,12 +312,16 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--antialias", action="store_true")
     ap.add_argument("--crop-flip", action="store_true")
+    ap.add_argument("--interpolation", choices=list(stream.TENSOR_INTERPOLATIONS), default="bilinear")
     ap.add_argument("--baseline-lib", help="another build of libb200av1.so: time its export of the same jobs instead of the chain")
     ap.add_argument("--kernel-only", action="store_true")
     ap.add_argument("--out")
     args = ap.parse_args()
+    if args.baseline_lib and args.interpolation != "bilinear":
+        ap.error("--baseline-lib compares the bilinear and triangle exports, which an earlier library also has")
     assert torch.cuda.is_available(), "needs a CUDA device"
-    lines = kernel_level(args) + ([] if args.antialias or args.crop_flip or args.kernel_only else decoder_level(args))
+    kernel_only = args.antialias or args.crop_flip or args.kernel_only or args.interpolation != "bilinear"
+    lines = kernel_level(args) + ([] if kernel_only else decoder_level(args))
     if args.out:
         with open(args.out, "w") as fh:
             for line in lines:
