@@ -303,6 +303,7 @@ _SIGS = {
     "b200_export_picture": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_export_tensor": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_export_tensor_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
+    "b200_export_tensor_tone_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     # ---- ipred
     "b200_ipred_batch": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "b200_ipred": (C.c_int, [C.c_int, C.c_void_p, C.c_ssize_t, C.c_void_p] + [C.c_int] * 6),
@@ -389,6 +390,12 @@ class TensorJob(C.Structure):
                 ("dst", C.c_void_p), ("pitch_c", C.c_int64), ("pitch_y", C.c_int64), ("flip", C.c_int32), ("interpolation", C.c_int32)]
 
 
+class ToneMap(C.Structure):
+    """B200ToneMap: the HDR to SDR stage of a tensor export (curve and OETF tables in device memory, gamut matrix)"""
+    _fields_ = [("curve", C.c_void_p), ("oetf", C.c_void_p), ("curve_len", C.c_int32), ("oetf_bits", C.c_int32),
+                ("m", C.c_float * 9), ("pad", C.c_int32)]
+
+
 ABI_STRUCTS = [McFrame, McBlock, CompBlock, BlendBlock, WarpBlock, ItxBlock, LfFrame, CdefFrame, LrFrame, FrameJob,
                Av1Filter, Av1Restoration, FgFrame, FilmGrainData, IntraTx, IntraFrame, McScaledBlock, CoefBlock, IntraSb, CompFusedBlock, FrameBand, ResizeFrame,
-               ExportJob, TensorJob]
+               ExportJob, TensorJob, ToneMap]

@@ -12,6 +12,7 @@
 // tensor kernel's thread owns 4 adjacent output pixels, written per channel with one 16-byte (fp32) or 8-byte store.
 #include "common.cuh"
 #include "host_util.h"
+#include <cmath>
 #ifndef B200_EMU
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -27,6 +28,7 @@ static inline __half __float2half_rn(float v) { return (__half)v; }
 static inline __nv_bfloat16 __float2bfloat16_rn(float v) { return (__nv_bfloat16)v; }
 static inline unsigned short __half_as_ushort(__half h) { unsigned short u; memcpy(&u, &h, 2); return u; }
 static inline unsigned short __bfloat16_as_ushort(__nv_bfloat16 h) { unsigned short u; memcpy(&u, &h, 2); return u; }
+static inline int __float2int_rn(float v) { return (int)lrintf(v); }     // the default rounding mode: to nearest even
 #endif
 
 namespace b200 {
@@ -174,8 +176,9 @@ B200_DEV void run_samples(int (&q)[4], const pixel *plane, int stride, const Tap
 template <int DT> struct TensorElem { typedef uint16_t type; };
 template <> struct TensorElem<B200_TENSOR_F32> { typedef float type; };
 
-template <int DT>
-B200_DEV typename TensorElem<DT>::type tensor_value(int v, float scale, float bias)
+// v: the matrix's integer R, or with a tone map the float T
+template <int DT, class V>
+B200_DEV typename TensorElem<DT>::type tensor_value(V v, float scale, float bias)
 {
     const float f = __fadd_rn(__fmul_rn((float)v, scale), bias);
     if constexpr (DT == B200_TENSOR_F16) return __half_as_ushort(__float2half_rn(f));
@@ -220,12 +223,28 @@ B200_DEV void store_pixels(const B200TensorJob &j, E *row, int x, int n, const E
     }
 }
 
+// The HDR to SDR stage of a tone-mapped job (B200ToneMap, include/b200av1.h): curve, gamut matrix, clip and OETF of the
+// matrix's R, G, B (each 0 .. 4 * bdmax) into T, on the same scale
+B200_DEV void tone_map(const B200ToneMap &t, const int (&rgb)[3], float (&T)[3])
+{
+    float L[3];
+#pragma unroll
+    for (int c = 0; c < 3; c++) L[c] = __ldg(t.curve + rgb[c]);
+    const float top = (float)(1 << t.oetf_bits);
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+        const float g = __fadd_rn(__fadd_rn(__fmul_rn(t.m[3 * r], L[0]), __fmul_rn(t.m[3 * r + 1], L[1])), __fmul_rn(t.m[3 * r + 2], L[2]));
+        T[r] = __ldg(t.oetf + __float2int_rn(__fmul_rn(fminf(fmaxf(g, 0.0f), 1.0f), top)));
+    }
+}
+
 // The epilogue of both tensor kernels: Q of a run of n (<= 4) output pixels at (x, y), per plane, through the matrix, the
-// clip, scale / bias and rounding into the destination (yoff, coff, qmax as include/b200av1.h defines them for the job);
-// MIRROR = j.flip, a parameter of the kernels: jobs with and without a flip take kernels of their own
-template <int DT, bool HWC, bool MIRROR>
-B200_DEV void tensor_store(const B200TensorJob &j, int x, int y, int n, const int (&qy)[4], const int (&qu)[4], const int (&qv)[4],
-                           int yoff, int coff, int qmax)
+// clip, (TONE: the tone map tm) scale / bias and rounding into the destination (yoff, coff, qmax as include/b200av1.h
+// defines them for the job); MIRROR = j.flip and TONE, parameters of the kernels: jobs with and without a flip or a tone
+// map take kernels of their own
+template <int DT, bool HWC, bool MIRROR, bool TONE>
+B200_DEV void tensor_store(const B200TensorJob &j, const B200ToneMap *tm, int x, int y, int n, const int (&qy)[4], const int (&qu)[4],
+                           const int (&qv)[4], int yoff, int coff, int qmax)
 {
     typedef typename TensorElem<DT>::type E;
     E o[3][4];
@@ -240,8 +259,15 @@ B200_DEV void tensor_store(const B200TensorJob &j, int x, int y, int n, const in
             rgb[1] = iclip((yy - j.gu * cb - j.gv * cr) >> 14, 0, qmax);
             rgb[2] = iclip((yy + j.bu * cb) >> 14, 0, qmax);
         }
+        if constexpr (TONE) {
+            float T[3];
+            tone_map(*tm, rgb, T);
 #pragma unroll
-        for (int c = 0; c < 3; c++) o[c][i] = tensor_value<DT>(rgb[c], j.scale[c], j.bias[c]);
+            for (int c = 0; c < 3; c++) o[c][i] = tensor_value<DT>(T[c], j.scale[c], j.bias[c]);
+        } else {
+#pragma unroll
+            for (int c = 0; c < 3; c++) o[c][i] = tensor_value<DT>(rgb[c], j.scale[c], j.bias[c]);
+        }
     }
     E *const row = (E *)j.dst + y * j.pitch_y;
     store_pixels<MIRROR, HWC>(j, row, x, n, o);
@@ -250,16 +276,26 @@ B200_DEV void tensor_store(const B200TensorJob &j, int x, int y, int n, const in
 // The jobs of one launch travel in the kernel's parameter block (no staging copy): B200_TENSOR_BATCH_MAX of them fit the
 // classic 4 KB limit. A one-job launch takes the N = 1 form: its job's fields are then read at fixed parameter offsets, as
 // operands of the instructions that use them; indexed by blockIdx.z they are separate loads, which made the prologue of a
-// small one-picture export up to a quarter slower.
-template <int N> struct TensorBatch { B200TensorJob job[N]; };
-static_assert(sizeof(TensorBatch<B200_TENSOR_BATCH_MAX>) <= 4096, "the jobs of one launch must fit a 4 KB kernel parameter block");
+// small one-picture export up to a quarter slower. Tone-mapped jobs (TONE) carry their B200ToneMap beside them, and
+// always take the batched form.
+template <int N, bool TONE> struct TensorBatch { B200TensorJob job[N]; };
+template <int N> struct TensorBatch<N, true> { B200TensorJob job[N]; B200ToneMap tone[N]; };
+static_assert(sizeof(TensorBatch<B200_TENSOR_BATCH_MAX, false>) <= 4096, "the jobs of one launch must fit a 4 KB kernel parameter block");
+static_assert(sizeof(TensorBatch<B200_TENSOR_TONE_BATCH_MAX, true>) <= 4096,
+              "the tone-mapped jobs of one launch must fit a 4 KB kernel parameter block");
+template <int N, bool TONE>
+B200_DEV const B200ToneMap *tone_of(const TensorBatch<N, TONE> &b)
+{
+    if constexpr (TONE) return &b.tone[N == 1 ? 0 : blockIdx.z];
+    else return nullptr;
+}
 
 // grid (runs of 4 output columns / 32, output rows / (8 * kTensorRows), jobs), block (32, 8): x / y cover the largest
 // output of the launch, z selects the job. A thread converts its run of 4 columns on kTensorRows rows 8 apart, so the
 // column taps are worked out once for all of them
 constexpr int kTensorRows = 4;
-template <bool HBD, int DT, bool HWC, int N, bool MIRROR>
-__global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constant__ TensorBatch<N> b)
+template <bool HBD, int DT, bool HWC, int N, bool MIRROR, bool TONE>
+__global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constant__ TensorBatch<N, TONE> b)
 {
     B200_PDL_ENTRY();
     typedef typename Bd<HBD>::pixel pixel;
@@ -285,7 +321,7 @@ __global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constan
             run_samples(qu, src + j.plane_off[1], j.stride[1], crow, ch, ct);
             run_samples(qv, src + j.plane_off[2], j.stride[2], crow, ch, ct);
         }
-        tensor_store<DT, HWC, MIRROR>(j, x, y, n, qy, qu, qv, yoff, coff, qmax);
+        tensor_store<DT, HWC, MIRROR, TONE>(j, tone_of(b), x, y, n, qy, qu, qv, yoff, coff, qmax);
     }
 }
 
@@ -434,8 +470,8 @@ B200_DEV auto filter_axis(const B200TensorJob &j, int x, int in, int out, int n,
 // in the weight fills alone. The antialiased cubic weights are cumulative sums: a warp owns a column (or an output row)
 // and scans its taps 32 at a time, carrying C_j and R_j in shared memory across tap windows (row chunks).
 constexpr int kAaCols = 32, kAaRowsMax = 32, kAaChunk = 32, kAaTaps = 64;
-template <bool HBD, int DT, bool HWC, int N, bool MIRROR, int F>
-__global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_constant__ TensorBatch<N> b, int th)
+template <bool HBD, int DT, bool HWC, int N, bool MIRROR, int F, bool TONE>
+__global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_constant__ TensorBatch<N, TONE> b, int th)
 {
     B200_PDL_ENTRY();
     typedef typename Bd<HBD>::pixel pixel;
@@ -580,7 +616,7 @@ __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_cons
             qy[i] = qs[0][t][c + i];
             if (!j.mono) { qu[i] = qs[1][t][c + i]; qv[i] = qs[2][t][c + i]; }
         }
-        tensor_store<DT, HWC, MIRROR>(j, x, y0 + t, imin(4, j.out_w - x), qy, qu, qv, yoff, coff, 4 * bdmax);
+        tensor_store<DT, HWC, MIRROR, TONE>(j, tone_of(b), x, y0 + t, imin(4, j.out_w - x), qy, qu, qv, yoff, coff, 4 * bdmax);
     }
 }
 
@@ -657,8 +693,8 @@ static int tensor_job_kind(const B200TensorJob &j)
 // the tile kernel's launch: the tallest tile (th output rows) whose grid still has kAaMinCtas CTAs, the SM count of an
 // H100 SXM, so that a single picture reduced to a small output still spreads over the whole GPU
 constexpr int kAaMinCtas = 132;
-template <int N, int F>
-static int launch_tensor_aa_jobs(const TensorBatch<N> &b, int n, int out_w, int out_h, cudaStream_t stream)
+template <int N, int F, bool T>
+static int launch_tensor_aa_jobs(const TensorBatch<N, T> &b, int n, int out_w, int out_h, cudaStream_t stream)
 {
     const B200TensorJob &j = b.job[0];
     const int xt = (out_w + kAaCols - 1) / kAaCols;
@@ -667,47 +703,53 @@ static int launch_tensor_aa_jobs(const TensorBatch<N> &b, int n, int out_w, int 
     const dim3 grid(xt, (out_h + th - 1) / th, n);
     return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, stream, [&](auto hbd) {
         constexpr bool H = decltype(hbd)::value;
-        void (*const k[2][3][2])(TensorBatch<N>, int) = {
-            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, false, F>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, false, F>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, false, F>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, false, F>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, false, F>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, false, F>}},
-            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, true, F>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, true, F>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, true, F>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, true, F>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, true, F>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, true, F>}}};
+        void (*const k[2][3][2])(TensorBatch<N, T>, int) = {
+            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, false, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, false, F, T>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, false, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, false, F, T>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, false, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, false, F, T>}},
+            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, true, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, true, F, T>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, true, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, true, F, T>},
+             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, true, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, true, F, T>}}};
         return std::make_tuple(k[j.flip][j.dtype][j.layout], b, th);
     });
 }
 
-// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype, layout, kernel kind and flip
-template <int N>
-static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, int kind, cudaStream_t stream)
+// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype, layout, kernel kind and flip, and with
+// T the tone maps at `tones`
+template <int N, bool T>
+static int launch_tensor_jobs(const B200TensorJob *const *jobs, const B200ToneMap *const *tones, int n, int kind, cudaStream_t stream)
 {
-    TensorBatch<N> b{};
+    TensorBatch<N, T> b{};
     int out_w = 0, out_h = 0;
     for (int i = 0; i < n; i++) {
         b.job[i] = *jobs[i];
+        if constexpr (T) b.tone[i] = *tones[i];
         out_w = imax(out_w, jobs[i]->out_w); out_h = imax(out_h, jobs[i]->out_h);
     }
-    if (kind == kTriangle) return launch_tensor_aa_jobs<N, kTriangle>(b, n, out_w, out_h, stream);
-    if (kind == kCubic) return launch_tensor_aa_jobs<N, kCubic>(b, n, out_w, out_h, stream);
+    if (kind == kTriangle) return launch_tensor_aa_jobs<N, kTriangle, T>(b, n, out_w, out_h, stream);
+    if (kind == kCubic) return launch_tensor_aa_jobs<N, kCubic, T>(b, n, out_w, out_h, stream);
     const B200TensorJob &j = b.job[0];
     const int runs = (out_w + 3) / 4;
     const dim3 grid((runs + 31) / 32, (out_h + 8 * kTensorRows - 1) / (8 * kTensorRows), n);
     return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, stream, [&](auto hbd) {
         constexpr bool H = decltype(hbd)::value;
-        void (*const k[2][3][2])(TensorBatch<N>) = {
-            {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, false>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, false>},
-             {export_tensor_kernel<H, B200_TENSOR_F16, false, N, false>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, false>},
-             {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, false>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, false>}},
-            {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, true>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, true>},
-             {export_tensor_kernel<H, B200_TENSOR_F16, false, N, true>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, true>},
-             {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, true>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, true>}}};
+        void (*const k[2][3][2])(TensorBatch<N, T>) = {
+            {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, false, T>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, false, T>},
+             {export_tensor_kernel<H, B200_TENSOR_F16, false, N, false, T>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, false, T>},
+             {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, false, T>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, false, T>}},
+            {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, true, T>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, true, T>},
+             {export_tensor_kernel<H, B200_TENSOR_F16, false, N, true, T>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, true, T>},
+             {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, true, T>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, true, T>}}};
         return std::make_tuple(k[j.flip][j.dtype][j.layout], b);
     });
 }
-static int launch_tensor_jobs(const B200TensorJob *const *jobs, int n, int kind, cudaStream_t stream)
+// the tone-mapped forms are batched forms only: the N = 1 specialisation would double their build time for a prologue
+static int launch_tensor_group(const B200TensorJob *const *jobs, const B200ToneMap *const *tones, int n, int kind, int tone,
+                               cudaStream_t stream)
 {
-    return n == 1 ? launch_tensor_jobs<1>(jobs, n, kind, stream) : launch_tensor_jobs<B200_TENSOR_BATCH_MAX>(jobs, n, kind, stream);
+    if (tone) return launch_tensor_jobs<B200_TENSOR_TONE_BATCH_MAX, true>(jobs, tones, n, kind, stream);
+    return n == 1 ? launch_tensor_jobs<1, false>(jobs, tones, n, kind, stream)
+                  : launch_tensor_jobs<B200_TENSOR_BATCH_MAX, false>(jobs, tones, n, kind, stream);
 }
 
 extern "C" int b200_export_tensor(const B200TensorJob *job, void *stream)
@@ -717,30 +759,54 @@ extern "C" int b200_export_tensor(const B200TensorJob *job, void *stream)
 
 extern "C" int b200_export_tensor_batch(const B200TensorJob *jobs, int n, void *stream)
 {
-    if (!jobs || n < 1) { b200_set_error("b200_export_tensor_batch: no jobs (%d)", n); return -2; }
+    return b200_export_tensor_tone_batch(jobs, nullptr, n, stream);
+}
+
+// a job's tone map, checked as it arrives from outside the library: 0, or -2 with the error set
+static int check_tone_map(const B200ToneMap &t, const B200TensorJob &j, int i)
+{
+    bool finite = true;
+    for (int k = 0; k < 9; k++) finite &= std::isfinite(t.m[k]);
+    if (!t.curve || !t.oetf || t.curve_len != 4 * j.bitdepth_max + 1 || t.oetf_bits < 8 || t.oetf_bits > 16 || !finite) {
+        b200_set_error("b200_export_tensor_tone_batch: bad tone map of job %d (curve_len %d for bitdepth_max %d, oetf_bits %d)", i,
+                       t.curve_len, j.bitdepth_max, t.oetf_bits);
+        return -2;
+    }
+    return 0;
+}
+
+extern "C" int b200_export_tensor_tone_batch(const B200TensorJob *jobs, const B200ToneMap *const *tones, int n, void *stream)
+{
+    const char *const who = tones ? "b200_export_tensor_tone_batch" : n == 1 ? "b200_export_tensor" : "b200_export_tensor_batch";
+    if (!jobs || n < 1) { b200_set_error("%s: no jobs (%d)", who, n); return -2; }
     for (int i = 0; i < n; i++) {
-        if (int r = check_tensor_job(jobs[i], n == 1 ? "b200_export_tensor" : "b200_export_tensor_batch")) return r;
+        if (int r = check_tensor_job(jobs[i], who)) return r;
         if (jobs[i].dtype != jobs[0].dtype || jobs[i].layout != jobs[0].layout) {
-            b200_set_error("b200_export_tensor_batch: job %d has another dtype or layout than job 0", i);
+            b200_set_error("%s: job %d has another dtype or layout than job 0", who, i);
             return -2;
         }
+        if (tones && tones[i])
+            if (int r = check_tone_map(*tones[i], jobs[i], i)) return r;
     }
-    // one launch per bit-depth class, kernel kind (bilinear, triangle, cubic) and flip present and per
-    // B200_TENSOR_BATCH_MAX jobs of it, jobs in their order
-    for (int group = 0; group < 12; group++) {
-        const int hbd = group & 1, kind = (group >> 1) % 3, flip = group / 6;
+    // one launch per bit-depth class, kernel kind (bilinear, triangle, cubic), flip and tone map present and per
+    // B200_TENSOR_BATCH_MAX (tone-mapped: B200_TENSOR_TONE_BATCH_MAX) jobs of it, jobs in their order
+    for (int group = 0; group < 24; group++) {
+        const int hbd = group & 1, kind = (group >> 1) % 3, flip = (group / 6) & 1, tone = group / 12;
+        const int cap = tone ? B200_TENSOR_TONE_BATCH_MAX : B200_TENSOR_BATCH_MAX;
         const B200TensorJob *part[B200_TENSOR_BATCH_MAX];
+        const B200ToneMap *tpart[B200_TENSOR_BATCH_MAX];
         int m = 0;
         for (int i = 0; i < n; i++) {
-            if ((jobs[i].bitdepth_max > 255) != hbd || tensor_job_kind(jobs[i]) != kind || jobs[i].flip != flip) continue;
-            part[m++] = &jobs[i];
-            if (m == B200_TENSOR_BATCH_MAX) {
-                if (int r = launch_tensor_jobs(part, m, kind, (cudaStream_t)stream)) return r;
+            const B200ToneMap *const t = tones ? tones[i] : nullptr;
+            if ((jobs[i].bitdepth_max > 255) != hbd || tensor_job_kind(jobs[i]) != kind || jobs[i].flip != flip || !!t != tone) continue;
+            part[m] = &jobs[i]; tpart[m++] = t;
+            if (m == cap) {
+                if (int r = launch_tensor_group(part, tpart, m, kind, tone, (cudaStream_t)stream)) return r;
                 m = 0;
             }
         }
         if (m)
-            if (int r = launch_tensor_jobs(part, m, kind, (cudaStream_t)stream)) return r;
+            if (int r = launch_tensor_group(part, tpart, m, kind, tone, (cudaStream_t)stream)) return r;
     }
     return 0;
 }

@@ -56,7 +56,8 @@ def obu(obu_type, payload):
     return bytes([(obu_type << 3) | 2]) + leb128(len(payload)) + payload
 
 
-OBU_SEQ_HDR, OBU_TD, OBU_FRAME_HDR, OBU_FRAME = 1, 2, 3, 6
+OBU_SEQ_HDR, OBU_TD, OBU_FRAME_HDR, OBU_METADATA, OBU_FRAME = 1, 2, 3, 5, 6
+METADATA_HDR_CLL, METADATA_HDR_MDCV = 1, 2
 
 
 # 4:2:2 (layout="422") is expressible in the headers below, but random tile payloads are only sometimes legal 4:2:2 streams:
@@ -75,7 +76,8 @@ def sequence_header(w, h, bpc=8, sb128=0, film_grain=0, filter_intra=1, intra_ed
                     chroma_sample_position=0, color=None):
     """chroma_sample_position (4:2:0 only): enum Dav1dChromaSamplePosition, 0 unknown, 1 vertical, 2 colocated;
     color = (matrix_coefficients, color_range): a colour description with BT.709 primaries and transfer (matrix 0, identity,
-    is not supported here); None writes none and limited range"""
+    is not supported here), or (matrix_coefficients, color_range, color_primaries, transfer_characteristics); None writes
+    none and limited range"""
     b = BitWriter()
     profile = _profile(bpc, layout)
     b.f(3, profile)
@@ -108,7 +110,8 @@ def sequence_header(w, h, bpc=8, sb128=0, film_grain=0, filter_intra=1, intra_ed
     b.f(1, color is not None)                # color_description_present
     if color is not None:
         assert color[0] != 0, "identity matrix_coefficients need the sRGB special case"
-        b.f(8, 1); b.f(8, 1); b.f(8, color[0])   # color_primaries, transfer_characteristics (BT.709), matrix_coefficients
+        pri, trc = color[2:4] if len(color) == 4 else (1, 1)
+        b.f(8, pri); b.f(8, trc); b.f(8, color[0])   # color_primaries, transfer_characteristics, matrix_coefficients
     b.f(1, color[1] if color is not None else 0)  # color_range
     if not mono:
         if profile == 2 and bpc == 12:       # explicit subsampling
@@ -286,6 +289,26 @@ def key_frame(rng, w, h, sb128=0, log2_cols=0, log2_rows=0, payload_bytes_per_sb
     if film_grain_seq:
         _film_grain_params(b, rng, 0, layout)
     return obu(OBU_FRAME, _tile_group(b, rng, cols, rows, tile_w, tile_h, sbw, sbh, sb128, payload_bytes_per_sb64))
+
+
+def metadata_hdr_cll(max_cll, max_fall):
+    """OBU_METADATA of type HDR_CLL (AV1 spec 5.8.3): MaxCLL and MaxFALL in cd/m^2, for a temporal unit ahead of its frame"""
+    b = BitWriter()
+    b.f(16, max_cll); b.f(16, max_fall)
+    b.trailing()
+    return obu(OBU_METADATA, leb128(METADATA_HDR_CLL) + b.bytes())
+
+
+def metadata_hdr_mdcv(max_luminance, min_luminance, primaries=((0.708, 0.292), (0.170, 0.797), (0.131, 0.046)),
+                      white=(0.3127, 0.3290)):
+    """OBU_METADATA of type HDR_MDCV (AV1 spec 5.8.4): the mastering display's max / min luminance in cd/m^2 (stored as
+    24.8 / 18.14 fixed point), its primaries (R, G, B) and white point as CIE 1931 xy (0.16 fixed point)"""
+    b = BitWriter()
+    for x, y in list(primaries) + [white]:
+        b.f(16, round(x * 65536)); b.f(16, round(y * 65536))
+    b.f(32, round(max_luminance * 256)); b.f(32, round(min_luminance * 16384))
+    b.trailing()
+    return obu(OBU_METADATA, leb128(METADATA_HDR_MDCV) + b.bytes())
 
 
 def temporal_unit(*obus):
@@ -490,13 +513,14 @@ def show_existing_frame(slot):
 
 
 def inter_stream(seed, w, h, n_frames=3, bpc=8, sb128=0, log2_cols=0, log2_rows=0, motion_modes=0, film_grain=0, screen_content=0, layout="420",
-                 hidden_every=0, intra_only_every=0, sizes=None, super_res=0, chroma_sample_position=0, color=None, **kw):
+                 hidden_every=0, intra_only_every=0, sizes=None, super_res=0, chroma_sample_position=0, color=None, metadata=(), **kw):
     """Temporal units: one key frame, then n_frames - 1 inter frames (single and compound references incl. wedge /
     difference-weighted masks and distance weights, switchable interpolation filters, variable transform trees, intra
     blocks; identity global motion). motion_modes=1 additionally enables the per-block motion mode (overlapped block
     motion compensation, locally warped motion), motion_modes=2 inter-intra prediction as well. hidden_every=k makes
     every k-th inter frame a hidden future frame (decoded early, referenced with backward prediction, output later by a
-    show_existing_frame header). color: the sequence header's colour description (sequence_header)."""
+    show_existing_frame header). color: the sequence header's colour description (sequence_header); metadata: OBUs
+    (metadata_hdr_cll, metadata_hdr_mdcv) placed behind the sequence header, which dav1d attaches to every later picture."""
     rng = np.random.default_rng(seed)
     seq = sequence_header(w, h, bpc=bpc, sb128=sb128, inter_intra=1 if motion_modes >= 2 else 0, warped_motion=1 if motion_modes else 0, film_grain=film_grain, screen_content=screen_content, layout=layout, super_res=super_res,
                           chroma_sample_position=chroma_sample_position, color=color)
@@ -508,7 +532,7 @@ def inter_stream(seed, w, h, n_frames=3, bpc=8, sb128=0, log2_cols=0, log2_rows=
     if film_grain:
         kw = dict(kw, film_grain_seq=1)
     hints = [0] * 8
-    tus = [temporal_unit(seq, key_frame(rng, w, h, sb128=sb128, log2_cols=log2_cols, log2_rows=log2_rows, film_grain_seq=film_grain, screen_content=screen_content, layout=layout, super_res=super_res))]
+    tus = [temporal_unit(seq, *metadata, key_frame(rng, w, h, sb128=sb128, log2_cols=log2_cols, log2_rows=log2_rows, film_grain_seq=film_grain, screen_content=screen_content, layout=layout, super_res=super_res))]
     for i in range(1, n_frames):
         if intra_only_every and i % intra_only_every == 0:
             refresh = int(rng.integers(1, 255))

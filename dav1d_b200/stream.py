@@ -11,7 +11,7 @@ import threading
 
 import numpy as np
 
-from ._lib import ExportJob, TensorJob  # noqa: F401  (B200ExportJob / B200TensorJob, filled by DeviceDecoder)
+from ._lib import ExportJob, TensorJob, ToneMap  # noqa: F401  (B200ExportJob / B200TensorJob / B200ToneMap, filled by DeviceDecoder)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -263,6 +263,127 @@ def cubic_weights(out, inn, n, s=0, k=0, antialias=False):
     return W
 
 
+# ---- HDR to SDR (B200ToneMap, include/b200av1.h): the curves in float64 --------------------------------------------
+# the sequence header's transfer_characteristics (enum Dav1dTransferCharacteristics) of the transfers tone_tables knows
+TRANSFERS = {"pq": 16, "hlg": 18}
+# color_primaries (enum Dav1dColorPrimaries) -> CIE 1931 xy of R, G, B; 2 (unspecified) is taken as BT.2020 for PQ / HLG
+PRIMARIES = {1: ((0.640, 0.330), (0.300, 0.600), (0.150, 0.060)),      # BT.709
+             9: ((0.708, 0.292), (0.170, 0.797), (0.131, 0.046)),      # BT.2020
+             12: ((0.680, 0.320), (0.265, 0.690), (0.150, 0.060))}     # P3-D65 (SMPTE EG 432-1)
+PRIMARIES[2] = PRIMARIES[9]
+D65 = (0.3127, 0.3290)
+SDR_PEAK = 203.0                         # cd/m^2: BT.2408's HDR reference white, where SDR white lands
+HDR_PEAK = 1000.0                        # cd/m^2: the source peak without metadata, and HLG's nominal display peak
+PQ_M1, PQ_M2 = 2610 / 16384, 2523 / 4096 * 128
+PQ_C1, PQ_C2, PQ_C3 = 3424 / 4096, 2413 / 4096 * 32, 2392 / 4096 * 32
+HLG_A = 0.17883277
+HLG_B, HLG_C = 1 - 4 * HLG_A, 0.5 - HLG_A * np.log(4 * HLG_A)
+BT709_ALPHA, BT709_BETA = 1.09929682680944, 0.018053968510807
+
+
+def pq_eotf(e):
+    """SMPTE ST 2084: non-linear signal e in [0, 1] -> display light in cd/m^2"""
+    p = np.power(np.clip(np.asarray(e, np.float64), 0, 1), 1 / PQ_M2)
+    return 10000 * np.power(np.maximum(p - PQ_C1, 0) / (PQ_C2 - PQ_C3 * p), 1 / PQ_M1)
+
+
+def pq_inverse_eotf(lum):
+    """display light in cd/m^2 (0 .. 10000) -> the ST 2084 signal"""
+    y = np.power(np.clip(np.asarray(lum, np.float64) / 10000, 0, 1), PQ_M1)
+    return np.power((PQ_C1 + PQ_C2 * y) / (1 + PQ_C3 * y), PQ_M2)
+
+
+def hlg_inverse_oetf(e):
+    """BT.2100 HLG: non-linear signal e in [0, 1] -> normalised scene light E in [0, 1]"""
+    e = np.clip(np.asarray(e, np.float64), 0, 1)
+    return np.where(e <= 0.5, e * e / 3, (np.exp((e - HLG_C) / HLG_A) + HLG_B) / 12)
+
+
+def hlg_gamma(lw):
+    """the HLG system gamma of a display of peak lw cd/m^2 (BT.2100)"""
+    return 1.2 + 0.42 * np.log10(lw / 1000.0)
+
+
+def eetf(lum, peak, sdr_peak):
+    """BT.2390 EETF on display light (cd/m^2): the PQ-domain Hermite knee from source peak `peak` to target peak `sdr_peak`,
+    black at 0 on both sides. Light above `peak` clips to it; with sdr_peak >= peak nothing is compressed."""
+    lum = np.minimum(np.asarray(lum, np.float64), peak)
+    if sdr_peak >= peak:
+        return lum
+    black, white = pq_inverse_eotf(0.0), pq_inverse_eotf(peak)
+    e1 = np.clip((pq_inverse_eotf(lum) - black) / (white - black), 0, 1)
+    max_lum = (pq_inverse_eotf(sdr_peak) - black) / (white - black)
+    ks = 1.5 * max_lum - 0.5
+    t = (e1 - ks) / (1 - ks)
+    knee = (2 * t ** 3 - 3 * t ** 2 + 1) * ks + (t ** 3 - 2 * t ** 2 + t) * (1 - ks) + (-2 * t ** 3 + 3 * t ** 2) * max_lum
+    e2 = np.where(e1 < ks, e1, knee)
+    return pq_eotf(e2 * (white - black) + black)
+
+
+def bt709_oetf(lin):
+    """the BT.709 OETF with its exact constants: linear light in [0, 1] -> R', G', B' in [0, 1]"""
+    lin = np.clip(np.asarray(lin, np.float64), 0, 1)
+    return np.where(lin < BT709_BETA, 4.5 * lin, BT709_ALPHA * np.power(lin, 0.45) - (BT709_ALPHA - 1))
+
+
+def _rgb_to_xyz(prim):
+    xy = np.array(prim, np.float64)
+    m = np.stack([xy[:, 0] / xy[:, 1], np.ones(3), (1 - xy[:, 0] - xy[:, 1]) / xy[:, 1]])
+    white = np.array([D65[0] / D65[1], 1.0, (1 - D65[0] - D65[1]) / D65[1]])
+    return m * np.linalg.solve(m, white)[None, :]
+
+
+def gamut_matrix(primaries):
+    """float64 [3, 3]: linear RGB in the primaries of `primaries` (color_primaries code 1, 2, 9 or 12) -> linear BT.709 RGB,
+    both with a D65 white. ValueError for any other code."""
+    if primaries not in PRIMARIES:
+        raise ValueError("tone mapping knows color_primaries 1 (BT.709), 2 (unspecified: BT.2020), 9 (BT.2020) and 12 "
+                         "(P3-D65), not %r" % (primaries,))
+    if PRIMARIES[primaries] == PRIMARIES[1]:
+        return np.eye(3)
+    return np.linalg.solve(_rgb_to_xyz(PRIMARIES[1]), _rgb_to_xyz(PRIMARIES[primaries]))
+
+
+def tone_light(transfer, e, peak, sdr_peak=SDR_PEAK):
+    """float64 statement of the curve table: signal e in [0, 1] -> the EETF's display light over sdr_peak, in [0, 1].
+    PQ: the ST 2084 EOTF; HLG: peak * E^gamma per channel on the scene light E (peak = the display's Lw)."""
+    if transfer == "pq":
+        lum = pq_eotf(e)
+    else:
+        lum = peak * np.power(hlg_inverse_oetf(e), hlg_gamma(peak))
+    return np.clip(eetf(lum, peak, sdr_peak) / sdr_peak, 0, 1)
+
+
+def tone_tables(transfer, primaries, bpc, peak=None, sdr_peak=SDR_PEAK, bits=16):
+    """(curve, m, oetf) of a B200ToneMap (include/b200av1.h), computed in float64 and rounded once to float32: curve
+    [4 * bdmax + 1] = tone_light of R / (4 * bdmax), m [3, 3] = gamut_matrix(primaries), oetf [2^bits + 1] =
+    4 * bdmax * bt709_oetf(i / 2^bits). transfer: "pq" or "hlg" (or its transfer_characteristics code, 16 or 18); peak: the
+    source peak in cd/m^2 (None: 1000); sdr_peak: the light that becomes SDR white."""
+    transfer = {v: k for k, v in TRANSFERS.items()}.get(transfer, transfer)
+    if transfer not in TRANSFERS:
+        raise ValueError("transfer must be 'pq' or 'hlg', not %r" % (transfer,))
+    if bpc not in (8, 10, 12) or not 8 <= int(bits) <= 16:
+        raise ValueError("bpc must be 8, 10 or 12 and bits 8 .. 16")
+    peak = HDR_PEAK if peak is None else float(peak)
+    if not (np.isfinite(peak) and peak > 0 and np.isfinite(sdr_peak) and sdr_peak > 0):
+        raise ValueError("peak and sdr_peak must be positive (cd/m^2)")
+    qmax = 4 * ((1 << bpc) - 1)
+    curve = tone_light(transfer, np.arange(qmax + 1) / qmax, peak, float(sdr_peak)).astype(np.float32)
+    oetf = (qmax * bt709_oetf(np.arange((1 << bits) + 1) / (1 << bits))).astype(np.float32)
+    return curve, gamut_matrix(primaries).astype(np.float32), oetf
+
+
+def tone_reference(rgb, tone):
+    """the tone stage of B200ToneMap (include/b200av1.h) on the matrix's integer R, G, B ([3, ...], 0 .. 4 * bdmax):
+    float32 T on the same scale, exactly as the kernel computes it (numpy rounds each float32 operation on its own)"""
+    curve, m, oetf = (np.asarray(a, np.float32) for a in tone)
+    m = m.reshape(3, 3)
+    bits = (len(oetf) - 1).bit_length() - 1
+    L = curve[rgb]
+    G = [(m[r, 0] * L[0] + m[r, 1] * L[1]) + m[r, 2] * L[2] for r in range(3)]
+    return np.stack([oetf[np.rint(np.clip(g, np.float32(0), np.float32(1)) * np.float32(1 << bits)).astype(np.int64)] for g in G])
+
+
 def tensor_antialiased(w, h, size, antialias):
     """whether an export of a w x h picture to size = (OH, OW) takes the antialiased definition: antialias and a luma axis
     reduced (sigma > 256)"""
@@ -271,11 +392,12 @@ def tensor_antialiased(w, h, size, antialias):
 
 
 def tensor_reference(planes, bpc, layout, size=None, matrix="bt709", full_range=False, siting="left", mean=None, std=None,
-                     antialias=False, interpolation="bilinear"):
+                     antialias=False, interpolation="bilinear", tone=None):
     """numpy statement of the tensor export (include/b200av1.h B200TensorJob) for one picture's planes (layout = enum
     Dav1dPixelLayout): float32 [3, OH, OW] of R, G, B; size = (OH, OW), by default the picture's. antialias=True: the
     antialiased definition (triangle filter on reduced axes), which leaves exports without a reduced luma axis unchanged.
-    interpolation="bicubic": the bicubic definition instead, plain or (antialias=True) antialiased on every axis."""
+    interpolation="bicubic": the bicubic definition instead, plain or (antialias=True) antialiased on every axis.
+    tone=(curve, m, oetf), e.g. tone_tables(...): the HDR to SDR stage of B200ToneMap between the matrix and the output."""
     h, w = planes[0].shape
     oh, ow = size or (h, w)
     ssh, ssv = int(layout in (1, 2)), int(layout == 1)
@@ -314,7 +436,8 @@ def tensor_reference(planes, bpc, layout, size=None, matrix="bt709", full_range=
         cb, cr = (0, 0) if u is None else (u - (512 << s), v - (512 << s))
         rgb = np.clip(np.stack([(yy + rv * cr) >> 14, (yy - gu * cb - gv * cr) >> 14, (yy + bu * cb) >> 14]), 0, 4 * bdmax)
     scale, bias = tensor_scale_bias(bpc, mean, std)
-    return rgb.astype(np.float32) * scale[:, None, None] + bias[:, None, None]
+    t = rgb.astype(np.float32) if tone is None else tone_reference(rgb, tone)
+    return t * scale[:, None, None] + bias[:, None, None]
 
 
 def crop_planes(planes, layout, box):
@@ -388,11 +511,15 @@ class DeviceDecoder:
         d.b200hook_export_tensor.argtypes = [C.c_void_p, C.POINTER(TensorJob), C.c_void_p, C.c_void_p]
         d.b200hook_export_tensor_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         d.refdrv_stream_chroma_position.argtypes = [C.c_void_p]
+        d.refdrv_stream_color.argtypes = [C.c_void_p, C.c_void_p]
+        d.b200hook_export_tensor_tone_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        self._tones = {}                         # (transfer, primaries, bpc, peak, sdr_peak, device) -> (ToneMap, tables)
 
     def stats(self, reset=False):
         return self._hooked.stats(reset)
 
     def release(self):
+        self._drop_tones()
         self._hooked.release()
 
     def pictures(self, tus, format="planes", matrix="auto", full_range=None, alloc=None, stream=None):
@@ -413,7 +540,7 @@ class DeviceDecoder:
 
     def tensors(self, tus, size=None, dtype="float32", layout="chw", mean=None, std=None, matrix="auto", full_range=None,
                 chroma_siting="auto", batch=None, alloc=None, stream=None, antialias=False, crop=None, flip=False,
-                interpolation="bilinear"):
+                interpolation="bilinear", tonemap=None, peak=None, sdr_peak=SDR_PEAK):
         """Decodes the temporal units `tus` and yields every output picture as a model input: R, G, B resized to
         size = (height, width) (default: the picture's own) by bilinear sampling at half-sample centres, like
         torch.nn.functional.interpolate(mode="bilinear", align_corners=False) (chroma upsampling is part of the same
@@ -437,7 +564,13 @@ class DeviceDecoder:
         (torchvision's resized_crop; RandomResizedCrop with a random box). On a chroma-subsampled axis an odd top / left
         is rounded down and the box grown to keep its bottom / right edge (align_crop). size=None exports the box at that
         (aligned) size. flip: True, or a callable k -> bool, mirrors the output horizontally after resizing
-        (torchvision's hflip). ValueError, naming the picture, for a box outside the picture."""
+        (torchvision's hflip). ValueError, naming the picture, for a box outside the picture.
+        tonemap: None (the default) exports every stream as it is coded. "auto" tone-maps streams whose sequence header says
+        PQ (transfer_characteristics 16) or HLG (18) to SDR BT.709 (include/b200av1.h B200ToneMap; tone_tables states the
+        curves) and exports every other stream exactly as None does; "pq" or "hlg" force that transfer, for streams without
+        a colour description. peak: the source peak in cd/m^2, by default MaxCLL, else the mastering display's maximum
+        luminance, else 1000 (HLG: 1000); sdr_peak: the light that becomes SDR white (203 cd/m^2, BT.2408). The colour
+        primaries come from the header (unspecified: BT.2020). The tone map applies to the resized signal."""
         if dtype not in TENSOR_DTYPES or layout not in TENSOR_LAYOUTS:
             raise ValueError("dtype must be one of %s, layout 'chw' or 'hwc'" % ", ".join(TENSOR_DTYPES))
         if matrix != "auto" and matrix != "identity" and matrix not in MATRICES:
@@ -455,10 +588,12 @@ class DeviceDecoder:
         if not callable(flip) and not _is_flag(flip):
             raise ValueError("flip must be a bool or a callable")
         _check_interpolation(interpolation)
+        _check_tonemap(tonemap, peak, sdr_peak)
         tensor_scale_bias(8, mean, std)                          # checks mean / std
         alloc, stream = _default_alloc(alloc, stream)
         esize = 4 if dtype == "float32" else 2
         state = {"buf": None, "n": 0, "shape": None, "k": 0}
+        tone_kw = dict(tonemap=tonemap, peak=peak, sdr_peak=sdr_peak)
 
         def export(h, info):
             k = state["k"]
@@ -472,7 +607,7 @@ class DeviceDecoder:
             if batch is None:
                 out = alloc(shape, dtype)
                 self._export_tensor(h, info, _data_ptr(out), oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
-                                    antialias, stream, box, fl, interpolation)
+                                    antialias, stream, box, fl, interpolation, self._tone(h, info, out, **tone_kw))
                 return [out]
             done = []
             if state["buf"] is not None and state["shape"] != shape:       # another size closes the batch
@@ -482,7 +617,7 @@ class DeviceDecoder:
                 state.update(buf=alloc((int(batch),) + shape, dtype), n=0, shape=shape)
             dst = _data_ptr(state["buf"]) + state["n"] * 3 * oh * ow * esize
             self._export_tensor(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, antialias, stream,
-                                box, fl, interpolation)
+                                box, fl, interpolation, self._tone(h, info, state["buf"], **tone_kw))
             state["n"] += 1
             if state["n"] == batch:
                 done.append(state["buf"])
@@ -496,7 +631,7 @@ class DeviceDecoder:
 
     def clips(self, streams, frames, step=1, start=0, size=None, dtype="float32", layout="chw", mean=None, std=None,
               matrix="auto", full_range=None, chroma_siting="auto", workers=None, alloc=None, stream=None, antialias=False,
-              crop=None, flip=False, interpolation="bilinear"):
+              crop=None, flip=False, interpolation="bilinear", tonemap=None, peak=None, sdr_peak=SDR_PEAK):
         """Decodes N streams (each a list of temporal units) concurrently and returns one clip per stream as a
         [N, frames, 3, OH, OW] tensor (layout="hwc": [N, frames, OH, OW, 3]): x[i, t] is output picture
         start_i + t * step of stream i, exported exactly as tensors() exports it. `start` is one int or one per stream.
@@ -504,7 +639,9 @@ class DeviceDecoder:
         stream mean what they mean in tensors(); "auto" matrix, range and siting are resolved per stream from its own headers.
         crop: one box (top, left, height, width) for every stream, one box per stream, or a callable (i, height, width) -> box
         called once per stream i on its first sampled picture; flip: one bool, or one per stream. Every picture of a clip
-        takes its stream's box and flip (tensors() says what they do), so a clip stays consistent in time.
+        takes its stream's box and flip (tensors() says what they do), so a clip stays consistent in time. tonemap, peak and
+        sdr_peak: as in tensors(), resolved per stream from its own headers and metadata ("auto" converts the PQ and HLG
+        streams of a batch and exports the others as they are, in the same batched launches).
         Each stream has a dav1d context of its own (this decoder's n_threads / max_frame_delay) driven by a host thread of
         its own; at most `workers` streams are open at once (default min(N, CLIP_WORKERS), at most CLIP_MAX_WORKERS).
         Pictures that are not sampled are released unexported, and a stream is closed once its last sampled picture is
@@ -543,6 +680,7 @@ class DeviceDecoder:
         else:
             raise ValueError("flip must be a bool or one bool per stream")
         _check_interpolation(interpolation)
+        _check_tonemap(tonemap, peak, sdr_peak)
         tensor_scale_bias(8, mean, std)                          # checks mean / std
         alloc, stream = _default_alloc(alloc, stream)
         self._hooked._bind()
@@ -572,6 +710,7 @@ class DeviceDecoder:
                     jobs = (TensorJob * len(items))()
                     pics = (C.c_void_p * len(items))()
                     boxes = (C.c_int32 * (4 * len(items)))() if crop is not None else None
+                    tones = (C.POINTER(ToneMap) * len(items))()
                     for k, (i, t, h, info, _) in enumerate(items):
                         if callable(crops[i]):                  # the stream's box, from its first sampled picture
                             crops[i] = crops[i](i, int(info[1]), int(info[0]))
@@ -589,7 +728,11 @@ class DeviceDecoder:
                         jobs[k] = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
                                                    antialias, flips[i], interpolation)
                         pics[k] = self.dll.refdrv_stream_picture(h)
-                    if self.dll.b200hook_export_tensor_batch(pics, jobs, boxes, len(items), C.c_void_p(stream)) != 0:
+                        tm = self._tone(h, info, out, tonemap, peak, sdr_peak)
+                        if tm is not None:
+                            tones[k] = C.pointer(tm)
+                    if self.dll.b200hook_export_tensor_tone_batch(pics, jobs, boxes, tones if any(tones) else None, len(items),
+                                                                  C.c_void_p(stream)) != 0:
                         raise RuntimeError("exporting pictures failed (see stderr)")
                     left -= len(items)
                 finally:
@@ -691,12 +834,62 @@ class DeviceDecoder:
         return name
 
     def _export_tensor(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, stream, box,
-                       flip, interpolation):
+                       flip, interpolation, tone=None):
         job = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip,
                                interpolation)
         box = (C.c_int32 * 4)(*box) if box else None
-        if self.dll.b200hook_export_tensor(self.dll.refdrv_stream_picture(h), C.byref(job), box, C.c_void_p(stream)) != 0:
+        pic = self.dll.refdrv_stream_picture(h)
+        if tone is None:
+            rc = self.dll.b200hook_export_tensor(pic, C.byref(job), box, C.c_void_p(stream))
+        else:
+            rc = self.dll.b200hook_export_tensor_tone_batch((C.c_void_p * 1)(pic), C.byref(job), box,
+                                                            (C.POINTER(ToneMap) * 1)(C.pointer(tone)), 1, C.c_void_p(stream))
+        if rc != 0:
             raise RuntimeError("exporting a picture failed (see stderr)")
+
+    def color(self, h):
+        """the colour description and HDR metadata of the picture stream h holds: dict of primaries, transfer (codes of the
+        sequence header), max_cll, max_fall (cd/m^2) and mastering_max / mastering_min (cd/m^2), 0 where absent"""
+        out = np.zeros(6, np.int32)
+        if self.dll.refdrv_stream_color(h, out.ctypes.data) != 0:
+            raise RuntimeError("no picture is held")
+        pri, trc, cll, fall, mx, mn = (int(v) for v in out)
+        return dict(primaries=pri, transfer=trc, max_cll=cll, max_fall=fall, mastering_max=(mx & 0xffffffff) / 256.0,
+                    mastering_min=(mn & 0xffffffff) / 16384.0)
+
+    def _tone(self, h, info, out, tonemap, peak, sdr_peak):
+        """the B200ToneMap of the picture stream h holds, None when it is exported as it is coded. Its tables are built once
+        per (transfer, primaries, bit depth, peak, SDR peak) and kept by this decoder, until release(), on the device of
+        the destination `out` (host arrays for a host destination), so they outlive every launch that reads them."""
+        if tonemap is None:
+            return None
+        col = self.color(h)
+        transfer = {v: k for k, v in TRANSFERS.items()}.get(col["transfer"]) if tonemap == "auto" else tonemap
+        if transfer is None:
+            return None
+        if peak is None:
+            peak = (col["max_cll"] or col["mastering_max"] or HDR_PEAK) if transfer == "pq" else HDR_PEAK
+        bpc = int(info[2])
+        device = out.device if getattr(out, "is_cuda", False) else None
+        key = (transfer, col["primaries"], bpc, float(peak), float(sdr_peak), str(device))
+        if key not in self._tones:
+            curve, m, oetf = tone_tables(transfer, col["primaries"], bpc, peak, sdr_peak)
+            tables = [_on_device(curve, device), _on_device(oetf, device)]
+            tm = ToneMap()
+            tm.curve, tm.oetf = _data_ptr(tables[0]), _data_ptr(tables[1])
+            tm.curve_len, tm.oetf_bits = len(curve), (len(oetf) - 1).bit_length() - 1
+            for k in range(9):
+                tm.m[k] = float(m.ravel()[k])
+            self._tones[key] = (tm, tables)
+        return self._tones[key][0]
+
+    def _drop_tones(self):
+        """frees the tone tables once the launches that may still read them have completed"""
+        import sys
+        if "torch" in sys.modules:
+            for dev in {t.device for _, tables in self._tones.values() for t in tables if getattr(t, "is_cuda", False)}:
+                sys.modules["torch"].cuda.synchronize(dev)
+        self._tones.clear()
 
     def _tensor_job(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip,
                     interpolation="bilinear"):
@@ -764,6 +957,26 @@ def _default_alloc(alloc, stream):
         if stream is None:
             stream = torch.cuda.current_stream()
     return alloc, getattr(stream, "cuda_stream", stream) or 0
+
+
+def _check_tonemap(tonemap, peak, sdr_peak):
+    if tonemap is not None and tonemap != "auto" and tonemap not in TRANSFERS:
+        raise ValueError("tonemap must be None, 'auto', 'pq' or 'hlg', not %r" % (tonemap,))
+    for name, v in (("peak", peak), ("sdr_peak", sdr_peak)):
+        if v is not None and not (isinstance(v, (int, float, np.integer, np.floating)) and np.isfinite(v) and v > 0):
+            raise ValueError("%s must be a positive number of cd/m^2, not %r" % (name, v))
+    if sdr_peak is None:
+        raise ValueError("sdr_peak must be a positive number of cd/m^2")
+
+
+def _on_device(a, device):
+    """the numpy array a as a CUDA tensor on `device`, its copy complete when this returns, or a itself for device None"""
+    if device is None:
+        return a
+    import torch
+    t = torch.from_numpy(a).to(device)
+    torch.cuda.synchronize(device)
+    return t
 
 
 def _picture_box(box, info, who):

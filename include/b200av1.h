@@ -649,7 +649,7 @@ B200_API int b200_frame_run_batch(const B200FrameJob *const *jobs, int n_jobs, v
 /* sizeof() of the ABI structs as compiled into the library (binding self-check): 0 McFrame, 1 McBlock, 2 CompBlock,
  * 3 BlendBlock, 4 WarpBlock, 5 ItxBlock, 6 LfFrame, 7 CdefFrame, 8 LrFrame, 9 FrameJob, 10 Av1Filter, 11 Av1Restoration,
  * 12 FgFrame, 13 FilmGrainData, 14 IntraTx, 15 IntraFrame, 16 McScaledBlock, 17 CoefBlock, 18 IntraSb, 19 CompFusedBlock,
- * 20 FrameBand, 21 ResizeFrame, 22 ExportJob, 23 TensorJob */
+ * 20 FrameBand, 21 ResizeFrame, 22 ExportJob, 23 TensorJob, 24 ToneMap */
 B200_API int b200_struct_size(int which);
 
 /* ==== band-sliced frame job + cross-GPU reference exchange (SURVEY.md §8e) ===================== */
@@ -887,6 +887,49 @@ B200_API int b200_export_tensor(const B200TensorJob *job, void *stream);
  * is the n = 1 case. */
 #define B200_TENSOR_BATCH_MAX 24
 B200_API int b200_export_tensor_batch(const B200TensorJob *jobs, int n, void *stream);
+
+/* ==== HDR to SDR tone mapping in the tensor export ============================================ */
+/* An optional stage of the tensor export between the matrix and the output rule above, for PQ (SMPTE ST 2084) and HLG
+ * (ARIB STD-B67 / BT.2100) pictures that a model trained on SDR BT.709 input should see as SDR. R_c (0 .. 4 * bdmax, the
+ * matrix's result, identity and mono included) becomes a float T_c on the same scale:
+ *   Curve:  L_c = curve[R_c]                   float32, curve_len = 4 * bdmax + 1 entries, one table for all three channels,
+ *                                              values in [0, 1]: every per-channel 1-D step before the gamut change (EOTF,
+ *                                              tone curve, normalisation to the SDR peak)
+ *   Gamut:  G_r = clip(((m[3r] * L_0) + (m[3r + 1] * L_1)) + (m[3r + 2] * L_2), 0, 1)   per row r, each float32 multiply
+ *                                              and add rounded to nearest on its own (never fused), in that order
+ *   OETF:   T_c = oetf[rint(G_c * 2^B)]        B = oetf_bits, rint to nearest even (the product is exact); float32,
+ *                                              2^B + 1 entries of 4 * bdmax * OETF_709(i / 2^B)
+ *   Output: out = (T_c * scale[c]) + bias[c]   the rule above with T_c in place of R_c
+ * Given the tables the result is exact. The stage follows resampling like the matrix does: it tone-maps the resized
+ * signal, not the source samples. The tables are data: the library never builds them. The Python binding computes them
+ * in float64 and rounds them once to float32 (dav1d_b200/stream.py tone_tables):
+ *   PQ:  the ST 2084 EOTF (cd/m^2); the BT.2390 EETF on each of R', G', B' in the PQ domain from the source peak to the SDR
+ *        peak, black at 0 (Hermite knee from KS = 1.5 maxLum - 0.5; light above the source peak clips to it; no compression
+ *        when the SDR peak is at or above the source peak); divided by the SDR peak (203 cd/m^2 by default, BT.2408's HDR
+ *        reference white). The source peak is MaxCLL when present and non-zero, else the mastering display's maximum, else
+ *        1000 cd/m^2.
+ *   HLG: the BT.2100 inverse OETF (scene light E), display light Lw * E^gamma per channel with Lw = the peak (1000 cd/m^2)
+ *        and gamma = 1.2 + 0.42 log10(Lw / 1000), then the EETF and normalisation of PQ. The per-channel OOTF approximates
+ *        BT.2100's luminance-based one and is exact on neutral colours; HLG's 75 % reference white lands at about
+ *        203 cd/m^2, as BT.2408 expects.
+ *   m:   the linear-light RGB -> RGB matrix from the source primaries (BT.709, BT.2020, P3-D65) to BT.709, D65 white.
+ *   oetf: the BT.709 OETF (alpha = 1.09929682680944, beta = 0.018053968510807), B = 16. */
+typedef struct B200ToneMap {
+    const float *curve;            /* device, curve_len entries */
+    const float *oetf;             /* device, (1 << oetf_bits) + 1 entries */
+    int32_t curve_len;             /* 4 * bitdepth_max + 1 of the job */
+    int32_t oetf_bits;             /* B: 8 .. 16 */
+    float m[9];                    /* row major, finite */
+    int32_t pad;
+} B200ToneMap;
+/* b200_export_tensor_batch with an optional tone map per job: tones = NULL, or tones[i] = NULL, exports job i exactly as
+ * b200_export_tensor_batch does (that function is the tones = NULL case). Jobs with a tone map take launches of their own,
+ * grouped like the others, of at most B200_TENSOR_TONE_BATCH_MAX jobs (a job and its tone map ride in the parameter
+ * block). -2 with nothing launched for what b200_export_tensor_batch rejects and for a bad tone map: a NULL table, a
+ * curve_len other than 4 * bitdepth_max + 1, oetf_bits outside 8 .. 16 or a matrix entry that is not finite. Tables must
+ * stay valid until the launch has completed. */
+#define B200_TENSOR_TONE_BATCH_MAX 16
+B200_API int b200_export_tensor_tone_batch(const B200TensorJob *jobs, const B200ToneMap *const *tones, int n, void *stream);
 
 #ifdef __cplusplus
 }

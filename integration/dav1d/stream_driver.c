@@ -181,6 +181,22 @@ API int refdrv_stream_chroma_position(void *const hv)
     return h->held ? (int)h->pic.seq_hdr->chr : -1;
 }
 
+/* the colour description and HDR metadata of the held picture: out = color_primaries, transfer_characteristics (enum
+ * Dav1dColorPrimaries / Dav1dTransferCharacteristics), MaxCLL, MaxFALL (cd/m^2), the mastering display's max luminance
+ * (24.8 fixed point) and min luminance (18.14 fixed point), each 0 when absent; -1 when no picture is held */
+API int refdrv_stream_color(void *const hv, int32_t *const out)
+{
+    RefdrvStream *const h = hv;
+    if (!h->held) return -1;
+    const Dav1dPicture *const p = &h->pic;
+    const Dav1dContentLightLevel *const cl = p->content_light;
+    const Dav1dMasteringDisplay *const md = p->mastering_display;
+    out[0] = (int32_t)p->seq_hdr->pri; out[1] = (int32_t)p->seq_hdr->trc;
+    out[2] = cl ? cl->max_content_light_level : 0; out[3] = cl ? cl->max_frame_average_light_level : 0;
+    out[4] = md ? (int32_t)md->max_luminance : 0; out[5] = md ? (int32_t)md->min_luminance : 0;
+    return 0;
+}
+
 API void refdrv_stream_close(void *const hv)
 {
     RefdrvStream *const h = hv;

@@ -1,7 +1,7 @@
 """The tensor export (b200_export_tensor) against the torch chain it replaces (run on a GPU machine):
 
     python tools/bench_tensor_export.py [--launches 200] [--rounds 5] [--reps 3] [--antialias] [--crop-flip] [--kernel-only]
-                                        [--interpolation bilinear | bicubic] [--baseline-lib SO] [--out FILE]
+                                        [--interpolation bilinear | bicubic] [--tonemap] [--baseline-lib SO] [--out FILE]
 
 Kernel level, one JSON line per configuration, on synthetic device pictures (random planes, 4:2:0):
   fused        one b200_export_tensor launch
@@ -26,6 +26,10 @@ Decoder level, one JSON line per stream workload of bench.py: pictures per secon
 --interpolation bicubic: the kernel level only, on BICUBIC_CONFIGS (or CROP_FLIP_CONFIGS with --crop-flip), with
   B200TensorJob.interpolation = B200_TENSOR_BICUBIC (antialiased with --antialias or --crop-flip) against the chain with
   interpolate(mode="bicubic", ...).
+--tonemap: the kernel level only, on TONEMAP_CONFIGS: 10-bit BT.2020 PQ or HLG pictures tone-mapped to SDR BT.709
+  (b200_export_tensor_tone_batch, one job with the tables of stream.tone_tables) against the chain with the same
+  definition: the RGB export, .float(), the curve gather, the 3 x 3 matrix, clamp, the OETF gather, interpolate,
+  (x - mean) / std, .to(dtype).
 --baseline-lib SO: the kernel level times the same jobs (flip = 0) through another build of the library (an earlier
   commit's libb200av1.so) instead of the torch chain, alternated with this tree's, as `fused_baseline`.
 The GPU's name, power limit and SM clock are read in the same run."""
@@ -85,6 +89,25 @@ CROP_FLIP_CONFIGS = [  # AA_CONFIGS' fields, then the box (top, left, height, wi
 ]
 
 
+TONEMAP_CONFIGS = [  # AA_CONFIGS' fields, no box, then (transfer, antialias, interpolation)
+    ("pq 4k10 -> 224x224 bf16 chw, aa bilinear", 3840, 2160, 10, (224, 224), "bfloat16", "chw", 1, None, ("pq", 1, "bilinear")),
+    ("pq 4k10 -> 224x224 bf16 chw, aa bicubic", 3840, 2160, 10, (224, 224), "bfloat16", "chw", 1, None, ("pq", 1, "bicubic")),
+    ("pq 4k10 -> 1920x1080 fp16 chw, bilinear", 3840, 2160, 10, (1080, 1920), "float16", "chw", 1, None, ("pq", 0, "bilinear")),
+    ("hlg 1080p10 -> 224x224 bf16 chw, aa bilinear", 1920, 1080, 10, (224, 224), "bfloat16", "chw", 1, None, ("hlg", 1, "bilinear")),
+]
+
+
+def tone_chain(rgb, bdmax, tables, size, dtype, mean, std, antialias, mode):
+    """the tone-mapped export in torch: R, G, B at the stream's bit depth -> curve -> matrix -> clamp -> OETF -> resize"""
+    curve, m, oetf = tables
+    L = curve[rgb.long() * 4]                        # R on the 0 .. 4 * bdmax scale of the curve
+    G = torch.einsum("rc,chw->rhw", m, L).clamp_(0, 1)
+    x = oetf[torch.round(G * 65536).long()] / (4 * bdmax)
+    if size is not None:
+        x = F.interpolate(x[None], size=size, mode=mode, align_corners=False, antialias=antialias)[0]
+    return ((x - mean) / std).to(getattr(torch, dtype))
+
+
 def torch_chain(rgb, bdmax, size, dtype, layout, mean, std, antialias=False, flip=False, mode="bilinear"):
     x = rgb.float() / bdmax
     if size is not None:
@@ -94,7 +117,7 @@ def torch_chain(rgb, bdmax, size, dtype, layout, mean, std, antialias=False, fli
     return x.permute(1, 2, 0).contiguous() if layout == "hwc" else x
 
 
-def chain_bytes(w, h, sb, size, dtype, layout, box=None):
+def chain_bytes(w, h, sb, size, dtype, layout, box=None, tone=False):
     """algorithmic bytes of the torch chain: each step reads its input and writes its output once"""
     px, (oh, ow) = w * h, size or (h, w)
     op = oh * ow
@@ -103,6 +126,8 @@ def chain_bytes(w, h, sb, size, dtype, layout, box=None):
         px = box[2] * box[3]
         b += 2 * 3 * op * 4                          # .flip(-1)
     b += 3 * px * sb + 3 * px * 4 + 2 * 3 * px * 4   # .float(), / bdmax
+    if tone:                                         # int64 curve index, gather, matrix, clamp, OETF index, gather
+        b += 3 * px * (sb + 8) + 3 * px * (8 + 4) + 3 * px * (4 + 4) + 2 * 3 * px * 4 + 3 * px * (4 + 8) + 3 * px * (8 + 4)
     if size is not None:
         b += 3 * px * 4 + 3 * op * 4                 # interpolate
     b += 2 * (2 * 3 * op * 4)                        # - mean, / std
@@ -133,12 +158,14 @@ def kernel_level(args):
     s = torch.cuda.Stream()
     lines = []
     bicubic = args.interpolation == "bicubic"
-    configs = CROP_FLIP_CONFIGS if args.crop_flip else BICUBIC_CONFIGS if bicubic else AA_CONFIGS if args.antialias else \
-        [c + (1,) for c in CONFIGS] + [BATCH_CONFIG]
+    configs = TONEMAP_CONFIGS if args.tonemap else CROP_FLIP_CONFIGS if args.crop_flip else BICUBIC_CONFIGS if bicubic else \
+        AA_CONFIGS if args.antialias else [c + (1,) for c in CONFIGS] + [BATCH_CONFIG]
     base = baseline_lib(args.baseline_lib) if args.baseline_lib else None
-    for name, w, h, bpc, size, dtype, layout, pics, *box in configs:
-        box = box[0] if box else None
-        antialias = args.antialias or box is not None
+    for name, w, h, bpc, size, dtype, layout, pics, *extra in configs:
+        box = extra[0] if extra else None
+        tone = extra[1] if len(extra) > 1 else None
+        antialias = tone[1] if tone else args.antialias or box is not None
+        interpolation = tone[2] if tone else args.interpolation
         rng = np.random.default_rng(w + bpc)
         bdmax, sb = (1 << bpc) - 1, 1 if bpc == 8 else 2
         planes = [rng.integers(0, bdmax + 1, (ph, pw)).astype(np.uint8 if bpc == 8 else np.int16) for pw, ph in stream.plane_dims(w, h, 1)]
@@ -154,13 +181,21 @@ def kernel_level(args):
         tj.w, tj.h, tj.ss_hor, tj.ss_ver, tj.bitdepth_max = w, h, 1, 1, bdmax
         tj.out_w, tj.out_h = ow, oh
         tj.dtype, tj.layout, tj.siting_x, tj.siting_y = stream.TENSOR_DTYPES[dtype], stream.TENSOR_LAYOUTS[layout], 0, 1
-        tj.cy, tj.rv, tj.gu, tj.gv, tj.bu = stream.rgb_coefficients("bt709", False)
+        tj.cy, tj.rv, tj.gu, tj.gv, tj.bu = stream.rgb_coefficients("bt2020" if tone else "bt709", False)
         scale, bias = stream.tensor_scale_bias(bpc, MEAN, STD)
         for c in range(3):
             tj.scale[c], tj.bias[c] = float(scale[c]), float(bias[c])
         tj.dst, tj.pitch_c, tj.pitch_y = out.data_ptr(), (oh * ow if layout == "chw" else 1), (ow if layout == "chw" else 3 * ow)
         tj.antialias = int(antialias)
-        tj.interpolation = stream.TENSOR_INTERPOLATIONS[args.interpolation]
+        tj.interpolation = stream.TENSOR_INTERPOLATIONS[interpolation]
+        if tone:                                 # BT.2020 primaries, source peak 1000 cd/m^2, SDR white at 203
+            tables = stream.tone_tables(tone[0], 9, bpc)
+            d_tables = [torch.from_numpy(t).cuda() for t in tables]
+            tm = stream.ToneMap()
+            tm.curve, tm.oetf, tm.curve_len, tm.oetf_bits = d_tables[0].data_ptr(), d_tables[2].data_ptr(), len(tables[0]), 16
+            for k in range(9):
+                tm.m[k] = float(tables[1].ravel()[k])
+            tones = (C.POINTER(stream.ToneMap) * 1)(C.pointer(tm))
         if box is not None:                      # the box is the source; the output is mirrored
             top, left, tj.h, tj.w = box
             tj.plane_off[0] += top * tj.stride[0] + left
@@ -186,7 +221,9 @@ def kernel_level(args):
         sp = C.c_void_p(s.cuda_stream)
 
         def fused():
-            if pics > 1:
+            if tone:
+                lib.check(lib.b200_export_tensor_tone_batch(C.byref(tj), tones, 1, sp), "b200_export_tensor_tone_batch")
+            elif pics > 1:
                 lib.check(lib.b200_export_tensor_batch(tjs, pics, sp), "b200_export_tensor_batch")
             else:
                 lib.check(lib.b200_export_tensor(C.byref(tj), sp), "b200_export_tensor")
@@ -195,7 +232,10 @@ def kernel_level(args):
             for _ in range(pics):
                 lib.check(lib.b200_export_picture(C.byref(ej), sp), "b200_export_picture")
                 x = rgb if box is None else rgb[:, box[0]:box[0] + box[2], box[1]:box[1] + box[3]]
-                torch_chain(x, bdmax, size, dtype, layout, mean, std, antialias, box is not None, args.interpolation)
+                if tone:
+                    tone_chain(x, bdmax, d_tables, size, dtype, mean, std, antialias, interpolation)
+                else:
+                    torch_chain(x, bdmax, size, dtype, layout, mean, std, antialias, box is not None, interpolation)
 
         arms = {"fused": fused}
         if base is not None:                     # the same jobs in the other build's struct layout
@@ -230,13 +270,15 @@ def kernel_level(args):
         sw, sh = (box[3], box[2]) if box else (w, h)
         fused_bytes = pics * (sw * sh * 3 // 2 * sb + 3 * oh * ow * ESIZE[dtype])
         line = {"config": name, "gpu": gpu_info(), "launches_per_round": args.launches, "rounds": args.rounds, "us": {}, "bytes": {
-            "fused": fused_bytes, "fused_baseline": fused_bytes, "torch_chain": pics * chain_bytes(w, h, sb, size, dtype, layout, box)},
+            "fused": fused_bytes, "fused_baseline": fused_bytes, "torch_chain": pics * chain_bytes(w, h, sb, size, dtype, layout, box, bool(tone))},
             "GBps": {}, "share_of_3.35TBps": {}}
         line["bytes"] = {k: v for k, v in line["bytes"].items() if k in times}
         if antialias:
             line["antialias"] = True
-        if bicubic:
+        if interpolation == "bicubic":
             line["interpolation"] = "bicubic"
+        if tone:
+            line["tonemap"] = {"transfer": tone[0], "primaries": "bt2020", "peak": 1000.0, "sdr_peak": 203.0}
         if box is not None:
             line["crop_box"], line["flip"] = list(box), True
         if base is not None:
@@ -313,14 +355,15 @@ def main():
     ap.add_argument("--antialias", action="store_true")
     ap.add_argument("--crop-flip", action="store_true")
     ap.add_argument("--interpolation", choices=list(stream.TENSOR_INTERPOLATIONS), default="bilinear")
+    ap.add_argument("--tonemap", action="store_true")
     ap.add_argument("--baseline-lib", help="another build of libb200av1.so: time its export of the same jobs instead of the chain")
     ap.add_argument("--kernel-only", action="store_true")
     ap.add_argument("--out")
     args = ap.parse_args()
-    if args.baseline_lib and args.interpolation != "bilinear":
+    if args.baseline_lib and (args.interpolation != "bilinear" or args.tonemap):
         ap.error("--baseline-lib compares the bilinear and triangle exports, which an earlier library also has")
     assert torch.cuda.is_available(), "needs a CUDA device"
-    kernel_only = args.antialias or args.crop_flip or args.kernel_only or args.interpolation != "bilinear"
+    kernel_only = args.antialias or args.crop_flip or args.tonemap or args.kernel_only or args.interpolation != "bilinear"
     lines = kernel_level(args) + ([] if kernel_only else decoder_level(args))
     if args.out:
         with open(args.out, "w") as fh:
