@@ -304,6 +304,7 @@ _SIGS = {
     "b200_export_tensor": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_export_tensor_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "b200_export_tensor_tone_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "b200_export_tensor_jitter_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     # ---- ipred
     "b200_ipred_batch": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "b200_ipred": (C.c_int, [C.c_int, C.c_void_p, C.c_ssize_t, C.c_void_p] + [C.c_int] * 6),
@@ -396,6 +397,14 @@ class ToneMap(C.Structure):
                 ("m", C.c_float * 9), ("pad", C.c_int32)]
 
 
+class ColorJitter(C.Structure):
+    """B200ColorJitter: the colour jitter / grayscale stage of a tensor export (factors, order, and the device scratch of
+    the contrast mean)"""
+    _fields_ = [("brightness", C.c_float), ("contrast", C.c_float), ("saturation", C.c_float), ("hue", C.c_float),
+                ("contrast1", C.c_float), ("saturation1", C.c_float), ("order", C.c_int32 * 4), ("enabled", C.c_int32),
+                ("grayscale", C.c_int32), ("acc", C.c_void_p)]
+
+
 ABI_STRUCTS = [McFrame, McBlock, CompBlock, BlendBlock, WarpBlock, ItxBlock, LfFrame, CdefFrame, LrFrame, FrameJob,
                Av1Filter, Av1Restoration, FgFrame, FilmGrainData, IntraTx, IntraFrame, McScaledBlock, CoefBlock, IntraSb, CompFusedBlock, FrameBand, ResizeFrame,
-               ExportJob, TensorJob, ToneMap]
+               ExportJob, TensorJob, ToneMap, ColorJitter]

@@ -19,11 +19,16 @@
 #else
 // Host build of these sources (tests/emu): the rounding intrinsics of the tensor export with the same results. Each fp32
 // operation is rounded on its own (the volatile store keeps the compiler from contracting a multiply and an add into an
-// FMA), and g++'s _Float16 / __bf16 conversions round to nearest even like __float2half_rn / __float2bfloat16_rn.
+// FMA), and g++'s _Float16 / __bf16 conversions round to nearest even like __float2half_rn / __float2bfloat16_rn. The
+// library is built with --use_fast_math, whose -ftz=true makes a subnormal operand or result of these operations a zero
+// of the same sign on the GPU: emu_ftz does the same here.
 typedef _Float16 __half;
 typedef __bf16 __nv_bfloat16;
-static inline float __fmul_rn(float a, float b) { volatile float r = a * b; return r; }
-static inline float __fadd_rn(float a, float b) { volatile float r = a + b; return r; }
+static inline float emu_ftz(float v) { return std::fabs(v) < 1.17549435e-38f ? std::copysign(0.0f, v) : v; }
+static inline float __fmul_rn(float a, float b) { volatile float r = emu_ftz(a) * emu_ftz(b); return emu_ftz(r); }
+static inline float __fadd_rn(float a, float b) { volatile float r = emu_ftz(a) + emu_ftz(b); return emu_ftz(r); }
+static inline float __fsub_rn(float a, float b) { volatile float r = emu_ftz(a) - emu_ftz(b); return emu_ftz(r); }
+static inline float __fdiv_rn(float a, float b) { volatile float r = emu_ftz(a) / emu_ftz(b); return emu_ftz(r); }
 static inline __half __float2half_rn(float v) { return (__half)v; }
 static inline __nv_bfloat16 __float2bfloat16_rn(float v) { return (__nv_bfloat16)v; }
 static inline unsigned short __half_as_ushort(__half h) { unsigned short u; memcpy(&u, &h, 2); return u; }
@@ -238,13 +243,94 @@ B200_DEV void tone_map(const B200ToneMap &t, const int (&rgb)[3], float (&T)[3])
     }
 }
 
+// ---- colour jitter (B200ColorJitter, include/b200av1.h): torchvision's float32 operations, each rounded on its own ----
+enum { kJitBrightness = 0, kJitContrast = 1, kJitSaturation = 2, kJitHue = 3 };
+B200_DEV float unit_clip(float v) { return fminf(fmaxf(v, 0.0f), 1.0f); }
+B200_DEV float jitter_gray(const float (&x)[3])
+{
+    return __fadd_rn(__fadd_rn(__fmul_rn(0.2989f, x[0]), __fmul_rn(0.587f, x[1])), __fmul_rn(0.114f, x[2]));
+}
+// clip(a * x_c + a1 * g) per channel: torchvision's _blend
+B200_DEV void jitter_blend(float (&x)[3], float a, float a1, float g)
+{
+#pragma unroll
+    for (int c = 0; c < 3; c++) x[c] = unit_clip(__fadd_rn(__fmul_rn(a, x[c]), __fmul_rn(a1, g)));
+}
+// _rgb2hsv, h = remainder(h + hue, 1), _hsv2rgb
+B200_DEV void jitter_hue(float (&x)[3], float hue)
+{
+    const float r = x[0], g = x[1], b = x[2];
+    const float maxc = fmaxf(fmaxf(r, g), b), minc = fminf(fminf(r, g), b);
+    const bool eqc = maxc == minc;
+    const float cr = __fsub_rn(maxc, minc), d = eqc ? 1.0f : cr;
+    const float s = __fdiv_rn(cr, eqc ? 1.0f : maxc);
+    const float rc = __fdiv_rn(__fsub_rn(maxc, r), d), gc = __fdiv_rn(__fsub_rn(maxc, g), d), bc = __fdiv_rn(__fsub_rn(maxc, b), d);
+    float h = maxc == r ? __fsub_rn(bc, gc) : maxc == g ? __fsub_rn(__fadd_rn(2.0f, rc), bc) : __fsub_rn(__fadd_rn(4.0f, gc), rc);
+    h = __fadd_rn(__fdiv_rn(h, 6.0f), 1.0f);           // in [5/6, 11/6]: fmod(h, 1) is exact
+    if (h >= 1.0f) h = __fsub_rn(h, 1.0f);
+    h = __fadd_rn(h, hue);                             // in [-1/2, 3/2]: torch.remainder(h, 1)
+    if (h >= 1.0f) h = __fsub_rn(h, 1.0f);
+    if (h < 0.0f) h = __fadd_rn(h, 1.0f);
+    const float h6 = __fmul_rn(h, 6.0f), fi = floorf(h6), f = __fsub_rn(h6, fi);
+    const float p = unit_clip(__fmul_rn(maxc, __fsub_rn(1.0f, s)));
+    const float q = unit_clip(__fmul_rn(maxc, __fsub_rn(1.0f, __fmul_rn(s, f))));
+    const float t = unit_clip(__fmul_rn(maxc, __fsub_rn(1.0f, __fmul_rn(s, __fsub_rn(1.0f, f)))));
+    switch ((int)fi % 6) {
+    case 0: x[0] = maxc; x[1] = t; x[2] = p; break;
+    case 1: x[0] = q; x[1] = maxc; x[2] = p; break;
+    case 2: x[0] = p; x[1] = maxc; x[2] = t; break;
+    case 3: x[0] = p; x[1] = q; x[2] = maxc; break;
+    case 4: x[0] = t; x[1] = p; x[2] = maxc; break;
+    default: x[0] = maxc; x[1] = p; x[2] = q; break;
+    }
+}
+// the enabled operations in t.order on x (in [0, 1]); PRE: only those before contrast, whose gray the contrast pass sums.
+// m = the contrast mean M
+template <bool PRE>
+B200_DEV void color_jitter(const B200ColorJitter &t, float m, float (&x)[3])
+{
+#pragma unroll 1
+    for (int k = 0; k < 4; k++) {
+        const int op = t.order[k];
+        if (!((t.enabled >> op) & 1)) continue;
+        if (op == kJitContrast) {
+            if (PRE) return;
+            jitter_blend(x, t.contrast, t.contrast1, m);
+        } else if (op == kJitBrightness) {
+#pragma unroll
+            for (int c = 0; c < 3; c++) x[c] = unit_clip(__fmul_rn(t.brightness, x[c]));
+        } else if (op == kJitSaturation) {
+            jitter_blend(x, t.saturation, t.saturation1, jitter_gray(x));
+        } else {
+            jitter_hue(x, t.hue);
+        }
+    }
+    if (!PRE && t.grayscale) x[0] = x[1] = x[2] = jitter_gray(x);
+}
+// M of a jittered job from the contrast pass's sum S at t.acc: f32(f64(S) / (f64(OW * OH) * 2^24))
+B200_DEV float contrast_mean(const B200ColorJitter &t, const B200TensorJob &j)
+{
+    if (!((t.enabled >> kJitContrast) & 1)) return 0.0f;
+    return (float)((double)*t.acc / ((double)j.out_w * (double)j.out_h * 16777216.0));
+}
+
+// The epilogues of the tensor kernels (kernel template parameter EPI): plain, tone-mapped (B200ToneMap), colour-jittered
+// (B200ColorJitter, the tone map a runtime branch: tone.curve NULL is none) and the contrast pass of jittered jobs, which
+// stores nothing and adds rint(gray * 2^24) of each output pixel before contrast into its thread's sum
+enum { kEpiPlain = 0, kEpiTone = 1, kEpiJitter = 2, kEpiContrast = 3 };
+// what the jittered epilogues take besides the job: the jitter t, the contrast mean M, unit = f32(1 / (4 * bdmax)) (both
+// worked out once per thread) and, in the contrast pass, the thread's sum: at most 16 pixels (export_tensor_kernel's 4 x 4;
+// the tile kernel's epilogue gives a thread one run of 4) of at most 2^24 each, so 32 bits hold it
+struct JitterArgs { const B200ColorJitter *t; float mean, unit; uint32_t *sum; };
+
 // The epilogue of both tensor kernels: Q of a run of n (<= 4) output pixels at (x, y), per plane, through the matrix, the
-// clip, (TONE: the tone map tm) scale / bias and rounding into the destination (yoff, coff, qmax as include/b200av1.h
-// defines them for the job); MIRROR = j.flip and TONE, parameters of the kernels: jobs with and without a flip or a tone
-// map take kernels of their own
-template <int DT, bool HWC, bool MIRROR, bool TONE>
+// clip, (kEpiTone: the tone map tm; kEpiJitter: tm when it has a curve, then the jitter ja.t with contrast mean ja.mean) scale /
+// bias and rounding into the destination (yoff, coff, qmax as include/b200av1.h defines them for the job); MIRROR =
+// j.flip and EPI, parameters of the kernels: jobs with and without a flip, tone map or jitter take kernels of their own.
+// kEpiContrast adds to *ja.sum instead of storing.
+template <int DT, bool HWC, bool MIRROR, int EPI>
 B200_DEV void tensor_store(const B200TensorJob &j, const B200ToneMap *tm, int x, int y, int n, const int (&qy)[4], const int (&qu)[4],
-                           const int (&qv)[4], int yoff, int coff, int qmax)
+                           const int (&qv)[4], int yoff, int coff, int qmax, const JitterArgs &ja = {})
 {
     typedef typename TensorElem<DT>::type E;
     E o[3][4];
@@ -259,7 +345,25 @@ B200_DEV void tensor_store(const B200TensorJob &j, const B200ToneMap *tm, int x,
             rgb[1] = iclip((yy - j.gu * cb - j.gv * cr) >> 14, 0, qmax);
             rgb[2] = iclip((yy + j.bu * cb) >> 14, 0, qmax);
         }
-        if constexpr (TONE) {
+        if constexpr (EPI >= kEpiJitter) {
+            float J[3];
+            if (tm->curve) {
+                tone_map(*tm, rgb, J);
+#pragma unroll
+                for (int c = 0; c < 3; c++) J[c] = __fmul_rn(J[c], ja.unit);
+            } else {
+#pragma unroll
+                for (int c = 0; c < 3; c++) J[c] = __fmul_rn((float)rgb[c], ja.unit);
+            }
+            if constexpr (EPI == kEpiContrast) {
+                color_jitter<true>(*ja.t, 0.0f, J);
+                if (i < n) *ja.sum += (uint32_t)__float2int_rn(__fmul_rn(jitter_gray(J), 16777216.0f));
+            } else {
+                color_jitter<false>(*ja.t, ja.mean, J);
+#pragma unroll
+                for (int c = 0; c < 3; c++) o[c][i] = tensor_value<DT>(J[c], j.scale[c], j.bias[c]);
+            }
+        } else if constexpr (EPI == kEpiTone) {
             float T[3];
             tone_map(*tm, rgb, T);
 #pragma unroll
@@ -269,39 +373,90 @@ B200_DEV void tensor_store(const B200TensorJob &j, const B200ToneMap *tm, int x,
             for (int c = 0; c < 3; c++) o[c][i] = tensor_value<DT>(rgb[c], j.scale[c], j.bias[c]);
         }
     }
-    E *const row = (E *)j.dst + y * j.pitch_y;
-    store_pixels<MIRROR, HWC>(j, row, x, n, o);
+    if constexpr (EPI != kEpiContrast) {
+        E *const row = (E *)j.dst + y * j.pitch_y;
+        store_pixels<MIRROR, HWC>(j, row, x, n, o);
+    }
 }
 
 // The jobs of one launch travel in the kernel's parameter block (no staging copy): B200_TENSOR_BATCH_MAX of them fit the
 // classic 4 KB limit. A one-job launch takes the N = 1 form: its job's fields are then read at fixed parameter offsets, as
 // operands of the instructions that use them; indexed by blockIdx.z they are separate loads, which made the prologue of a
-// small one-picture export up to a quarter slower. Tone-mapped jobs (TONE) carry their B200ToneMap beside them, and
-// always take the batched form.
-template <int N, bool TONE> struct TensorBatch { B200TensorJob job[N]; };
-template <int N> struct TensorBatch<N, true> { B200TensorJob job[N]; B200ToneMap tone[N]; };
-static_assert(sizeof(TensorBatch<B200_TENSOR_BATCH_MAX, false>) <= 4096, "the jobs of one launch must fit a 4 KB kernel parameter block");
-static_assert(sizeof(TensorBatch<B200_TENSOR_TONE_BATCH_MAX, true>) <= 4096,
+// small one-picture export up to a quarter slower. Tone-mapped jobs (kEpiTone) carry their B200ToneMap beside them, and
+// jittered ones (kEpiJitter, and their contrast pass) a tone map (curve NULL: none) and their B200ColorJitter; both always
+// take the batched form.
+template <int N, int B> struct TensorBatch { B200TensorJob job[N]; };
+template <int N> struct TensorBatch<N, kEpiTone> { B200TensorJob job[N]; B200ToneMap tone[N]; };
+template <int N> struct TensorBatch<N, kEpiJitter> { B200TensorJob job[N]; B200ToneMap tone[N]; B200ColorJitter jit[N]; };
+// the batch an epilogue's kernels take: the contrast pass reads the jittered jobs' own
+constexpr int batch_of(int epi) { return epi == kEpiContrast ? kEpiJitter : epi; }
+static_assert(sizeof(TensorBatch<B200_TENSOR_BATCH_MAX, kEpiPlain>) <= 4096, "the jobs of one launch must fit a 4 KB kernel parameter block");
+static_assert(sizeof(TensorBatch<B200_TENSOR_TONE_BATCH_MAX, kEpiTone>) <= 4096,
               "the tone-mapped jobs of one launch must fit a 4 KB kernel parameter block");
-template <int N, bool TONE>
-B200_DEV const B200ToneMap *tone_of(const TensorBatch<N, TONE> &b)
+static_assert(sizeof(TensorBatch<B200_TENSOR_JITTER_BATCH_MAX, kEpiJitter>) + sizeof(int) <= 4096,
+              "the jittered jobs of one launch must fit a 4 KB kernel parameter block");
+template <int N, int B>
+B200_DEV const B200ToneMap *tone_of(const TensorBatch<N, B> &b)
 {
-    if constexpr (TONE) return &b.tone[N == 1 ? 0 : blockIdx.z];
+    if constexpr (B != kEpiPlain) return &b.tone[N == 1 ? 0 : blockIdx.z];
     else return nullptr;
+}
+template <int N, int B>
+B200_DEV const B200ColorJitter *jitter_of(const TensorBatch<N, B> &b)
+{
+    if constexpr (B == kEpiJitter) return &b.jit[blockIdx.z];
+    else return nullptr;
+}
+// __launch_bounds__'s minimum of resident CTAs per SM: 0 (none) for every form but the contrast pass, where 2 keeps
+// ptxas from choosing a register budget that spills (64 registers and a 48-byte stack frame in the 10/12-bit cubic one)
+template <int EPI> constexpr int kMinBlocks = EPI == kEpiContrast ? 2 : 0;
+// the JitterArgs of the epilogue EPI for job j of b (the contrast pass reads no M: it is summing it)
+template <int EPI, int N, int B>
+B200_DEV JitterArgs jitter_args(const TensorBatch<N, B> &b, const B200TensorJob &j, uint32_t *sum)
+{
+    if constexpr (EPI == kEpiJitter || EPI == kEpiContrast) {
+        const B200ColorJitter &t = *jitter_of(b);
+        return {&t, EPI == kEpiJitter ? contrast_mean(t, j) : 0.0f, __fdiv_rn(1.0f, (float)(4 * j.bitdepth_max)), sum};
+    } else {
+        return {nullptr, 0.0f, 0.0f, sum};
+    }
+}
+
+// The contrast pass's end: the sums of a warp's threads added into the job's S with one 64-bit integer atomic add, so
+// that S does not depend on the order of the adds. Every thread of the warp calls it, at the kernel's end
+B200_DEV void contrast_add(const B200ColorJitter &t, uint64_t sum)
+{
+    for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if (threadIdx.x == 0 && sum) atomicAdd((unsigned long long *)t.acc, (unsigned long long)sum);
+}
+
+// grid (1), block (32): zeroes S of the n jittered jobs with contrast, before their contrast pass
+template <int N>
+__global__ void __launch_bounds__(32) contrast_zero_kernel(const __grid_constant__ TensorBatch<N, kEpiJitter> b, int n)
+{
+    B200_PDL_ENTRY();
+    const int i = threadIdx.x;
+    if (i < n && ((b.jit[i].enabled >> kJitContrast) & 1)) *b.jit[i].acc = 0;
 }
 
 // grid (runs of 4 output columns / 32, output rows / (8 * kTensorRows), jobs), block (32, 8): x / y cover the largest
 // output of the launch, z selects the job. A thread converts its run of 4 columns on kTensorRows rows 8 apart, so the
 // column taps are worked out once for all of them
 constexpr int kTensorRows = 4;
-template <bool HBD, int DT, bool HWC, int N, bool MIRROR, bool TONE>
-__global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constant__ TensorBatch<N, TONE> b)
+template <bool HBD, int DT, bool HWC, int N, bool MIRROR, int EPI>
+__global__ void __launch_bounds__(256, kMinBlocks<EPI>) export_tensor_kernel(const __grid_constant__ TensorBatch<N, batch_of(EPI)> b)
 {
     B200_PDL_ENTRY();
     typedef typename Bd<HBD>::pixel pixel;
     const B200TensorJob &j = b.job[N == 1 ? 0 : blockIdx.z];
+    if constexpr (EPI == kEpiContrast)
+        if (!((jitter_of(b)->enabled >> kJitContrast) & 1)) return;
+    uint32_t sum = 0;
+    const JitterArgs ja = jitter_args<EPI>(b, j, &sum);
     const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 4, y0 = blockIdx.y * 8 * kTensorRows + threadIdx.y;
-    if (x >= j.out_w || y0 >= j.out_h) return;
+    // the contrast pass keeps every lane to its one contrast_add at the end: a lane outside the output skips the rows
+    if (x >= j.out_w || y0 >= j.out_h)
+        if constexpr (EPI != kEpiContrast) return;
     const int n = imin(4, j.out_w - x);
     const int cw = (j.w + j.ss_hor) >> j.ss_hor, ch = (j.h + j.ss_ver) >> j.ss_ver;
     const int kx = j.ss_hor ? j.siting_x : 0, ky = j.ss_ver ? j.siting_y : 0;
@@ -315,14 +470,17 @@ __global__ void __launch_bounds__(256) export_tensor_kernel(const __grid_constan
     for (int k = 0; k < kTensorRows; k++, lrow.next(), crow.next()) {
         const int y = y0 + 8 * k;
         if (y >= j.out_h) break;
+        if constexpr (EPI == kEpiContrast)
+            if (x >= j.out_w) break;
         int qy[4], qu[4] = {}, qv[4] = {};
         run_samples(qy, src + j.plane_off[0], j.stride[0], lrow, j.h, lt);
         if (!j.mono) {
             run_samples(qu, src + j.plane_off[1], j.stride[1], crow, ch, ct);
             run_samples(qv, src + j.plane_off[2], j.stride[2], crow, ch, ct);
         }
-        tensor_store<DT, HWC, MIRROR, TONE>(j, tone_of(b), x, y, n, qy, qu, qv, yoff, coff, qmax);
+        tensor_store<DT, HWC, MIRROR, EPI>(j, tone_of(b), x, y, n, qy, qu, qv, yoff, coff, qmax, ja);
     }
+    if constexpr (EPI == kEpiContrast) contrast_add(*jitter_of(b), sum);
 }
 
 // ---- antialiased reduction (B200TensorJob.antialias = 1, include/b200av1.h) ----
@@ -470,8 +628,8 @@ B200_DEV auto filter_axis(const B200TensorJob &j, int x, int in, int out, int n,
 // in the weight fills alone. The antialiased cubic weights are cumulative sums: a warp owns a column (or an output row)
 // and scans its taps 32 at a time, carrying C_j and R_j in shared memory across tap windows (row chunks).
 constexpr int kAaCols = 32, kAaRowsMax = 32, kAaChunk = 32, kAaTaps = 64;
-template <bool HBD, int DT, bool HWC, int N, bool MIRROR, int F, bool TONE>
-__global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_constant__ TensorBatch<N, TONE> b, int th)
+template <bool HBD, int DT, bool HWC, int N, bool MIRROR, int F, int EPI>
+__global__ void __launch_bounds__(256, kMinBlocks<EPI>) export_tensor_aa_kernel(const __grid_constant__ TensorBatch<N, batch_of(EPI)> b, int th)
 {
     B200_PDL_ENTRY();
     typedef typename Bd<HBD>::pixel pixel;
@@ -481,8 +639,10 @@ __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_cons
     __shared__ int qs[3][kAaRowsMax][kAaCols];       // Q of the tile
     __shared__ int cjlo[kAaCols], cnt[kAaCols];
     const B200TensorJob &j = b.job[N == 1 ? 0 : blockIdx.z];
+    if constexpr (EPI == kEpiContrast)
+        if (!((jitter_of(b)->enabled >> kJitContrast) & 1)) return;
     const int x0 = blockIdx.x * kAaCols, y0 = blockIdx.y * th;
-    if (x0 >= j.out_w || y0 >= j.out_h) return;
+    if (x0 >= j.out_w || y0 >= j.out_h) return;        // the whole CTA
     const int lane = threadIdx.x, warp = threadIdx.y, tid = warp * 32 + lane;
     const int rows = imin(th, j.out_h - y0);
     for (int p = 0; p < (j.mono ? 1 : 3); p++) {
@@ -606,7 +766,9 @@ __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_cons
     __syncthreads();
     const int bdmax = j.bitdepth_max, s = bdmax == 4095 ? 4 : bdmax == 1023 ? 2 : 0;
     const int yoff = j.full_range ? 0 : 64 << s, coff = 512 << s;
-    // the epilogue: a thread per run of 4 columns of one row
+    // the epilogue: a thread per run of 4 columns of one row (the jitter's arguments taken here, not held through the loops)
+    uint32_t sum = 0;
+    const JitterArgs ja = jitter_args<EPI>(b, j, &sum);
     for (int e = tid; e < rows * (kAaCols / 4); e += 256) {
         const int t = e / (kAaCols / 4), c = 4 * (e % (kAaCols / 4)), x = x0 + c;
         if (x >= j.out_w) continue;
@@ -616,8 +778,10 @@ __global__ void __launch_bounds__(256) export_tensor_aa_kernel(const __grid_cons
             qy[i] = qs[0][t][c + i];
             if (!j.mono) { qu[i] = qs[1][t][c + i]; qv[i] = qs[2][t][c + i]; }
         }
-        tensor_store<DT, HWC, MIRROR, TONE>(j, tone_of(b), x, y0 + t, imin(4, j.out_w - x), qy, qu, qv, yoff, coff, 4 * bdmax);
+        tensor_store<DT, HWC, MIRROR, EPI>(j, tone_of(b), x, y0 + t, imin(4, j.out_w - x), qy, qu, qv, yoff, coff, 4 * bdmax,
+                                           ja);
     }
+    if constexpr (EPI == kEpiContrast) contrast_add(*jitter_of(b), sum);
 }
 
 }  // namespace b200
@@ -693,8 +857,8 @@ static int tensor_job_kind(const B200TensorJob &j)
 // the tile kernel's launch: the tallest tile (th output rows) whose grid still has kAaMinCtas CTAs, the SM count of an
 // H100 SXM, so that a single picture reduced to a small output still spreads over the whole GPU
 constexpr int kAaMinCtas = 132;
-template <int N, int F, bool T>
-static int launch_tensor_aa_jobs(const TensorBatch<N, T> &b, int n, int out_w, int out_h, cudaStream_t stream)
+template <int N, int F, int E>
+static int launch_tensor_aa_jobs(const TensorBatch<N, batch_of(E)> &b, int n, int out_w, int out_h, cudaStream_t stream)
 {
     const B200TensorJob &j = b.job[0];
     const int xt = (out_w + kAaCols - 1) / kAaCols;
@@ -703,53 +867,86 @@ static int launch_tensor_aa_jobs(const TensorBatch<N, T> &b, int n, int out_w, i
     const dim3 grid(xt, (out_h + th - 1) / th, n);
     return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, stream, [&](auto hbd) {
         constexpr bool H = decltype(hbd)::value;
-        void (*const k[2][3][2])(TensorBatch<N, T>, int) = {
-            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, false, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, false, F, T>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, false, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, false, F, T>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, false, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, false, F, T>}},
-            {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, true, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, true, F, T>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, true, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, true, F, T>},
-             {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, true, F, T>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, true, F, T>}}};
-        return std::make_tuple(k[j.flip][j.dtype][j.layout], b, th);
+        if constexpr (E == kEpiContrast) {          // S depends on none of dtype, layout and flip
+            return std::make_tuple(export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, false, F, E>, b, th);
+        } else {
+            void (*const k[2][3][2])(TensorBatch<N, E>, int) = {
+                {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, false, F, E>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, false, F, E>},
+                 {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, false, F, E>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, false, F, E>},
+                 {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, false, F, E>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, false, F, E>}},
+                {{export_tensor_aa_kernel<H, B200_TENSOR_F32, false, N, true, F, E>, export_tensor_aa_kernel<H, B200_TENSOR_F32, true, N, true, F, E>},
+                 {export_tensor_aa_kernel<H, B200_TENSOR_F16, false, N, true, F, E>, export_tensor_aa_kernel<H, B200_TENSOR_F16, true, N, true, F, E>},
+                 {export_tensor_aa_kernel<H, B200_TENSOR_BF16, false, N, true, F, E>, export_tensor_aa_kernel<H, B200_TENSOR_BF16, true, N, true, F, E>}}};
+            return std::make_tuple(k[j.flip][j.dtype][j.layout], b, th);
+        }
     });
 }
 
-// one launch for the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype, layout, kernel kind and flip, and with
-// T the tone maps at `tones`
-template <int N, bool T>
-static int launch_tensor_jobs(const B200TensorJob *const *jobs, const B200ToneMap *const *tones, int n, int kind, cudaStream_t stream)
+// one launch of the epilogue E for the n jobs of b, all of one bit-depth class, dtype, layout, kernel kind and flip
+template <int N, int E>
+static int launch_tensor_kind(const TensorBatch<N, batch_of(E)> &b, int n, int kind, cudaStream_t stream)
 {
-    TensorBatch<N, T> b{};
     int out_w = 0, out_h = 0;
-    for (int i = 0; i < n; i++) {
-        b.job[i] = *jobs[i];
-        if constexpr (T) b.tone[i] = *tones[i];
-        out_w = imax(out_w, jobs[i]->out_w); out_h = imax(out_h, jobs[i]->out_h);
-    }
-    if (kind == kTriangle) return launch_tensor_aa_jobs<N, kTriangle, T>(b, n, out_w, out_h, stream);
-    if (kind == kCubic) return launch_tensor_aa_jobs<N, kCubic, T>(b, n, out_w, out_h, stream);
+    for (int i = 0; i < n; i++) { out_w = imax(out_w, b.job[i].out_w); out_h = imax(out_h, b.job[i].out_h); }
+    if (kind == kTriangle) return launch_tensor_aa_jobs<N, kTriangle, E>(b, n, out_w, out_h, stream);
+    if (kind == kCubic) return launch_tensor_aa_jobs<N, kCubic, E>(b, n, out_w, out_h, stream);
     const B200TensorJob &j = b.job[0];
     const int runs = (out_w + 3) / 4;
     const dim3 grid((runs + 31) / 32, (out_h + 8 * kTensorRows - 1) / (8 * kTensorRows), n);
     return launch_hbd(j.bitdepth_max, Launch::pdl, grid, dim3(32, 8), 0, stream, [&](auto hbd) {
         constexpr bool H = decltype(hbd)::value;
-        void (*const k[2][3][2])(TensorBatch<N, T>) = {
-            {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, false, T>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, false, T>},
-             {export_tensor_kernel<H, B200_TENSOR_F16, false, N, false, T>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, false, T>},
-             {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, false, T>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, false, T>}},
-            {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, true, T>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, true, T>},
-             {export_tensor_kernel<H, B200_TENSOR_F16, false, N, true, T>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, true, T>},
-             {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, true, T>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, true, T>}}};
-        return std::make_tuple(k[j.flip][j.dtype][j.layout], b);
+        if constexpr (E == kEpiContrast) {
+            return std::make_tuple(export_tensor_kernel<H, B200_TENSOR_F32, false, N, false, E>, b);
+        } else {
+            void (*const k[2][3][2])(TensorBatch<N, E>) = {
+                {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, false, E>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, false, E>},
+                 {export_tensor_kernel<H, B200_TENSOR_F16, false, N, false, E>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, false, E>},
+                 {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, false, E>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, false, E>}},
+                {{export_tensor_kernel<H, B200_TENSOR_F32, false, N, true, E>, export_tensor_kernel<H, B200_TENSOR_F32, true, N, true, E>},
+                 {export_tensor_kernel<H, B200_TENSOR_F16, false, N, true, E>, export_tensor_kernel<H, B200_TENSOR_F16, true, N, true, E>},
+                 {export_tensor_kernel<H, B200_TENSOR_BF16, false, N, true, E>, export_tensor_kernel<H, B200_TENSOR_BF16, true, N, true, E>}}};
+            return std::make_tuple(k[j.flip][j.dtype][j.layout], b);
+        }
     });
 }
-// the tone-mapped forms are batched forms only: the N = 1 specialisation would double their build time for a prologue
-static int launch_tensor_group(const B200TensorJob *const *jobs, const B200ToneMap *const *tones, int n, int kind, int tone,
-                               cudaStream_t stream)
+
+// the launches of the n (1 .. N) jobs at `jobs`, all of one bit-depth class, dtype, layout, kernel kind and flip, with
+// (E = kEpiTone) the tone maps at `tones`, or (kEpiJitter) the optional tone maps at `tones` and the jitters at `jits`.
+// Jittered jobs with contrast first take their contrast pass: S zeroed, then summed by the kernel's sampling code; the
+// export's B200_PDL_ENTRY waits for it before reading S.
+template <int N, int E>
+static int launch_tensor_jobs(const B200TensorJob *const *jobs, const B200ToneMap *const *tones, const B200ColorJitter *const *jits,
+                              int n, int kind, cudaStream_t stream)
 {
-    if (tone) return launch_tensor_jobs<B200_TENSOR_TONE_BATCH_MAX, true>(jobs, tones, n, kind, stream);
-    return n == 1 ? launch_tensor_jobs<1, false>(jobs, tones, n, kind, stream)
-                  : launch_tensor_jobs<B200_TENSOR_BATCH_MAX, false>(jobs, tones, n, kind, stream);
+    TensorBatch<N, E> b{};
+    bool contrast = false;
+    for (int i = 0; i < n; i++) {
+        b.job[i] = *jobs[i];
+        if constexpr (E != kEpiPlain) if (tones[i]) b.tone[i] = *tones[i];
+        if constexpr (E == kEpiJitter) {
+            b.jit[i] = *jits[i];
+            contrast |= (jits[i]->enabled >> kJitContrast) & 1;
+        }
+    }
+    if constexpr (E == kEpiJitter) {
+        if (contrast) {
+            if (int r = launch_hbd(b.job[0].bitdepth_max, Launch::pdl, dim3(1), dim3(32), 0, stream,
+                                   [&](auto) { return std::make_tuple(contrast_zero_kernel<N>, b, n); }))
+                return r;
+            if (int r = launch_tensor_kind<N, kEpiContrast>(b, n, kind, stream)) return r;
+        }
+    }
+    return launch_tensor_kind<N, E>(b, n, kind, stream);
+}
+// the tone-mapped and jittered forms are batched forms only: the N = 1 specialisation would double their build time for
+// a prologue
+static int launch_tensor_group(const B200TensorJob *const *jobs, const B200ToneMap *const *tones, const B200ColorJitter *const *jits,
+                               int n, int kind, int epi, cudaStream_t stream)
+{
+    if (epi == kEpiJitter) return launch_tensor_jobs<B200_TENSOR_JITTER_BATCH_MAX, kEpiJitter>(jobs, tones, jits, n, kind, stream);
+    if (epi == kEpiTone) return launch_tensor_jobs<B200_TENSOR_TONE_BATCH_MAX, kEpiTone>(jobs, tones, jits, n, kind, stream);
+    return n == 1 ? launch_tensor_jobs<1, kEpiPlain>(jobs, tones, jits, n, kind, stream)
+                  : launch_tensor_jobs<B200_TENSOR_BATCH_MAX, kEpiPlain>(jobs, tones, jits, n, kind, stream);
 }
 
 extern "C" int b200_export_tensor(const B200TensorJob *job, void *stream)
@@ -762,22 +959,48 @@ extern "C" int b200_export_tensor_batch(const B200TensorJob *jobs, int n, void *
     return b200_export_tensor_tone_batch(jobs, nullptr, n, stream);
 }
 
+extern "C" int b200_export_tensor_tone_batch(const B200TensorJob *jobs, const B200ToneMap *const *tones, int n, void *stream)
+{
+    return b200_export_tensor_jitter_batch(jobs, tones, nullptr, n, stream);
+}
+
 // a job's tone map, checked as it arrives from outside the library: 0, or -2 with the error set
-static int check_tone_map(const B200ToneMap &t, const B200TensorJob &j, int i)
+static int check_tone_map(const B200ToneMap &t, const B200TensorJob &j, int i, const char *who)
 {
     bool finite = true;
     for (int k = 0; k < 9; k++) finite &= std::isfinite(t.m[k]);
     if (!t.curve || !t.oetf || t.curve_len != 4 * j.bitdepth_max + 1 || t.oetf_bits < 8 || t.oetf_bits > 16 || !finite) {
-        b200_set_error("b200_export_tensor_tone_batch: bad tone map of job %d (curve_len %d for bitdepth_max %d, oetf_bits %d)", i,
+        b200_set_error("%s: bad tone map of job %d (curve_len %d for bitdepth_max %d, oetf_bits %d)", who, i,
                        t.curve_len, j.bitdepth_max, t.oetf_bits);
         return -2;
     }
     return 0;
 }
 
-extern "C" int b200_export_tensor_tone_batch(const B200TensorJob *jobs, const B200ToneMap *const *tones, int n, void *stream)
+// a job's colour jitter, checked as it arrives from outside the library: 0, or -2 with the error set
+static int check_jitter(const B200ColorJitter &t, int i, const char *who)
 {
-    const char *const who = tones ? "b200_export_tensor_tone_batch" : n == 1 ? "b200_export_tensor" : "b200_export_tensor_batch";
+    const float f[6] = {t.brightness, t.contrast, t.saturation, t.hue, t.contrast1, t.saturation1};
+    bool finite = true;
+    for (float v : f) finite &= std::isfinite(v);
+    int seen = 0;
+    for (int k = 0; k < 4; k++) seen |= (unsigned)t.order[k] < 4 ? 1 << t.order[k] : 16;
+    const bool contrast = (t.enabled >> kJitContrast) & 1;
+    if (!finite || t.brightness < 0 || t.contrast < 0 || t.saturation < 0 || !(t.hue >= -0.5f && t.hue <= 0.5f) || seen != 15 ||
+        (t.enabled & ~15) || (unsigned)t.grayscale > 1 || (contrast && (!t.acc || ((uintptr_t)t.acc & 7)))) {
+        b200_set_error("%s: bad colour jitter of job %d (factors %g %g %g %g, order %d %d %d %d, enabled %#x, grayscale %d, acc %p)",
+                       who, i, t.brightness, t.contrast, t.saturation, t.hue, t.order[0], t.order[1], t.order[2], t.order[3],
+                       t.enabled, t.grayscale, (const void *)t.acc);
+        return -2;
+    }
+    return 0;
+}
+
+extern "C" int b200_export_tensor_jitter_batch(const B200TensorJob *jobs, const B200ToneMap *const *tones,
+                                               const B200ColorJitter *const *jits, int n, void *stream)
+{
+    const char *const who = jits ? "b200_export_tensor_jitter_batch" : tones ? "b200_export_tensor_tone_batch"
+                                                                      : n == 1 ? "b200_export_tensor" : "b200_export_tensor_batch";
     if (!jobs || n < 1) { b200_set_error("%s: no jobs (%d)", who, n); return -2; }
     for (int i = 0; i < n; i++) {
         if (int r = check_tensor_job(jobs[i], who)) return r;
@@ -786,27 +1009,33 @@ extern "C" int b200_export_tensor_tone_batch(const B200TensorJob *jobs, const B2
             return -2;
         }
         if (tones && tones[i])
-            if (int r = check_tone_map(*tones[i], jobs[i], i)) return r;
+            if (int r = check_tone_map(*tones[i], jobs[i], i, who)) return r;
+        if (jits && jits[i])
+            if (int r = check_jitter(*jits[i], i, who)) return r;
     }
-    // one launch per bit-depth class, kernel kind (bilinear, triangle, cubic), flip and tone map present and per
-    // B200_TENSOR_BATCH_MAX (tone-mapped: B200_TENSOR_TONE_BATCH_MAX) jobs of it, jobs in their order
-    for (int group = 0; group < 24; group++) {
-        const int hbd = group & 1, kind = (group >> 1) % 3, flip = (group / 6) & 1, tone = group / 12;
-        const int cap = tone ? B200_TENSOR_TONE_BATCH_MAX : B200_TENSOR_BATCH_MAX;
+    // one launch per bit-depth class, kernel kind (bilinear, triangle, cubic), flip and epilogue (plain, tone-mapped,
+    // jittered with or without a tone map) and per B200_TENSOR_BATCH_MAX (tone-mapped: B200_TENSOR_TONE_BATCH_MAX,
+    // jittered: B200_TENSOR_JITTER_BATCH_MAX) jobs of it, jobs in their order
+    for (int group = 0; group < 36; group++) {
+        const int hbd = group & 1, kind = (group >> 1) % 3, flip = (group / 6) & 1, epi = group / 12;
+        const int cap = epi == kEpiJitter ? B200_TENSOR_JITTER_BATCH_MAX : epi == kEpiTone ? B200_TENSOR_TONE_BATCH_MAX : B200_TENSOR_BATCH_MAX;
         const B200TensorJob *part[B200_TENSOR_BATCH_MAX];
         const B200ToneMap *tpart[B200_TENSOR_BATCH_MAX];
+        const B200ColorJitter *jpart[B200_TENSOR_BATCH_MAX];
         int m = 0;
         for (int i = 0; i < n; i++) {
             const B200ToneMap *const t = tones ? tones[i] : nullptr;
-            if ((jobs[i].bitdepth_max > 255) != hbd || tensor_job_kind(jobs[i]) != kind || jobs[i].flip != flip || !!t != tone) continue;
-            part[m] = &jobs[i]; tpart[m++] = t;
+            const B200ColorJitter *const c = jits ? jits[i] : nullptr;
+            const int e = c ? kEpiJitter : t ? kEpiTone : kEpiPlain;
+            if ((jobs[i].bitdepth_max > 255) != hbd || tensor_job_kind(jobs[i]) != kind || jobs[i].flip != flip || e != epi) continue;
+            part[m] = &jobs[i]; tpart[m] = t; jpart[m++] = c;
             if (m == cap) {
-                if (int r = launch_tensor_group(part, tpart, m, kind, tone, (cudaStream_t)stream)) return r;
+                if (int r = launch_tensor_group(part, tpart, jpart, m, kind, epi, (cudaStream_t)stream)) return r;
                 m = 0;
             }
         }
         if (m)
-            if (int r = launch_tensor_group(part, tpart, m, kind, tone, (cudaStream_t)stream)) return r;
+            if (int r = launch_tensor_group(part, tpart, jpart, m, kind, epi, (cudaStream_t)stream)) return r;
     }
     return 0;
 }

@@ -542,7 +542,7 @@ int b200_struct_size(int which)
     case 12: return sizeof(B200FgFrame); case 13: return sizeof(B200FilmGrainData);
     case 14: return sizeof(B200IntraTx); case 15: return sizeof(B200IntraFrame); case 16: return sizeof(B200McScaledBlock); case 17: return sizeof(B200CoefBlock); case 18: return sizeof(B200IntraSb); case 19: return sizeof(B200CompFusedBlock); case 20: return sizeof(B200FrameBand); case 21: return sizeof(B200ResizeFrame);
     case 22: return sizeof(B200ExportJob); case 23: return sizeof(B200TensorJob);
-    case 24: return sizeof(B200ToneMap);
+    case 24: return sizeof(B200ToneMap); case 25: return sizeof(B200ColorJitter);
     }
     return -1;
 }

@@ -11,7 +11,7 @@ import threading
 
 import numpy as np
 
-from ._lib import ExportJob, TensorJob, ToneMap  # noqa: F401  (B200ExportJob / B200TensorJob / B200ToneMap, filled by DeviceDecoder)
+from ._lib import ColorJitter, ExportJob, TensorJob, ToneMap  # noqa: F401  (the B200 structs DeviceDecoder fills)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -190,15 +190,16 @@ SITINGS = {"left": (0, 1), "topleft": (0, 0), "center": (1, 1)}
 CHR_TO_SITING = {0: "left", 1: "left", 2: "topleft"}
 
 
-def tensor_scale_bias(bpc, mean=None, std=None):
+def tensor_scale_bias(bpc, mean=None, std=None, jittered=False):
     """float32 (scale, bias) per channel of the tensor export: out = R * scale + bias with R in 0 .. 4 * bdmax, so that
-    out = (R / (4 * bdmax) - mean) / std; mean 0 and std 1 by default (outputs in [0, 1])"""
+    out = (R / (4 * bdmax) - mean) / std; mean 0 and std 1 by default (outputs in [0, 1]). jittered=True: the scale of a
+    colour-jittered job (B200ColorJitter), whose J is in [0, 1] already: out = (J - mean) / std"""
     bdmax = (1 << bpc) - 1
     mean = [0.0] * 3 if mean is None else [float(v) for v in mean]
     std = [1.0] * 3 if std is None else [float(v) for v in std]
     if len(mean) != 3 or len(std) != 3 or not all(v > 0 for v in std):
         raise ValueError("mean and std need 3 values each, std > 0")
-    scale = np.array([1.0 / (4 * bdmax * s) for s in std], np.float32)
+    scale = np.array([1.0 / (s if jittered else 4 * bdmax * s) for s in std], np.float32)
     bias = np.array([-m / s for m, s in zip(mean, std)], np.float32)
     return scale, bias
 
@@ -384,6 +385,155 @@ def tone_reference(rgb, tone):
     return np.stack([oetf[np.rint(np.clip(g, np.float32(0), np.float32(1)) * np.float32(1 << bits)).astype(np.int64)] for g in G])
 
 
+# ---- colour jitter (B200ColorJitter, include/b200av1.h): torchvision's ColorJitter in float32 ------------------------
+JITTER_OPS = ("brightness", "contrast", "saturation", "hue")     # torchvision's numbering of fn_idx
+
+
+def _is_jitter(j):
+    """whether j has the shape of what torchvision.transforms.ColorJitter.get_params returns: (fn_idx, b, c, s, h)"""
+    if not isinstance(j, (tuple, list)) or len(j) != 5:
+        return False
+    try:
+        return len(j[0]) == 4
+    except TypeError:
+        return False
+
+
+def jitter_factors(jitter):
+    """(order, enabled, b, c, s, hue, c1, s1) of B200ColorJitter for jitter = (fn_idx, b, c, s, h), the tuple
+    torchvision.transforms.ColorJitter.get_params returns (None: that op is off). The factors are float32, c1 and s1 are
+    f32(1.0 - factor) with the difference taken in float64, as torchvision's _blend does; a disabled op gets a neutral
+    factor. ValueError for a fn_idx that is not a permutation of 0 .. 3, a factor that is not a finite number, a negative
+    brightness, contrast or saturation, or a hue outside [-0.5, 0.5]."""
+    if not _is_jitter(jitter):
+        raise ValueError("jitter must be None or (fn_idx, brightness, contrast, saturation, hue) as ColorJitter.get_params "
+                         "returns it, not %r" % (jitter,))
+    try:
+        order = [int(v) for v in jitter[0]]
+    except (TypeError, ValueError):
+        order = None
+    if order is None or sorted(order) != [0, 1, 2, 3]:
+        raise ValueError("jitter fn_idx must be a permutation of 0 .. 3, not %r" % (jitter[0],))
+    enabled, f = 0, []
+    for op, v in enumerate(jitter[1:]):
+        if v is None:
+            f.append(0.0 if op == 3 else 1.0)
+            continue
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)) or not np.isfinite(v):
+            raise ValueError("jitter %s factor must be a finite number, not %r" % (JITTER_OPS[op], v))
+        v = float(v)
+        if (op < 3 and v < 0) or (op == 3 and not -0.5 <= v <= 0.5):
+            raise ValueError("jitter %s factor %r is out of range (%s)" % (JITTER_OPS[op], v, ">= 0" if op < 3 else "-0.5 .. 0.5"))
+        enabled |= 1 << op
+        f.append(v)
+    b, c, s, h = f
+    c1, s1 = (1.0 - c if enabled & 2 else 0.0), (1.0 - s if enabled & 4 else 0.0)
+    return (order, enabled) + tuple(np.float32(v) for v in (b, c, s, h, c1, s1))
+
+
+def color_jitter(jitter, grayscale=False, acc=None):
+    """the B200ColorJitter of jitter (jitter_factors; None: no op) and grayscale, its contrast scratch at address acc"""
+    if not _is_flag(grayscale):
+        raise ValueError("grayscale must be a bool, not %r" % (grayscale,))
+    order, enabled, b, c, s, h, c1, s1 = jitter_factors(jitter) if jitter is not None else ([0, 1, 2, 3], 0) + (1, 1, 1, 0, 0, 0)
+    t = ColorJitter()
+    t.brightness, t.contrast, t.saturation, t.hue, t.contrast1, t.saturation1 = (float(v) for v in (b, c, s, h, c1, s1))
+    t.order[:] = order
+    t.enabled, t.grayscale, t.acc = enabled, int(grayscale), acc
+    return t
+
+
+# float32 operations as the export kernels compute them under -ftz: a subnormal operand or result is a zero of its sign
+_TINY = np.float32(2.0 ** -126)
+
+
+def _ftz(a):
+    a = np.asarray(a, np.float32)
+    return np.where(np.abs(a) < _TINY, np.copysign(np.float32(0), a), a).astype(np.float32)
+
+
+def _fmul(a, b):
+    return _ftz(_ftz(a) * _ftz(b))
+
+
+def _fadd(a, b):
+    return _ftz(_ftz(a) + _ftz(b))
+
+
+def _fsub(a, b):
+    return _ftz(_ftz(a) - _ftz(b))
+
+
+def _fdiv(a, b):
+    return _ftz(_ftz(a) / _ftz(b))
+
+
+def _unit_clip(a):
+    return np.minimum(np.maximum(a, np.float32(0)), np.float32(1))
+
+
+def jitter_gray(x):
+    """torchvision's rgb_to_grayscale of x [3, ...] in float32: ((0.2989 r + 0.587 g) + 0.114 b)"""
+    f = np.float32
+    return _fadd(_fadd(_fmul(f(0.2989), x[0]), _fmul(f(0.587), x[1])), _fmul(f(0.114), x[2]))
+
+
+def _jitter_hue(x, hue):
+    """torchvision's adjust_hue on x [3, ...]: _rgb2hsv, remainder(h + hue, 1), _hsv2rgb"""
+    f = np.float32
+    r, g, b = x
+    maxc, minc = np.maximum(np.maximum(r, g), b), np.minimum(np.minimum(r, g), b)
+    eqc = maxc == minc
+    cr = _fsub(maxc, minc)
+    s = _fdiv(cr, np.where(eqc, f(1), maxc))
+    d = np.where(eqc, f(1), cr)
+    rc, gc, bc = (_fdiv(_fsub(maxc, c), d) for c in (r, g, b))
+    h = np.where(maxc == r, _fsub(bc, gc), np.where(maxc == g, _fsub(_fadd(f(2), rc), bc), _fsub(_fadd(f(4), gc), rc)))
+    h = np.fmod(_fadd(_fdiv(h, f(6)), f(1)), f(1))
+    h = np.fmod(_fadd(h, hue), f(1))
+    h = np.where(h < 0, _fadd(h, f(1)), h)
+    h6 = _fmul(h, f(6))
+    fi = np.floor(h6)
+    fr = _fsub(h6, fi)
+    p = _unit_clip(_fmul(maxc, _fsub(f(1), s)))
+    q = _unit_clip(_fmul(maxc, _fsub(f(1), _fmul(s, fr))))
+    t = _unit_clip(_fmul(maxc, _fsub(f(1), _fmul(s, _fsub(f(1), fr)))))
+    i = fi.astype(np.int64) % 6
+    return np.stack([np.choose(i, [maxc, q, p, p, t, maxc]), np.choose(i, [t, maxc, maxc, q, p, p]),
+                     np.choose(i, [p, p, t, maxc, maxc, q])]).astype(np.float32)
+
+
+def contrast_mean(gray):
+    """M of B200ColorJitter: the mean of gray over the picture, f32(f64(S) / (f64(n) * 2^24)) with the exact
+    S = sum of rint(gray * 2^24)"""
+    total = int(np.rint(_fmul(gray, np.float32(1 << 24))).astype(np.int64).sum())
+    return np.float32(float(total) / (float(gray.size) * float(1 << 24)))
+
+
+def jitter_reference(x, jitter, grayscale=False):
+    """numpy statement of the colour jitter stage (include/b200av1.h B200ColorJitter) on one picture x = float32
+    [3, H, W] in [0, 1]: the enabled ops of jitter = (fn_idx, b, c, s, h) (ColorJitter.get_params; None: none) in the
+    order fn_idx gives, contrast against the picture's mean gray M (contrast_mean), then with grayscale the gray on all
+    three channels. Each float32 operation is rounded on its own and flushed like the kernels'."""
+    x = _ftz(x).copy()
+    if jitter is not None:
+        order, enabled, b, c, s, h, c1, s1 = jitter_factors(jitter)
+        for op in order:
+            if not (enabled >> op) & 1:
+                continue
+            if op == 0:
+                x = _unit_clip(_fmul(b, x))
+            elif op == 1:
+                x = _unit_clip(_fadd(_fmul(c, x), _fmul(c1, contrast_mean(jitter_gray(x)))))
+            elif op == 2:
+                x = _unit_clip(_fadd(_fmul(s, x), _fmul(s1, jitter_gray(x))))
+            else:
+                x = _jitter_hue(x, h)
+    if grayscale:
+        x = np.broadcast_to(jitter_gray(x), x.shape).astype(np.float32)
+    return x
+
+
 def tensor_antialiased(w, h, size, antialias):
     """whether an export of a w x h picture to size = (OH, OW) takes the antialiased definition: antialias and a luma axis
     reduced (sigma > 256)"""
@@ -392,12 +542,14 @@ def tensor_antialiased(w, h, size, antialias):
 
 
 def tensor_reference(planes, bpc, layout, size=None, matrix="bt709", full_range=False, siting="left", mean=None, std=None,
-                     antialias=False, interpolation="bilinear", tone=None):
+                     antialias=False, interpolation="bilinear", tone=None, jitter=None, grayscale=False):
     """numpy statement of the tensor export (include/b200av1.h B200TensorJob) for one picture's planes (layout = enum
     Dav1dPixelLayout): float32 [3, OH, OW] of R, G, B; size = (OH, OW), by default the picture's. antialias=True: the
     antialiased definition (triangle filter on reduced axes), which leaves exports without a reduced luma axis unchanged.
     interpolation="bicubic": the bicubic definition instead, plain or (antialias=True) antialiased on every axis.
-    tone=(curve, m, oetf), e.g. tone_tables(...): the HDR to SDR stage of B200ToneMap between the matrix and the output."""
+    tone=(curve, m, oetf), e.g. tone_tables(...): the HDR to SDR stage of B200ToneMap between the matrix and the output.
+    jitter=(fn_idx, b, c, s, h) (ColorJitter.get_params) and / or grayscale=True: the colour jitter stage of
+    B200ColorJitter after it (jitter_reference), with its output rule."""
     h, w = planes[0].shape
     oh, ow = size or (h, w)
     ssh, ssv = int(layout in (1, 2)), int(layout == 1)
@@ -435,9 +587,13 @@ def tensor_reference(planes, bpc, layout, size=None, matrix="bt709", full_range=
         yy = cy * (y - (0 if full_range else 64 << s)) + 8192
         cb, cr = (0, 0) if u is None else (u - (512 << s), v - (512 << s))
         rgb = np.clip(np.stack([(yy + rv * cr) >> 14, (yy - gu * cb - gv * cr) >> 14, (yy + bu * cb) >> 14]), 0, 4 * bdmax)
-    scale, bias = tensor_scale_bias(bpc, mean, std)
     t = rgb.astype(np.float32) if tone is None else tone_reference(rgb, tone)
-    return t * scale[:, None, None] + bias[:, None, None]
+    if jitter is None and not grayscale:
+        scale, bias = tensor_scale_bias(bpc, mean, std)
+        return t * scale[:, None, None] + bias[:, None, None]
+    scale, bias = tensor_scale_bias(bpc, mean, std, jittered=True)
+    x = jitter_reference(_fmul(t, np.float32(1) / np.float32(4 * bdmax)), jitter, grayscale)
+    return _fadd(_fmul(x, scale[:, None, None]), bias[:, None, None])
 
 
 def crop_planes(planes, layout, box):
@@ -513,13 +669,15 @@ class DeviceDecoder:
         d.refdrv_stream_chroma_position.argtypes = [C.c_void_p]
         d.refdrv_stream_color.argtypes = [C.c_void_p, C.c_void_p]
         d.b200hook_export_tensor_tone_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        d.b200hook_export_tensor_jitter_batch.argtypes = [C.c_void_p] * 5 + [C.c_int, C.c_void_p]
         self._tones = {}                         # (transfer, primaries, bpc, peak, sdr_peak, device) -> (ToneMap, tables)
+        self._accs = {}                          # (device, stream) -> the contrast scratch of jittered exports, grown
 
     def stats(self, reset=False):
         return self._hooked.stats(reset)
 
     def release(self):
-        self._drop_tones()
+        self._drop_tables()
         self._hooked.release()
 
     def pictures(self, tus, format="planes", matrix="auto", full_range=None, alloc=None, stream=None):
@@ -540,7 +698,7 @@ class DeviceDecoder:
 
     def tensors(self, tus, size=None, dtype="float32", layout="chw", mean=None, std=None, matrix="auto", full_range=None,
                 chroma_siting="auto", batch=None, alloc=None, stream=None, antialias=False, crop=None, flip=False,
-                interpolation="bilinear", tonemap=None, peak=None, sdr_peak=SDR_PEAK):
+                interpolation="bilinear", tonemap=None, peak=None, sdr_peak=SDR_PEAK, jitter=None, grayscale=False):
         """Decodes the temporal units `tus` and yields every output picture as a model input: R, G, B resized to
         size = (height, width) (default: the picture's own) by bilinear sampling at half-sample centres, like
         torch.nn.functional.interpolate(mode="bilinear", align_corners=False) (chroma upsampling is part of the same
@@ -570,7 +728,14 @@ class DeviceDecoder:
         curves) and exports every other stream exactly as None does; "pq" or "hlg" force that transfer, for streams without
         a colour description. peak: the source peak in cd/m^2, by default MaxCLL, else the mastering display's maximum
         luminance, else 1000 (HLG: 1000); sdr_peak: the light that becomes SDR white (203 cd/m^2, BT.2408). The colour
-        primaries come from the header (unspecified: BT.2020). The tone map applies to the resized signal."""
+        primaries come from the header (unspecified: BT.2020). The tone map applies to the resized signal.
+        jitter: None (the default), the tuple (fn_idx, brightness, contrast, saturation, hue) that
+        torchvision.transforms.ColorJitter.get_params returns (None entries: those ops off), or a callable k -> tuple or
+        None for output picture k (RandomApply(ColorJitter, p) returns None with probability 1 - p): torchvision's colour
+        jitter, in the order fn_idx gives, on the resized (and tone-mapped) picture in [0, 1], contrast against that
+        picture's own mean gray (include/b200av1.h B200ColorJitter; jitter_reference states it). grayscale: a bool, or a
+        callable k -> bool: the gray of the jittered picture on all three channels (RandomGrayscale). mean / std apply
+        after both. ValueError, naming the picture, for a malformed tuple or an out-of-range factor."""
         if dtype not in TENSOR_DTYPES or layout not in TENSOR_LAYOUTS:
             raise ValueError("dtype must be one of %s, layout 'chw' or 'hwc'" % ", ".join(TENSOR_DTYPES))
         if matrix != "auto" and matrix != "identity" and matrix not in MATRICES:
@@ -589,6 +754,10 @@ class DeviceDecoder:
             raise ValueError("flip must be a bool or a callable")
         _check_interpolation(interpolation)
         _check_tonemap(tonemap, peak, sdr_peak)
+        if jitter is not None and not callable(jitter):
+            jitter_factors(jitter)
+        if not callable(grayscale) and not _is_flag(grayscale):
+            raise ValueError("grayscale must be a bool or a callable")
         tensor_scale_bias(8, mean, std)                          # checks mean / std
         alloc, stream = _default_alloc(alloc, stream)
         esize = 4 if dtype == "float32" else 2
@@ -602,12 +771,15 @@ class DeviceDecoder:
             fl = flip(k) if callable(flip) else flip
             if not _is_flag(fl):
                 raise ValueError("picture %d: flip must be a bool, not %r" % (k, fl))
+            jit = _picture_jitter(jitter(k) if callable(jitter) else jitter, grayscale(k) if callable(grayscale) else grayscale,
+                                  "picture %d" % k)
             oh, ow = size or ((box[2], box[3]) if box else (int(info[1]), int(info[0])))
             shape = (3, oh, ow) if layout == "chw" else (oh, ow, 3)
             if batch is None:
                 out = alloc(shape, dtype)
                 self._export_tensor(h, info, _data_ptr(out), oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
-                                    antialias, stream, box, fl, interpolation, self._tone(h, info, out, **tone_kw))
+                                    antialias, stream, box, fl, interpolation, self._tone(h, info, out, **tone_kw),
+                                    self._jitter(jit, out, stream))
                 return [out]
             done = []
             if state["buf"] is not None and state["shape"] != shape:       # another size closes the batch
@@ -617,7 +789,8 @@ class DeviceDecoder:
                 state.update(buf=alloc((int(batch),) + shape, dtype), n=0, shape=shape)
             dst = _data_ptr(state["buf"]) + state["n"] * 3 * oh * ow * esize
             self._export_tensor(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting, antialias, stream,
-                                box, fl, interpolation, self._tone(h, info, state["buf"], **tone_kw))
+                                box, fl, interpolation, self._tone(h, info, state["buf"], **tone_kw),
+                                self._jitter(jit, state["buf"], stream))
             state["n"] += 1
             if state["n"] == batch:
                 done.append(state["buf"])
@@ -631,7 +804,8 @@ class DeviceDecoder:
 
     def clips(self, streams, frames, step=1, start=0, size=None, dtype="float32", layout="chw", mean=None, std=None,
               matrix="auto", full_range=None, chroma_siting="auto", workers=None, alloc=None, stream=None, antialias=False,
-              crop=None, flip=False, interpolation="bilinear", tonemap=None, peak=None, sdr_peak=SDR_PEAK):
+              crop=None, flip=False, interpolation="bilinear", tonemap=None, peak=None, sdr_peak=SDR_PEAK, jitter=None,
+              grayscale=False):
         """Decodes N streams (each a list of temporal units) concurrently and returns one clip per stream as a
         [N, frames, 3, OH, OW] tensor (layout="hwc": [N, frames, OH, OW, 3]): x[i, t] is output picture
         start_i + t * step of stream i, exported exactly as tensors() exports it. `start` is one int or one per stream.
@@ -641,7 +815,11 @@ class DeviceDecoder:
         called once per stream i on its first sampled picture; flip: one bool, or one per stream. Every picture of a clip
         takes its stream's box and flip (tensors() says what they do), so a clip stays consistent in time. tonemap, peak and
         sdr_peak: as in tensors(), resolved per stream from its own headers and metadata ("auto" converts the PQ and HLG
-        streams of a batch and exports the others as they are, in the same batched launches).
+        streams of a batch and exports the others as they are, in the same batched launches). jitter: one tuple (as
+        tensors() takes it) for every stream, one tuple or None per stream, or a callable i -> tuple or None called once per
+        stream; grayscale: one bool, or one per stream. Every picture of a clip takes its stream's jitter and grayscale, as
+        it takes its box and flip, and contrast uses each picture's own mean gray, as torchvision's ColorJitter does on a
+        [T, 3, H, W] clip.
         Each stream has a dav1d context of its own (this decoder's n_threads / max_frame_delay) driven by a host thread of
         its own; at most `workers` streams are open at once (default min(N, CLIP_WORKERS), at most CLIP_MAX_WORKERS).
         Pictures that are not sampled are released unexported, and a stream is closed once its last sampled picture is
@@ -679,6 +857,21 @@ class DeviceDecoder:
             flips = [bool(f) for f in flip]
         else:
             raise ValueError("flip must be a bool or one bool per stream")
+        if jitter is None or callable(jitter) or _is_jitter(jitter):
+            jits = [jitter] * n
+        elif isinstance(jitter, (list, tuple)) and len(jitter) == n and all(j is None or _is_jitter(j) for j in jitter):
+            jits = list(jitter)
+        else:
+            raise ValueError("jitter must be None, a ColorJitter.get_params tuple, one tuple or None per stream or a callable")
+        if _is_flag(grayscale):
+            grays = [bool(grayscale)] * n
+        elif isinstance(grayscale, (list, tuple, np.ndarray)) and len(grayscale) == n and all(_is_flag(g) for g in grayscale):
+            grays = [bool(g) for g in grayscale]
+        else:
+            raise ValueError("grayscale must be a bool or one bool per stream")
+        for i in range(n):
+            if not callable(jits[i]):
+                jits[i] = _picture_jitter(jits[i], grays[i], "stream %d" % i)
         _check_interpolation(interpolation)
         _check_tonemap(tonemap, peak, sdr_peak)
         tensor_scale_bias(8, mean, std)                          # checks mean / std
@@ -711,9 +904,13 @@ class DeviceDecoder:
                     pics = (C.c_void_p * len(items))()
                     boxes = (C.c_int32 * (4 * len(items)))() if crop is not None else None
                     tones = (C.POINTER(ToneMap) * len(items))()
+                    jitters = (C.POINTER(ColorJitter) * len(items))()
+                    keep = []
                     for k, (i, t, h, info, _) in enumerate(items):
                         if callable(crops[i]):                  # the stream's box, from its first sampled picture
                             crops[i] = crops[i](i, int(info[1]), int(info[0]))
+                        if callable(jits[i]):                   # the stream's jitter, asked for once
+                            jits[i] = _picture_jitter(jits[i](i), grays[i], "stream %d" % i)
                         box = _picture_box(crops[i], info, "stream %d picture %d" % (i, starts[i] + t * step))
                         if box:
                             boxes[4 * k:4 * k + 4] = box
@@ -726,13 +923,17 @@ class DeviceDecoder:
                                              "pictures of different sizes" % (i, starts[i] + t * step, ow, oh, hw[1], hw[0]))
                         dst = _data_ptr(out) + (i * frames + t) * 3 * oh * ow * esize
                         jobs[k] = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, chroma_siting,
-                                                   antialias, flips[i], interpolation)
+                                                   antialias, flips[i], interpolation, jits[i] is not None)
                         pics[k] = self.dll.refdrv_stream_picture(h)
                         tm = self._tone(h, info, out, tonemap, peak, sdr_peak)
                         if tm is not None:
                             tones[k] = C.pointer(tm)
-                    if self.dll.b200hook_export_tensor_tone_batch(pics, jobs, boxes, tones if any(tones) else None, len(items),
-                                                                  C.c_void_p(stream)) != 0:
+                        if jits[i] is not None:
+                            keep.append(color_jitter(*jits[i], acc=self._acc(out, stream, len(items)) + 8 * k))
+                            jitters[k] = C.pointer(keep[-1])
+                    if self.dll.b200hook_export_tensor_jitter_batch(pics, jobs, boxes, tones if any(tones) else None,
+                                                                    jitters if any(jitters) else None, len(items),
+                                                                    C.c_void_p(stream)) != 0:
                         raise RuntimeError("exporting pictures failed (see stderr)")
                     left -= len(items)
                 finally:
@@ -834,16 +1035,19 @@ class DeviceDecoder:
         return name
 
     def _export_tensor(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, stream, box,
-                       flip, interpolation, tone=None):
+                       flip, interpolation, tone=None, jitter=None):
         job = self._tensor_job(h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip,
-                               interpolation)
+                               interpolation, jitter is not None)
         box = (C.c_int32 * 4)(*box) if box else None
         pic = self.dll.refdrv_stream_picture(h)
-        if tone is None:
+        tones = (C.POINTER(ToneMap) * 1)(C.pointer(tone)) if tone is not None else None
+        if jitter is not None:
+            rc = self.dll.b200hook_export_tensor_jitter_batch((C.c_void_p * 1)(pic), C.byref(job), box, tones,
+                                                              (C.POINTER(ColorJitter) * 1)(C.pointer(jitter)), 1, C.c_void_p(stream))
+        elif tone is None:
             rc = self.dll.b200hook_export_tensor(pic, C.byref(job), box, C.c_void_p(stream))
         else:
-            rc = self.dll.b200hook_export_tensor_tone_batch((C.c_void_p * 1)(pic), C.byref(job), box,
-                                                            (C.POINTER(ToneMap) * 1)(C.pointer(tone)), 1, C.c_void_p(stream))
+            rc = self.dll.b200hook_export_tensor_tone_batch((C.c_void_p * 1)(pic), C.byref(job), box, tones, 1, C.c_void_p(stream))
         if rc != 0:
             raise RuntimeError("exporting a picture failed (see stderr)")
 
@@ -883,16 +1087,40 @@ class DeviceDecoder:
             self._tones[key] = (tm, tables)
         return self._tones[key][0]
 
-    def _drop_tones(self):
-        """frees the tone tables once the launches that may still read them have completed"""
+    def _jitter(self, jit, out, stream):
+        """the B200ColorJitter of jit = (jitter tuple or None, grayscale) as _picture_jitter gives it (None: no jitter),
+        with contrast scratch from _acc"""
+        if jit is None:
+            return None
+        return color_jitter(*jit, acc=self._acc(out, stream, 1))
+
+    def _acc(self, out, stream, n):
+        """the address of n uint64 contrast sums (B200ColorJitter.acc) on the device of the destination `out` (host memory
+        for a host destination), for exports on `stream`. Each (device, stream) has its own, so exports on different streams
+        never share one; on one stream, the export of the next call waits for the last. Kept until release()."""
+        device = out.device if getattr(out, "is_cuda", False) else None
+        bufs = self._accs.setdefault((str(device), stream), [])
+        if not bufs or len(bufs[-1]) < n:
+            size = max(n, 2 * len(bufs[-1]) if bufs else 16)
+            if device is None:
+                bufs.append(np.zeros(size, np.uint64))
+            else:
+                import torch
+                bufs.append(torch.empty(size, dtype=torch.int64, device=device))
+        return _data_ptr(bufs[-1])
+
+    def _drop_tables(self):
+        """frees the tone tables and the contrast scratch once the launches that may still read them have completed"""
         import sys
         if "torch" in sys.modules:
-            for dev in {t.device for _, tables in self._tones.values() for t in tables if getattr(t, "is_cuda", False)}:
+            arrays = [t for _, tables in self._tones.values() for t in tables] + [a for bufs in self._accs.values() for a in bufs]
+            for dev in {t.device for t in arrays if getattr(t, "is_cuda", False)}:
                 sys.modules["torch"].cuda.synchronize(dev)
         self._tones.clear()
+        self._accs.clear()
 
     def _tensor_job(self, h, info, dst, oh, ow, dtype, layout, mean, std, matrix, full_range, siting, antialias, flip,
-                    interpolation="bilinear"):
+                    interpolation="bilinear", jittered=False):
         """the B200TensorJob of the picture stream h holds (info as _decode gives it): "auto" matrix, range and siting come
         from that stream's own headers"""
         w, hh, bpc, pl, mtrx, color_range = (int(v) for v in info)
@@ -906,7 +1134,7 @@ class DeviceDecoder:
         if siting == "auto":
             siting = CHR_TO_SITING.get(self.dll.refdrv_stream_chroma_position(h), "left")
         job.siting_x, job.siting_y = SITINGS[siting]
-        scale, bias = tensor_scale_bias(bpc, mean, std)
+        scale, bias = tensor_scale_bias(bpc, mean, std, jittered)
         for c in range(3):
             job.scale[c], job.bias[c] = float(scale[c]), float(bias[c])
         job.antialias = int(bool(antialias))
@@ -977,6 +1205,20 @@ def _on_device(a, device):
     t = torch.from_numpy(a).to(device)
     torch.cuda.synchronize(device)
     return t
+
+
+def _picture_jitter(jitter, grayscale, who):
+    """(jitter, grayscale) of one picture or stream, checked (ValueError naming `who`), or None when it has neither"""
+    if not _is_flag(grayscale):
+        raise ValueError("%s: grayscale must be a bool, not %r" % (who, grayscale))
+    if jitter is None and not grayscale:
+        return None
+    if jitter is not None:
+        try:
+            jitter_factors(jitter)
+        except ValueError as e:
+            raise ValueError("%s: %s" % (who, e)) from None
+    return jitter, bool(grayscale)
 
 
 def _picture_box(box, info, who):

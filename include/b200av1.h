@@ -649,7 +649,7 @@ B200_API int b200_frame_run_batch(const B200FrameJob *const *jobs, int n_jobs, v
 /* sizeof() of the ABI structs as compiled into the library (binding self-check): 0 McFrame, 1 McBlock, 2 CompBlock,
  * 3 BlendBlock, 4 WarpBlock, 5 ItxBlock, 6 LfFrame, 7 CdefFrame, 8 LrFrame, 9 FrameJob, 10 Av1Filter, 11 Av1Restoration,
  * 12 FgFrame, 13 FilmGrainData, 14 IntraTx, 15 IntraFrame, 16 McScaledBlock, 17 CoefBlock, 18 IntraSb, 19 CompFusedBlock,
- * 20 FrameBand, 21 ResizeFrame, 22 ExportJob, 23 TensorJob, 24 ToneMap */
+ * 20 FrameBand, 21 ResizeFrame, 22 ExportJob, 23 TensorJob, 24 ToneMap, 25 ColorJitter */
 B200_API int b200_struct_size(int which);
 
 /* ==== band-sliced frame job + cross-GPU reference exchange (SURVEY.md §8e) ===================== */
@@ -930,6 +930,60 @@ typedef struct B200ToneMap {
  * stay valid until the launch has completed. */
 #define B200_TENSOR_TONE_BATCH_MAX 16
 B200_API int b200_export_tensor_tone_batch(const B200TensorJob *jobs, const B200ToneMap *const *tones, int n, void *stream);
+
+/* ==== colour jitter and grayscale in the tensor export ========================================= */
+/* An optional stage of the tensor export after the matrix and the tone map and before the output rule, on the resized
+ * signal: torchvision's ColorJitter (and RandomGrayscale), written as the float32 operations of its v1 tensor path
+ * (torchvision/transforms/_functional_tensor.py), each rounded to nearest on its own (never fused). Input, per channel:
+ *   x_c = R_c * unit       R_c the matrix's result (T_c when the job is tone-mapped), unit = the float32 nearest to
+ *                          1 / (4 * bdmax), so x_c is in [0, 1]
+ * Operations: for k = 0 .. 3, op = order[k] (torchvision's numbering: 0 brightness, 1 contrast, 2 saturation, 3 hue) is
+ * applied when bit op of `enabled` is set (a clear bit is torchvision's None; a set bit applies the op even at a neutral
+ * factor, as torchvision does, and hue 0 is not an exact identity). With f32 constants and clip(v) = min(max(v, 0), 1):
+ *   gray(x)      = ((0.2989 * x_0) + (0.587 * x_1)) + (0.114 * x_2)
+ *   brightness:  x_c = clip(b * x_c)
+ *   saturation:  x_c = clip((s * x_c) + (s1 * gray(x)))
+ *   contrast:    x_c = clip((c * x_c) + (c1 * M)), M below
+ *   hue:         _rgb2hsv:  maxc = max(x_0, x_1, x_2), minc = min(...), eqc = maxc == minc, cr = maxc - minc
+ *                           s' = cr / (eqc ? 1 : maxc), cr_divisor = eqc ? 1 : cr
+ *                           rc = (maxc - x_0) / cr_divisor, gc = (maxc - x_1) / cr_divisor, bc = (maxc - x_2) / cr_divisor
+ *                           h = maxc == x_0 ? bc - gc : maxc == x_1 ? (2 + rc) - bc : (4 + gc) - rc
+ *                           h = fmod((h / 6) + 1, 1)                     (exact: the sum is in [5/6, 11/6])
+ *                h = torch.remainder(h + hue, 1): m = fmod(h + hue, 1), then m + 1 where m < 0 (that sum rounded)
+ *                _hsv2rgb:  i = floor(h * 6), f = (h * 6) - i, v = maxc
+ *                           p = clip(v * (1 - s')), q = clip(v * (1 - (s' * f))), t = clip(v * (1 - (s' * (1 - f))))
+ *                           by i % 6 = 0 .. 5, (x_0, x_1, x_2) = (v, t, p), (q, v, p), (p, v, t), (p, q, v), (t, p, v), (v, p, q)
+ *   grayscale = 1: after the operations, x_c = gray(x) on all three channels (RandomGrayscale with 3 output channels)
+ *   Output: out = (J_c * scale[c]) + bias[c], the rule above with J_c = the stage's result in place of R_c; the Python
+ *     binding passes scale = f32(1 / std), bias = f32(-mean / std) for jittered jobs, J being in [0, 1] already.
+ * The library is built with -ftz: every float32 operand or result of the stage that is subnormal counts as a zero of the
+ * same sign (only tiny factors lead there; stream.jitter_reference does the same).
+ * Factors: b, c, s, hue are the float32 of torchvision's factors; c1 and s1 are f32(1 - c) and f32(1 - s) with 1 - c
+ * computed in float64, as Python computes 1.0 - ratio before torch rounds it. The caller computes all of them.
+ * Contrast mean: M is the mean, over the out_w x out_h output picture, of gray of the values the operations before
+ * contrast produce (torchvision's mean over dims -3, -2, -1: per picture, also inside a clip), exact and deterministic:
+ *   S = sum of rint(gray * 2^24) as a uint64,   M = f32(f64(S) / (f64(out_w * out_h) * 2^24))
+ * It differs from torch's float32 mean only by rounding. A job with contrast enabled takes a contrast pass before its
+ * export, on the same stream: S is zeroed at `acc`, then one launch of the export's own sampling code sums it. */
+typedef struct B200ColorJitter {
+    float brightness, contrast, saturation, hue;   /* b, c, s >= 0, hue in [-0.5, 0.5], all finite */
+    float contrast1, saturation1;                  /* c1, s1: finite */
+    int32_t order[4];              /* a permutation of 0 .. 3 */
+    int32_t enabled;               /* bit op set: op applied; bits 0 .. 3 only */
+    int32_t grayscale;             /* 0 or 1 */
+    uint64_t *acc;                 /* device scratch for S, 8-byte aligned: required with contrast enabled */
+} B200ColorJitter;
+/* b200_export_tensor_tone_batch with an optional colour jitter per job: jitters = NULL, or jitters[i] = NULL, exports job i
+ * exactly as b200_export_tensor_tone_batch does (that function is the jitters = NULL case). A jittered job may have a tone
+ * map too (tones[i]), applied first. Jittered jobs take launches of their own, grouped like the others, of at most
+ * B200_TENSOR_JITTER_BATCH_MAX jobs (a job, a tone map and a jitter ride in the parameter block), each behind a contrast
+ * pass when one of them has contrast enabled. -2 with nothing launched for what b200_export_tensor_tone_batch rejects and
+ * for a bad jitter: a factor that is not finite, a negative brightness, contrast or saturation, a hue outside
+ * [-0.5, 0.5], an order that is not a permutation, enabled bits above bit 3, grayscale outside 0 .. 1, or contrast enabled
+ * with a NULL or misaligned acc. Each job needs an acc of its own, valid until the launch has completed. */
+#define B200_TENSOR_JITTER_BATCH_MAX 14
+B200_API int b200_export_tensor_jitter_batch(const B200TensorJob *jobs, const B200ToneMap *const *tones,
+                                             const B200ColorJitter *const *jitters, int n, void *stream);
 
 #ifdef __cplusplus
 }

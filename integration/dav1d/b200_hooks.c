@@ -89,13 +89,13 @@ API int b200hook_set_backend(const char *path)
     SYM(event_record, "b200_event_record"); SYM(stream_wait_event, "b200_stream_wait_event");
     SYM(struct_size, "b200_struct_size");
     SYM(event_sync, "b200_event_sync"); SYM(export_picture, "b200_export_picture");
-    SYM(export_tensor_tone_batch, "b200_export_tensor_tone_batch");
+    SYM(export_tensor_jitter_batch, "b200_export_tensor_jitter_batch");
 #undef SYM
     /* binding self-check: the structs this file was compiled with are the ones the library was compiled with */
     if (be.struct_size(9) != (int)sizeof(B200FrameJob) || be.struct_size(14) != (int)sizeof(B200IntraTx) ||
         be.struct_size(10) != (int)sizeof(B200Av1Filter) || be.struct_size(11) != (int)sizeof(B200Av1Restoration) ||
         be.struct_size(22) != (int)sizeof(B200ExportJob) || be.struct_size(23) != (int)sizeof(B200TensorJob) ||
-        be.struct_size(24) != (int)sizeof(B200ToneMap)) {
+        be.struct_size(24) != (int)sizeof(B200ToneMap) || be.struct_size(25) != (int)sizeof(B200ColorJitter)) {
         fprintf(stderr, "b200hook: ABI struct size mismatch with %s\n", path);
         dlclose(h);
         return -1;
@@ -352,7 +352,7 @@ void b200hook_refpic_forget(const void *const key)
 }
 
 int b200hook_export_submit(HookRefPic *const *const r, const int n, const int tensor, const void *const jobs,
-                           const B200ToneMap *const *const tones, void *const stream)
+                           const B200ToneMap *const *const tones, const B200ColorJitter *const *const jitters, void *const stream)
 {
     const B200Backend *const be = b200hook_backend();
     if (!be) return -1;
@@ -370,7 +370,7 @@ int b200hook_export_submit(HookRefPic *const *const r, const int n, const int te
         for (int k = 0; k < i && !seen; k++) seen = r[k]->event == r[i]->event;
         if (r[i]->event && !seen) rc = be->stream_wait_event(stream, r[i]->event);
     }
-    if (!rc) rc = tensor ? be->export_tensor_tone_batch(jobs, tones, n, stream) : be->export_picture(jobs, stream);
+    if (!rc) rc = tensor ? be->export_tensor_jitter_batch(jobs, tones, jitters, n, stream) : be->export_picture(jobs, stream);
     /* a batch that failed part way may have enqueued launches that still read the pictures: they complete here, because no
      * export-done event is recorded for them */
     if (rc) be->frame_wait(stream);
@@ -426,10 +426,12 @@ HookRefPic *b200hook_tensor_source_16bpc(const Dav1dPicture *p, const int32_t *b
  * must be even on a chroma-subsampled axis (include/b200av1.h): else -1 and nothing is launched. The stream waits once for
  * each picture's job, and every picture's export-done event is recorded behind the launch, so each entry keeps its device
  * buffer until its export has completed. With `tones` (NULL: none) picture i is tone-mapped by tones[i] when that is not
- * NULL (include/b200av1.h b200_export_tensor_tone_batch); the tables must outlive the export. */
-API int b200hook_export_tensor_tone_batch(const Dav1dPicture *const *const pics, const B200TensorJob *const tmpls,
-                                          const int32_t *const boxes, const B200ToneMap *const *const tones, const int n,
-                                          void *const stream)
+ * NULL (include/b200av1.h b200_export_tensor_tone_batch); the tables must outlive the export. With `jitters` (NULL: none)
+ * picture i is colour-jittered by jitters[i] when that is not NULL (b200_export_tensor_jitter_batch); each jitter's acc
+ * must outlive the export. */
+API int b200hook_export_tensor_jitter_batch(const Dav1dPicture *const *const pics, const B200TensorJob *const tmpls,
+                                            const int32_t *const boxes, const B200ToneMap *const *const tones,
+                                            const B200ColorJitter *const *const jitters, const int n, void *const stream)
 {
     if (!pics || !tmpls || n < 1) return -1;
     B200TensorJob *const jobs = malloc((size_t)n * sizeof(*jobs));
@@ -443,9 +445,15 @@ API int b200hook_export_tensor_tone_batch(const Dav1dPicture *const *const pics,
         refs[i] = p->p.bpc > 8 ? b200hook_tensor_source_16bpc(p, box, &jobs[i]) : b200hook_tensor_source_8bpc(p, box, &jobs[i]);
         if (!refs[i]) rc = -1;
     }
-    if (!rc) rc = b200hook_export_submit(refs, n, 1, jobs, tones, stream);
+    if (!rc) rc = b200hook_export_submit(refs, n, 1, jobs, tones, jitters, stream);
     free(jobs); free(refs);
     return rc;
+}
+API int b200hook_export_tensor_tone_batch(const Dav1dPicture *const *const pics, const B200TensorJob *const tmpls,
+                                          const int32_t *const boxes, const B200ToneMap *const *const tones, const int n,
+                                          void *const stream)
+{
+    return b200hook_export_tensor_jitter_batch(pics, tmpls, boxes, tones, NULL, n, stream);
 }
 API int b200hook_export_tensor_batch(const Dav1dPicture *const *const pics, const B200TensorJob *const tmpls,
                                      const int32_t *const boxes, const int n, void *const stream)

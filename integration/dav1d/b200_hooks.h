@@ -36,7 +36,7 @@ typedef struct B200Backend {
     int (*struct_size)(int);
     int (*event_sync)(void *);
     int (*export_picture)(const B200ExportJob *, void *);
-    int (*export_tensor_tone_batch)(const B200TensorJob *, const B200ToneMap *const *, int, void *);
+    int (*export_tensor_jitter_batch)(const B200TensorJob *, const B200ToneMap *const *, const B200ColorJitter *const *, int, void *);
 } B200Backend;
 const B200Backend *b200hook_backend(void);   /* NULL (after logging) when no back end is loaded: the decode fails */
 
@@ -141,8 +141,10 @@ typedef struct HookRefPic { const void *key; void *dev; size_t bytes; int ready,
 HookRefPic *b200hook_refpic(const void *key, size_t bytes, int create);
 /* enqueues the export of n resident pictures r[0..n) on `stream` behind their own jobs (one wait per distinct job), and
  * records each entry's export-done event behind it: `jobs` is one B200ExportJob (b200_export_picture, n = 1) or, with
- * `tensor` set, n B200TensorJobs and their tone maps `tones` (NULL: none; one b200_export_tensor_tone_batch call) */
-int b200hook_export_submit(HookRefPic *const *r, int n, int tensor, const void *jobs, const B200ToneMap *const *tones, void *stream);
+ * `tensor` set, n B200TensorJobs, their tone maps `tones` and their colour jitters `jitters` (each NULL: none; one
+ * b200_export_tensor_jitter_batch call) */
+int b200hook_export_submit(HookRefPic *const *r, int n, int tensor, const void *jobs, const B200ToneMap *const *tones,
+                           const B200ColorJitter *const *jitters, void *stream);
 /* a decoder context (Dav1dContext *) opened for device output: its frame jobs and film grain leave the pictures in device
  * memory and copy nothing back into the host pictures */
 int b200hook_device_only(const void *ctx);

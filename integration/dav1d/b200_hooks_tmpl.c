@@ -1265,7 +1265,7 @@ int bitfn(b200hook_export_picture)(const Dav1dPicture *const p, const B200Export
     if (!r) return -1;
     B200ExportJob j = *tmpl;
     EXPORT_SOURCE(j, r, g, p);
-    return b200hook_export_submit(&r, 1, 0, &j, NULL, stream);
+    return b200hook_export_submit(&r, 1, 0, &j, NULL, NULL, stream);
 }
 /* fills the source fields of tensor job *j from the picture's device copy: that entry, NULL when it has none or when `box`
  * (top, left, height, width, or NULL for the whole picture) is not a box of the picture whose chroma keeps its siting

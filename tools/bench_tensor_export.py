@@ -1,7 +1,8 @@
 """The tensor export (b200_export_tensor) against the torch chain it replaces (run on a GPU machine):
 
     python tools/bench_tensor_export.py [--launches 200] [--rounds 5] [--reps 3] [--antialias] [--crop-flip] [--kernel-only]
-                                        [--interpolation bilinear | bicubic] [--tonemap] [--baseline-lib SO] [--out FILE]
+                                        [--interpolation bilinear | bicubic] [--tonemap] [--jitter] [--baseline-lib SO]
+                                        [--out FILE]
 
 Kernel level, one JSON line per configuration, on synthetic device pictures (random planes, 4:2:0):
   fused        one b200_export_tensor launch
@@ -29,6 +30,12 @@ Decoder level, one JSON line per stream workload of bench.py: pictures per secon
 --tonemap: the kernel level only, on TONEMAP_CONFIGS: 10-bit BT.2020 PQ or HLG pictures tone-mapped to SDR BT.709
   (b200_export_tensor_tone_batch, one job with the tables of stream.tone_tables) against the chain with the same
   definition: the RGB export, .float(), the curve gather, the 3 x 3 matrix, clamp, the OETF gather, interpolate,
+  (x - mean) / std, .to(dtype).
+--jitter: the kernel level only, on JITTER_CONFIGS: colour jitter (B200ColorJitter: brightness, contrast, saturation and
+  hue, contrast taking its pass over the picture) and grayscale fused into an antialiased export, one b200_export_tensor_jitter_batch call
+  for all pictures, against the same export without jitter (`fused_no_jitter`: what the jitter stage and the contrast
+  pass cost) and the torch chain: the RGB export, .float() / bdmax, the crop, interpolate(antialias=True),
+  torchvision.transforms.v2.functional's adjust_* in the same order, rgb_to_grayscale(num_output_channels=3), the flip,
   (x - mean) / std, .to(dtype).
 --baseline-lib SO: the kernel level times the same jobs (flip = 0) through another build of the library (an earlier
   commit's libb200av1.so) instead of the torch chain, alternated with this tree's, as `fused_baseline`.
@@ -97,6 +104,28 @@ TONEMAP_CONFIGS = [  # AA_CONFIGS' fields, no box, then (transfer, antialias, in
 ]
 
 
+JITTER = ([1, 0, 3, 2], 1.2, 0.8, 1.3, 0.05)    # ColorJitter.get_params-style: contrast first, every op on
+JITTER_CONFIGS = [  # AA_CONFIGS' fields, the box, no tone map
+    ("jitter 4k10 -> 224x224 bf16 chw, aa", 3840, 2160, 10, (224, 224), "bfloat16", "chw", 1, None, None),
+    ("jitter crop+flip 1080p8 -> 224x224 bf16 chw, aa", 1920, 1080, 8, (224, 224), "bfloat16", "chw", 1, (100, 372, 882, 1176), None),
+    ("jitter 8 x 16-frame clips 1080p8 -> 224x224 bf16 chw, aa, one batch call", 1920, 1080, 8, (224, 224), "bfloat16", "chw", 128,
+     None, None),
+]
+
+
+def jitter_chain(x, bdmax, size, dtype, mean, std, flip):
+    """the jittered export in torch: x / bdmax -> interpolate(antialias) -> v2 adjust_* in JITTER's order -> grayscale ->
+    normalise"""
+    from torchvision.transforms.v2 import functional as TF
+    x = F.interpolate((x.float() / bdmax)[None], size=size, mode="bilinear", align_corners=False, antialias=True)[0]
+    ops = [TF.adjust_brightness, TF.adjust_contrast, TF.adjust_saturation, TF.adjust_hue]
+    for op in JITTER[0]:
+        x = ops[op](x, JITTER[1 + op])
+    x = TF.rgb_to_grayscale(x, num_output_channels=3)
+    x = x.flip(-1) if flip else x
+    return ((x - mean) / std).to(getattr(torch, dtype))
+
+
 def tone_chain(rgb, bdmax, tables, size, dtype, mean, std, antialias, mode):
     """the tone-mapped export in torch: R, G, B at the stream's bit depth -> curve -> matrix -> clamp -> OETF -> resize"""
     curve, m, oetf = tables
@@ -158,13 +187,13 @@ def kernel_level(args):
     s = torch.cuda.Stream()
     lines = []
     bicubic = args.interpolation == "bicubic"
-    configs = TONEMAP_CONFIGS if args.tonemap else CROP_FLIP_CONFIGS if args.crop_flip else BICUBIC_CONFIGS if bicubic else \
+    configs = JITTER_CONFIGS if args.jitter else TONEMAP_CONFIGS if args.tonemap else CROP_FLIP_CONFIGS if args.crop_flip else BICUBIC_CONFIGS if bicubic else \
         AA_CONFIGS if args.antialias else [c + (1,) for c in CONFIGS] + [BATCH_CONFIG]
     base = baseline_lib(args.baseline_lib) if args.baseline_lib else None
     for name, w, h, bpc, size, dtype, layout, pics, *extra in configs:
         box = extra[0] if extra else None
         tone = extra[1] if len(extra) > 1 else None
-        antialias = tone[1] if tone else args.antialias or box is not None
+        antialias = tone[1] if tone else args.antialias or args.jitter or box is not None
         interpolation = tone[2] if tone else args.interpolation
         rng = np.random.default_rng(w + bpc)
         bdmax, sb = (1 << bpc) - 1, 1 if bpc == 8 else 2
@@ -202,12 +231,21 @@ def kernel_level(args):
             for k in (1, 2):
                 tj.plane_off[k] += (top >> 1) * tj.stride[k] + (left >> 1)
             tj.flip = 1
-        if pics > 1:                             # the same picture into pics slots, one call
+        if pics > 1 or args.jitter:              # the same picture into pics slots, one call
             out = torch.empty((pics,) + shape, dtype=getattr(torch, dtype), device="cuda")
             tjs = (stream.TensorJob * pics)()
             for k in range(pics):
                 tjs[k] = stream.TensorJob.from_buffer_copy(tj)
                 tjs[k].dst = out[k].data_ptr()
+        if args.jitter:                          # J in [0, 1]: scale 1 / std; one acc per picture
+            jscale, jbias = stream.tensor_scale_bias(bpc, MEAN, STD, jittered=True)
+            jjobs = (stream.TensorJob * pics).from_buffer_copy(tjs)
+            for k in range(pics):
+                for c in range(3):
+                    jjobs[k].scale[c], jjobs[k].bias[c] = float(jscale[c]), float(jbias[c])
+            acc = torch.zeros(pics, dtype=torch.int64, device="cuda")
+            jts = [stream.color_jitter(JITTER, True, acc=acc.data_ptr() + 8 * k) for k in range(pics)]
+            jits = (C.POINTER(stream.ColorJitter) * pics)(*[C.pointer(t) for t in jts])
         rgb = torch.empty((3, h, w), dtype=torch.uint8 if bpc == 8 else torch.int16, device="cuda")
         ej = stream.ExportJob()
         ej.src, ej.format = src.data_ptr(), 1
@@ -221,7 +259,9 @@ def kernel_level(args):
         sp = C.c_void_p(s.cuda_stream)
 
         def fused():
-            if tone:
+            if args.jitter:
+                lib.check(lib.b200_export_tensor_jitter_batch(jjobs, None, jits, pics, sp), "b200_export_tensor_jitter_batch")
+            elif tone:
                 lib.check(lib.b200_export_tensor_tone_batch(C.byref(tj), tones, 1, sp), "b200_export_tensor_tone_batch")
             elif pics > 1:
                 lib.check(lib.b200_export_tensor_batch(tjs, pics, sp), "b200_export_tensor_batch")
@@ -232,12 +272,16 @@ def kernel_level(args):
             for _ in range(pics):
                 lib.check(lib.b200_export_picture(C.byref(ej), sp), "b200_export_picture")
                 x = rgb if box is None else rgb[:, box[0]:box[0] + box[2], box[1]:box[1] + box[3]]
-                if tone:
+                if args.jitter:
+                    jitter_chain(x, bdmax, size, dtype, mean, std, box is not None)
+                elif tone:
                     tone_chain(x, bdmax, d_tables, size, dtype, mean, std, antialias, interpolation)
                 else:
                     torch_chain(x, bdmax, size, dtype, layout, mean, std, antialias, box is not None, interpolation)
 
         arms = {"fused": fused}
+        if args.jitter:
+            arms["fused_no_jitter"] = lambda: lib.check(lib.b200_export_tensor_batch(tjs, pics, sp), "b200_export_tensor_batch")
         if base is not None:                     # the same jobs in the other build's struct layout
             bsz = base.b200_struct_size(23)
             packed = (C.c_char * (bsz * pics))()
@@ -270,7 +314,7 @@ def kernel_level(args):
         sw, sh = (box[3], box[2]) if box else (w, h)
         fused_bytes = pics * (sw * sh * 3 // 2 * sb + 3 * oh * ow * ESIZE[dtype])
         line = {"config": name, "gpu": gpu_info(), "launches_per_round": args.launches, "rounds": args.rounds, "us": {}, "bytes": {
-            "fused": fused_bytes, "fused_baseline": fused_bytes, "torch_chain": pics * chain_bytes(w, h, sb, size, dtype, layout, box, bool(tone))},
+            "fused": fused_bytes, "fused_baseline": fused_bytes, "fused_no_jitter": fused_bytes, "torch_chain": pics * chain_bytes(w, h, sb, size, dtype, layout, box, bool(tone))},
             "GBps": {}, "share_of_3.35TBps": {}}
         line["bytes"] = {k: v for k, v in line["bytes"].items() if k in times}
         if antialias:
@@ -281,6 +325,8 @@ def kernel_level(args):
             line["tonemap"] = {"transfer": tone[0], "primaries": "bt2020", "peak": 1000.0, "sdr_peak": 203.0}
         if box is not None:
             line["crop_box"], line["flip"] = list(box), True
+        if args.jitter:
+            line["jitter"] = {"fn_idx": JITTER[0], "factors": list(JITTER[1:]), "grayscale": True}
         if base is not None:
             line["baseline_lib"] = args.baseline_lib
         for key, v in times.items():
@@ -356,14 +402,15 @@ def main():
     ap.add_argument("--crop-flip", action="store_true")
     ap.add_argument("--interpolation", choices=list(stream.TENSOR_INTERPOLATIONS), default="bilinear")
     ap.add_argument("--tonemap", action="store_true")
+    ap.add_argument("--jitter", action="store_true")
     ap.add_argument("--baseline-lib", help="another build of libb200av1.so: time its export of the same jobs instead of the chain")
     ap.add_argument("--kernel-only", action="store_true")
     ap.add_argument("--out")
     args = ap.parse_args()
-    if args.baseline_lib and (args.interpolation != "bilinear" or args.tonemap):
+    if args.baseline_lib and (args.interpolation != "bilinear" or args.tonemap or args.jitter):
         ap.error("--baseline-lib compares the bilinear and triangle exports, which an earlier library also has")
     assert torch.cuda.is_available(), "needs a CUDA device"
-    kernel_only = args.antialias or args.crop_flip or args.tonemap or args.kernel_only or args.interpolation != "bilinear"
+    kernel_only = args.antialias or args.crop_flip or args.tonemap or args.jitter or args.kernel_only or args.interpolation != "bilinear"
     lines = kernel_level(args) + ([] if kernel_only else decoder_level(args))
     if args.out:
         with open(args.out, "w") as fh:

@@ -23,9 +23,10 @@ void *b200_event_create(void) { return (void *)1; }
 void b200_event_destroy(void *e) { (void)e; }
 int b200_event_record(void *e, void *s) { (void)e; (void)s; return 0; }
 int b200_stream_wait_event(void *s, void *e) { (void)s; (void)e; return 0; }
-int b200_struct_size(int w) { switch (w) { case 9: return sizeof(B200FrameJob); case 14: return sizeof(B200IntraTx); case 10: return sizeof(B200Av1Filter); case 11: return sizeof(B200Av1Restoration); case 22: return sizeof(B200ExportJob); case 23: return sizeof(B200TensorJob); case 24: return sizeof(B200ToneMap); } return -1; }
+int b200_struct_size(int w) { switch (w) { case 9: return sizeof(B200FrameJob); case 14: return sizeof(B200IntraTx); case 10: return sizeof(B200Av1Filter); case 11: return sizeof(B200Av1Restoration); case 22: return sizeof(B200ExportJob); case 23: return sizeof(B200TensorJob); case 24: return sizeof(B200ToneMap); case 25: return sizeof(B200ColorJitter); } return -1; }
 int b200_event_sync(void *e) { (void)e; return 0; }
 int b200_export_picture(const B200ExportJob *j, void *s) { (void)j; (void)s; return 0; }
 int b200_export_tensor(const B200TensorJob *j, void *s) { (void)j; (void)s; return 0; }
 int b200_export_tensor_batch(const B200TensorJob *j, int n, void *s) { (void)j; (void)n; (void)s; return 0; }
 int b200_export_tensor_tone_batch(const B200TensorJob *j, const B200ToneMap *const *t, int n, void *s) { (void)j; (void)t; (void)n; (void)s; return 0; }
+int b200_export_tensor_jitter_batch(const B200TensorJob *j, const B200ToneMap *const *t, const B200ColorJitter *const *c, int n, void *s) { (void)j; (void)t; (void)c; (void)n; (void)s; return 0; }
